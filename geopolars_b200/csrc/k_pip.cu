@@ -1303,6 +1303,13 @@ __device__ __forceinline__ bool bucket_walk(const IndexView &ix, int32_t e0, int
                 if (HOLES) ring[j] = __ldg(ix.entry_ring + k + j);
             }
         }
+        // padding records belong to the last listed ring: with the ring of the previous batch, a batch that switches ring
+        // and ends in padding would close the ring early and restart the exterior with a winding number of 0
+        if (HOLES) {
+#pragma unroll
+            for (int j = 1; j < 4; ++j)
+                if (k + j >= e1) ring[j] = ring[j - 1];
+        }
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             if (HOLES) {

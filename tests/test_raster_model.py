@@ -8,7 +8,8 @@ parts the scanline fill claimed for the cell and strictly outside all others —
 is answering geo's `Polygon::contains`.  The GPU tests compare the CUDA implementation with the oracle; this file checks
 the ARGUMENT (DESIGN.md 4.2 "Exactness of the raster") on shapes chosen to stress it: spiky stars, nearly horizontal and
 exactly horizontal / vertical edges, vertices on cell lines, a hole, overlapping parts, rows with more crossings than the
-per-row list holds."""
+per-row list holds.  It also packs the codes into raster words and decodes them as the streaming kernel does, for fine rasters
+(one coarse cell per word) and coarse ones (rs < 4: a word spans several coarse cells; odd G: a partly used last word)."""
 import math
 
 import numpy as np
@@ -30,8 +31,15 @@ def fine_index(v, lo, inv, n):
     return min(max(d2i_rd((v - lo) * inv), 0), n - 1)
 
 
+CAND_IN_CELLS = 0xFFFFFFFE  # ph_raster_cand: the word spans several coarse cells, stage 2 asks cand01
+
+
 class RasterModel:
-    """polys: list of parts, a part = list of closed rings (ring 0 = exterior), a ring = list of (x, y) doubles"""
+    """polys: list of parts, a part = list of closed rings (ring 0 = exterior), a ring = list of (x, y) doubles.
+
+    Besides the mark / claim sets, the model keeps the packed raster the build writes: 16 cells of 2 bits per 32-bit word
+    (raster_or_span's masks, every write an OR), the coarse cells' ascending candidate lists (ph_cells), cand01
+    (ph_cell_finish) and the candidate row beside each word (ph_raster_cand); `decode` is stage 2 of k_pip_stream."""
 
     def __init__(self, polys, G, rs):
         self.polys = polys
@@ -40,22 +48,68 @@ class RasterModel:
         self.x1 = max(c[0] for r in ext for c in r)
         self.y0 = min(c[1] for r in ext for c in r)
         self.y1 = max(c[1] for r in ext for c in r)
+        self.G, self.rs = G, rs
         self.fg = G << rs
+        self.wpr = (self.fg + 15) >> 4
         self.inv_fw = self.fg / (self.x1 - self.x0)
         self.inv_fh = self.fg / (self.y1 - self.y0)
         self.marked = np.zeros((self.fg, self.fg), dtype=bool)
         self.claims = {}  # (fy, fx) -> set of parts whose fill covered the cell
+        self.words = [[0] * self.wpr for _ in range(self.fg)]
+        self.items = [[] for _ in range(G * G)]  # coarse cell -> ascending part ids whose exterior bbox overlaps it
+        for p, rings in enumerate(polys):
+            xs, ys = [c[0] for c in rings[0]], [c[1] for c in rings[0]]
+            cx0, cx1 = fine_index(min(xs), self.x0, self.inv_fw, self.fg) >> rs, fine_index(max(xs), self.x0, self.inv_fw, self.fg) >> rs
+            cy0, cy1 = fine_index(min(ys), self.y0, self.inv_fh, self.fg) >> rs, fine_index(max(ys), self.y0, self.inv_fh, self.fg) >> rs
+            for cy in range(cy0, cy1 + 1):
+                for cx in range(cx0, cx1 + 1):
+                    self.items[cy * G + cx].append(p)
+        self.cand01 = [(it[0] if it else -1, it[1] if len(it) > 1 else -1) for it in self.items]
         for p, rings in enumerate(polys):
             self._part(p, rings)
+        # ph_raster_cand: the row of candidate #0 beside the codes when a word lies inside one coarse cell
+        self.word_cand = [[self.cand01[(fy >> rs) * G + ((wx << 4) >> rs)][0] & 0xFFFFFFFF if rs >= 4 else CAND_IN_CELLS
+                           for wx in range(self.wpr)] for fy in range(self.fg)]
 
     # -- query side -------------------------------------------------------------------------------------------------
     def cell_of(self, x, y):
         return fine_index(y, self.y0, self.inv_fh, self.fg), fine_index(x, self.x0, self.inv_fw, self.fg)
 
+    def code(self, fy, fx):
+        return (self.words[fy][fx >> 4] >> ((fx & 15) * 2)) & 3
+
+    def decode(self, fy, fx):
+        """stage 2 of k_pip_stream for a point in fine cell (fy, fx): the row it answers, -1, or None (code 3: walk)"""
+        code = self.code(fy, fx)
+        if code == 0:
+            return -1
+        if code == 3:
+            return None
+        cc = (fy >> self.rs) * self.G + (fx >> self.rs)
+        y = self.word_cand[fy][fx >> 4]
+        if code == 1 and y != CAND_IN_CELLS:
+            return y - (1 << 32) if y >= 1 << 31 else y
+        return self.cand01[cc][0] if code == 1 else self.cand01[cc][1]
+
     # -- build side -------------------------------------------------------------------------------------------------
+    def _raster_or_span(self, fy, c0, c1, code):
+        row, rep = self.words[fy], (code * 0x55555555) & 0xFFFFFFFF
+        for w in range(c0 >> 4, (c1 >> 4) + 1):
+            lo, hi = max(c0 - (w << 4), 0), min(c1 - (w << 4), 15)
+            m = (0xFFFFFFFF >> (2 * (15 - hi))) & ((0xFFFFFFFF << (2 * lo)) & 0xFFFFFFFF)
+            row[w] |= rep & m
+
+    def _fill_span(self, fy, lo, hi, p):  # raster_fill_span + raster_rank_code
+        for cc in range(lo >> self.rs, (hi >> self.rs) + 1):
+            x0, x1 = max(lo, cc << self.rs), min(hi, ((cc + 1) << self.rs) - 1)
+            it = self.items[(fy >> self.rs) * self.G + cc]
+            code = 1 if it[:1] == [p] else 2 if it[1:2] == [p] else 3
+            self._raster_or_span(fy, x0, x1, code)
+
     def _or_span(self, fy, c0, c1):
         if c0 <= c1:
             self.marked[fy, c0:c1 + 1] = True
+            self._raster_or_span(fy, c0, c1, 3)
 
     def _mark_row(self, r, tsx, tsy, tex, tey, inv_dy):
         eps = 1e-6
@@ -133,6 +187,7 @@ class RasterModel:
                     if wn_ext != 0 and not in_hole:
                         for fx in range(lo, hi + 1):
                             self.claims.setdefault((fy, fx), set()).add(p)
+                        self._fill_span(fy, lo, hi, p)
 
     # -- every double that maps to a cell, sampled: its extremes and a few interior values -----------------------------
     def _axis_samples(self, c, lo, inv):
@@ -191,6 +246,31 @@ class RasterModel:
                             if not want:  # an unmarked cell holds no boundary point either
                                 assert all(exact.ring_position((x, y), r) != 1 for r in rings)
         return checked, inside
+
+    def check_decode(self):
+        """the packed words against the mark / claim sets: every marked cell reads code 3; every other cell decodes (stage 2)
+        to the row its claim set gives (none -> -1, one part -> that part unless it ranks after #1 in its coarse cell, two or
+        more -> walk); cells past fgx in a row's last word stay 0.  Returns {code: cells} over the unmarked cells."""
+        census = {0: 0, 1: 0, 2: 0, 3: 0}
+        for fy in range(self.fg):
+            for fx in range(self.fg):
+                code = self.code(fy, fx)
+                if self.marked[fy, fx]:
+                    assert code == 3, f"marked cell ({fy},{fx}) reads code {code}"
+                    continue
+                census[code] += 1
+                claim = self.claims.get((fy, fx), set())
+                got = self.decode(fy, fx)
+                it = self.items[(fy >> self.rs) * self.G + (fx >> self.rs)]
+                if not claim:
+                    assert got == -1, (fy, fx, got)
+                elif len(claim) == 1 and next(iter(claim)) in it[:2]:
+                    assert got == next(iter(claim)), f"cell ({fy},{fx}) claimed by {claim} decodes to {got} (candidates {it[:2]})"
+                else:
+                    assert got is None, (fy, fx, claim, got)
+            for fx in range(self.fg, self.wpr * 16):
+                assert self.code(fy, fx) == 0
+        return census
 
 
 def star(rng, cx, cy, n, r0, r1):
@@ -276,3 +356,66 @@ def test_the_referee_has_teeth():
     RasterModel([[outer], [tri]], G=2, rs=4).check_unmarked_cells()  # the faithful model passes
     with pytest.raises(AssertionError):
         Forgetful([[outer], [tri]], G=2, rs=4).check_unmarked_cells()
+
+
+def _coarse_field(rng):
+    """overlapping spiky stars on a 4 x 4 lattice (bboxes overlap, so cells have second and third candidates), one of them
+    with a hole, and one large polygon over a corner of the lattice"""
+    polys = []
+    for j in range(4):
+        for i in range(4):
+            rings = [star(rng, 10.0 * i + 5.0 + rng.uniform(-1, 1), 10.0 * j + 5.0 + rng.uniform(-1, 1), 9, 2.5, 7.0)]
+            if (i, j) == (1, 2):
+                cx = sum(c[0] for c in rings[0][:-1]) / 9.0
+                cy = sum(c[1] for c in rings[0][:-1]) / 9.0
+                rings.append(star(rng, cx, cy, 5, 0.5, 1.0)[::-1])
+            polys.append(rings)
+    polys.append([star(rng, 28.0, 28.0, 7, 6.0, 11.0)])
+    return polys
+
+
+@pytest.mark.parametrize("rs,G", [(0, 15), (1, 13), (2, 9), (3, 5)])
+def test_coarse_rasters_decode_to_the_claimed_row(rs, G):
+    """rs < 4: a raster word spans several coarse cells, so the build stores 0xfffffffe beside the codes and stage 2 takes
+    candidate #0 from cand01 of the point's OWN coarse cell; G odd: the last word of each row is only partly used"""
+    m = RasterModel(_coarse_field(np.random.default_rng(40 + rs)), G=G, rs=rs)
+    assert m.fg % 16 != 0 and m.wpr * 16 > m.fg  # the partial last word is modelled
+    assert all(v == CAND_IN_CELLS for row in m.word_cand for v in row)
+    checked, inside = m.check_unmarked_cells()
+    assert checked > 20 and inside > 5, (checked, inside)
+    census = m.check_decode()
+    assert census[1] > 0 and census[0] > 0, census
+    # code-1 cells whose coarse cell is not the coarse cell of their word's first fine cell: only cand01 answers them right
+    foreign = sum(1 for fy in range(m.fg) for fx in range(m.fg)
+                  if not m.marked[fy, fx] and m.code(fy, fx) == 1 and (fx >> rs) != (((fx >> 4) << 4) >> rs))
+    assert foreign > 0
+    assert max(len(it) for it in m.items) >= 3
+
+
+def test_fine_raster_keeps_the_row_beside_the_codes():
+    """rs >= 4: every word lies inside one coarse cell and carries its candidate #0"""
+    m = RasterModel(_coarse_field(np.random.default_rng(44)), G=3, rs=4)
+    assert all(v != CAND_IN_CELLS for row in m.word_cand for v in row)
+    census = m.check_decode()
+    assert census[1] > 0 and census[2] >= 0
+
+
+def test_the_decode_referee_has_teeth():
+    """negative controls: the candidate row of a word's first coarse cell used for every cell of the word (the rs >= 4 guard
+    dropped), and a span mask one cell short at its upper end, must both be caught by check_decode"""
+
+    class NoGuard(RasterModel):
+        def __init__(self, polys, G, rs):
+            super().__init__(polys, G, rs)
+            self.word_cand = [[self.cand01[(fy >> rs) * G + ((wx << 4) >> rs)][0] & 0xFFFFFFFF for wx in range(self.wpr)]
+                              for fy in range(self.fg)]
+
+    class ShortMask(RasterModel):
+        def _raster_or_span(self, fy, c0, c1, code):
+            super()._raster_or_span(fy, c0, c1 - 1, code)
+
+    polys = _coarse_field(np.random.default_rng(42))
+    RasterModel(polys, G=9, rs=2).check_decode()
+    for bad in (NoGuard, ShortMask):
+        with pytest.raises(AssertionError):
+            bad(polys, G=9, rs=2).check_decode()
