@@ -43,6 +43,10 @@ pub struct GplArray {
 pub struct GplPairs {
     _p: [u8; 0],
 }
+#[repr(C)]
+pub struct GplNearestIndex {
+    _p: [u8; 0],
+}
 
 const GPL_HOST: c_int = 0;
 const GPL_ORIGIN_CENTROID: c_int = 0;
@@ -86,6 +90,9 @@ extern "C" {
     fn gpl_pairs_count(pairs: *const GplPairs) -> i64;
     fn gpl_pairs_copy(ctx: *mut GplCtx, pairs: *const GplPairs, lhs: *mut u64, rhs: *mut u64, mem: c_int) -> c_int;
     fn gpl_pairs_free(pairs: *mut GplPairs);
+    fn gpl_nearest_index_build(ctx: *mut GplCtx, rhs: *const GplArray, out: *mut *mut GplNearestIndex) -> c_int;
+    fn gpl_nearest_index_free(idx: *mut GplNearestIndex);
+    fn gpl_nearest_join_pairs_array(ctx: *mut GplCtx, idx: *const GplNearestIndex, points: *const GplArray, max_distance: f64, out: *mut *mut GplPairs, distance: *mut f64, mem: c_int) -> c_int;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -382,6 +389,10 @@ pub trait GeoSeriesB200Ext {
     /// the (lhs_index, rhs_index) pair list of `spatial_join(lhs, rhs, SpatialJoinArgs { predicate, .. })`
     /// (spatial_index.rs:139-157) for any two geometry columns; feed it to the DataFrame joins at :159-203
     fn spatial_join_pairs(&self, rhs: &Series, predicate: c_int) -> Result<(Vec<u64>, Vec<u64>)>;
+    /// nearest-geometry join of this Point column against any geometry column (GeoPandas' `sjoin_nearest`): every
+    /// right row at the minimum distance <= `max_distance` (inclusive, `f64::INFINITY` = unbounded), as (lhs_index,
+    /// rhs_index, distance) sorted by (lhs, rhs); the distance is exactly what `distance` computes for the pair
+    fn nearest_join_pairs(&self, rhs: &Series, max_distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
 }
 
 impl GeoSeriesB200Ext for Series {
@@ -418,5 +429,27 @@ impl GeoSeriesB200Ext for Series {
         unsafe { gpl_pairs_free(pairs) };
         check(rc)?;
         Ok((l, r))
+    }
+
+    fn nearest_join_pairs(&self, rhs: &Series, max_distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let mut idx = std::ptr::null_mut();
+        check(unsafe { gpl_nearest_index_build(ctx, b.0, &mut idx) })?;
+        let mut dist = vec![0f64; self.len()];
+        let mut pairs = std::ptr::null_mut();
+        let rc = unsafe { gpl_nearest_join_pairs_array(ctx, idx, a.0, max_distance, &mut pairs, dist.as_mut_ptr(), GPL_HOST) };
+        unsafe { gpl_nearest_index_free(idx) };
+        if rc != 0 && !pairs.is_null() {
+            unsafe { gpl_pairs_free(pairs) };
+        }
+        check(rc)?;
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r) = (vec![0u64; n], vec![0u64; n]);
+        let rc = if n > 0 { unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) } } else { 0 };
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
+        let d = l.iter().map(|&i| dist[i as usize]).collect();
+        Ok((l, r, d))
     }
 }

@@ -154,6 +154,12 @@ SIGNATURES = {
     "gpl_contains_join_pairs_array": (_INT, [_P, _P, _P, C.POINTER(_P)]),
     "gpl_contains_join_host": (_INT, [_P, _P, _P, _I64, _P, _I64]),
     "gpl_join_histogram": (_INT, [_P, _P, _I64, _P, _I64, _INT]),
+    "gpl_nearest_index_build": (_INT, [_P, _P, C.POINTER(_P)]),
+    "gpl_nearest_index_free": (None, [_P]),
+    "gpl_nearest_index_stats": (_INT, [_P, _P, _P]),
+    "gpl_nearest_join": (_INT, [_P, _P, _P, _I64, _D, _P, _P, _P, _INT]),
+    "gpl_nearest_join_array": (_INT, [_P, _P, _P, _D, _P, _P, _P, _INT]),
+    "gpl_nearest_join_pairs_array": (_INT, [_P, _P, _P, _D, C.POINTER(_P), _P, _INT]),
     "gpl_gen_uniform_points": (_INT, [_P, C.c_uint64, _I64, _I64, _D, _P]),
     "gpl_gen_walk_linestrings": (_INT, [_P, C.c_uint64, _I64, _I64, _I64, C.c_int32, _P, _P]),
     "gpl_gen_blob_polygons": (_INT, [_P, C.c_uint64, _I64, _I64, C.c_int32, _P, _P, _P]),

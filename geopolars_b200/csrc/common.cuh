@@ -127,6 +127,13 @@ struct gpl_array {
     int refcount = 1;
 };
 
+// result of a join (gpl_spatial_join, gpl_contains_join_pairs_array, gpl_nearest_join_pairs_array): (lhs, rhs) row pairs
+struct gpl_pairs {
+    gpl_ctx *ctx = nullptr;
+    uint64_t *lhs = nullptr, *rhs = nullptr;  // device
+    int64_t n = 0;
+};
+
 namespace gpl {
 
 gpl_array *array_new(gpl_ctx *ctx, int32_t type);

@@ -28,6 +28,8 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "join_grid.cuh"
+#include "point_dist.cuh"
 #include "scan.cuh"
 
 namespace gpl {
@@ -372,96 +374,8 @@ __global__ void __launch_bounds__(kPairWarps * 32) k_ls_ls_exact(int64_t n, cons
 }
 
 // ---- point vs linestring / polygon -------------------------------------------------------------
-// pt_dist / line_segment_distance: common.cuh
-// geo-types line_string_contains_point (epsilon based, inexact by design), warp cooperative
-__device__ __forceinline__ bool line_string_contains_point(const double2 *__restrict__ xy, int64_t c0, int64_t n, double2 p,
-                                                           int lane) {
-    if (n == 0) return false;
-    if (n == 1) {
-        float d = (float)pt_dist(xy[c0], p);
-        return d <= 1.1920929e-07f;
-    }
-    bool hit = false;
-    for (int64_t i = lane; i < n; i += 32) {
-        double2 q = xy[c0 + i];
-        if (q.x == p.x && q.y == p.y) hit = true;
-    }
-    for (int64_t i = lane; i < n - 1; i += 32) {
-        double2 s = xy[c0 + i], e = xy[c0 + i + 1];
-        double dx = e.x - s.x, dy = e.y - s.y;
-        bool hx = dx != 0.0, hy = dy != 0.0;
-        double tx = hx ? (p.x - s.x) / dx : 0.0;
-        double ty = hy ? (p.y - s.y) / dy : 0.0;
-        bool c;
-        if (!hx && !hy) c = (p.x == s.x && p.y == s.y);
-        else if (hx && !hy) c = (p.y == s.y && 0.0 <= tx && tx <= 1.0);
-        else if (!hx && hy) c = (p.x == s.x && 0.0 <= ty && ty <= 1.0);
-        else c = (fabs(tx - ty) <= 2.220446049250313e-16 && 0.0 <= tx && tx <= 1.0);
-        hit = hit || c;
-    }
-    return __any_sync(0xffffffffu, hit);
-}
-__device__ __forceinline__ double point_ls_distance(const double2 *__restrict__ xy, int64_t c0, int64_t n, double2 p, int lane) {
-    if (n == 0 || line_string_contains_point(xy, c0, n, p, lane)) return 0.0;
-    double best = 1.7976931348623157e308;
-    for (int64_t i = lane; i < n - 1; i += 32) best = fmin(best, line_segment_distance(p, xy[c0 + i], xy[c0 + i + 1]));
-    return warp_min(best);
-}
-
-// coord_pos_relative_to_ring, warp cooperative: 0 outside, 1 boundary, 2 inside
-__device__ __forceinline__ int ring_position(const double2 *__restrict__ xy, int64_t c0, int64_t n, double2 p, int lane) {
-    if (n == 0) return 0;
-    if (n == 1) {
-        double2 q = xy[c0];
-        return (q.x == p.x && q.y == p.y) ? 1 : 0;
-    }
-    double2 first = xy[c0], last = xy[c0 + n - 1];
-    bool closing = !(first.x == last.x && first.y == last.y);  // Polygon::new would close the ring
-    int64_t nseg = n - 1 + (closing ? 1 : 0);
-    int wn = 0;
-    bool boundary = false;
-    for (int64_t i = lane; i < nseg; i += 32) {
-        double2 s = xy[c0 + i];
-        double2 e = (i + 1 < n) ? xy[c0 + i + 1] : first;
-        if (s.y <= p.y) {
-            if (e.y >= p.y) {
-                double o = orient2d(s.x, s.y, e.x, e.y, p.x, p.y);
-                if (o > 0.0 && e.y != p.y) wn += 1;
-                else if (o == 0.0 && value_in_between(p.x, s.x, e.x)) boundary = true;
-            }
-        } else if (e.y <= p.y) {
-            double o = orient2d(s.x, s.y, e.x, e.y, p.x, p.y);
-            if (o < 0.0) wn -= 1;
-            else if (o == 0.0 && value_in_between(p.x, s.x, e.x)) boundary = true;
-        }
-    }
-    if (__any_sync(0xffffffffu, boundary)) return 1;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) wn += __shfl_xor_sync(0xffffffffu, wn, o);
-    return wn == 0 ? 0 : 2;
-}
-// Polygon::calculate_coordinate_position over rings [r0,r1)
-__device__ __forceinline__ void polygon_position(const double2 *__restrict__ xy, const int64_t *__restrict__ ring_off, int64_t r0,
-                                                 int64_t r1, double2 p, int lane, bool &inside, int &boundary_count) {
-    if (r1 <= r0) return;
-    if (ring_off[r0 + 1] - ring_off[r0] == 0) return;
-    int pos = ring_position(xy, ring_off[r0], ring_off[r0 + 1] - ring_off[r0], p, lane);
-    if (pos == 0) return;
-    if (pos == 1) {
-        boundary_count += 1;
-        return;
-    }
-    for (int64_t r = r0 + 1; r < r1; ++r) {
-        int hp = ring_position(xy, ring_off[r], ring_off[r + 1] - ring_off[r], p, lane);
-        if (hp == 1) {
-            boundary_count += 1;
-            return;
-        }
-        if (hp == 2) return;
-    }
-    inside = true;
-}
-
+// pt_dist / line_segment_distance: common.cuh; line_string_contains_point, point_ls_distance, ring_position,
+// polygon_position, Side, point_polygon_distance: point_dist.cuh
 
 // ---- generic row-wise intersects: every pair of GeoArrow types --------------------------------------------
 // geo 0.27 intersects/{coordinate,line,line_string,polygon,collections}.rs (recalled).  The boolean is decided
@@ -508,11 +422,6 @@ __device__ __forceinline__ bool boxes_disjoint(const Box &a, const Box &b) {
     return a.has && b.has && (a.x0 > b.x1 || b.x0 > a.x1 || a.y0 > b.y1 || b.y0 > a.y1);
 }
 
-struct Side {
-    int type;
-    const double2 *xy;
-    const int64_t *go, *po, *ro;
-};
 __device__ __forceinline__ int side_class(int t) { return (t == GPL_POINT || t == GPL_MULTIPOINT) ? 0 : (t == GPL_LINESTRING || t == GPL_MULTILINESTRING) ? 1 : 2; }
 // sub-geometries of row r: points [lo,hi) of class 0; chains of class 1; polygon parts of class 2
 __device__ __forceinline__ void side_range(const Side &s, int64_t r, int64_t &lo, int64_t &hi) {
@@ -706,20 +615,6 @@ __global__ void __launch_bounds__(256) k_distance_generic(int64_t n, Side a, con
 // Members are addressed through VIEW sides of the single types: MultiPoint -> coordinate index, MultiLineString ->
 // LINESTRING view whose go is the ring_off level, MultiPolygon -> POLYGON view whose go is the part_off level.
 // A member pair on which geo would panic (nearest_neighbor on an empty tree) makes the row invalid.
-__device__ __forceinline__ double point_polygon_distance(const Side &s, int64_t q, double2 p, int lane) {
-    const int64_t r0 = s.go[q], r1 = s.go[q + 1];
-    if (r1 <= r0 || s.ro[r0 + 1] - s.ro[r0] == 0) return 0.0;
-    bool inside = false;
-    int bc = 0;
-    polygon_position(s.xy, s.ro, r0, r1, p, lane, inside, bc);
-    if (bc % 2 == 1 || inside) return 0.0;
-    double acc = 1.7976931348623157e308;
-    for (int64_t h = r0 + 1; h < r1; ++h) acc = fmin(acc, point_ls_distance(s.xy, s.ro[h], s.ro[h + 1] - s.ro[h], p, lane));
-    double ext = 1.7976931348623157e308;
-    const int64_t c0 = s.ro[r0], nn = s.ro[r0 + 1] - c0;
-    for (int64_t i = lane; i < nn - 1; i += 32) ext = fmin(ext, line_segment_distance(p, s.xy[c0 + i], s.xy[c0 + i + 1]));
-    return fmin(acc, warp_min(ext));
-}
 // a, b: single-type views (POINT / LINESTRING / POLYGON), ia / ib: member indices
 __device__ __forceinline__ double member_distance(const Side &a, int64_t ia, const Side &b, int64_t ib, int lane, bool &ok) {
     const int ca = side_class(a.type), cb = side_class(b.type);
@@ -1313,58 +1208,11 @@ extern "C" int gpl_distance(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b
 // the intersection box); count -> scan -> write gives the candidate list, a warp per candidate evaluates the
 // dispatched predicate, and a second scan compacts the hits.  Points x (Multi)Polygons with millions of points should
 // use gpl_pip_index_build + gpl_contains_join (the north-star path); this entry point is the general one.
-struct gpl_pairs {  // also defined (identically) in k_pip.cu for gpl_contains_join_pairs_array
-    gpl_ctx *ctx = nullptr;
-    uint64_t *lhs = nullptr, *rhs = nullptr;  // device
-    int64_t n = 0;
-};
-
+// JoinGrid, jg_cell, k_join_union, k_join_cells: join_grid.cuh; struct gpl_pairs: common.cuh
 namespace gpl {
 
 int envelope_raw(gpl_ctx *ctx, const gpl_array *in, double *out4_dev, uint8_t *valid_bytes_dev);
 
-struct JoinGrid {
-    double x0, y0, inv_w, inv_h;
-    int32_t g;
-};
-__device__ __forceinline__ int32_t jg_cell(double v, double lo, double inv, int32_t g) {
-    return min(max(__double2int_rd((v - lo) * inv), 0), g - 1);  // monotone (see k_pip.cu fine_index)
-}
-// union box of the valid envelopes: block reduce + ordered atomics (acc[0..3] zeroed by the host)
-__global__ void __launch_bounds__(256) k_join_union(const double *__restrict__ b4, const uint8_t *__restrict__ has, int64_t n,
-                                                    unsigned long long *__restrict__ acc) {
-    const double inf = __longlong_as_double(0x7ff0000000000000LL);
-    double x0 = inf, y0 = inf, x1 = -inf, y1 = -inf;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        if (has[i]) x0 = fmin(x0, b4[4 * i]), y0 = fmin(y0, b4[4 * i + 1]), x1 = fmax(x1, b4[4 * i + 2]), y1 = fmax(y1, b4[4 * i + 3]);
-    x0 = warp_min(x0), y0 = warp_min(y0), x1 = warp_max(x1), y1 = warp_max(y1);
-    auto enc = [](double d) {
-        const unsigned long long b = (unsigned long long)__double_as_longlong(d);
-        return (b >> 63) ? ~b : (b | 0x8000000000000000ULL);
-    };
-    if ((threadIdx.x & 31) == 0 && x0 <= x1 && y0 <= y1) {
-        atomicMax(acc + 0, ~enc(x0));
-        atomicMax(acc + 1, ~enc(y0));
-        atomicMax(acc + 2, enc(x1));
-        atomicMax(acc + 3, enc(y1));
-    }
-}
-// right rows into grid cells: pass 0 counts, pass 1 fills
-template <int PASS>
-__global__ void k_join_cells(const double *__restrict__ b4, const uint8_t *__restrict__ has, int64_t n, JoinGrid jg,
-                             int32_t *__restrict__ count_or_cursor, int32_t *__restrict__ items) {
-    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= n || !has[i]) return;
-    const int32_t cx0 = jg_cell(b4[4 * i], jg.x0, jg.inv_w, jg.g), cx1 = jg_cell(b4[4 * i + 2], jg.x0, jg.inv_w, jg.g);
-    const int32_t cy0 = jg_cell(b4[4 * i + 1], jg.y0, jg.inv_h, jg.g), cy1 = jg_cell(b4[4 * i + 3], jg.y0, jg.inv_h, jg.g);
-    for (int32_t cy = cy0; cy <= cy1; ++cy)
-        for (int32_t cx = cx0; cx <= cx1; ++cx) {
-            const int64_t c = (int64_t)cy * jg.g + cx;
-            if (PASS == 0) atomicAdd(&count_or_cursor[c], 1);
-            else items[atomicAdd(&count_or_cursor[c], 1)] = (int32_t)i;
-        }
-}
-// candidates of each left row: pass 0 counts, pass 1 writes (lhs, rhs) at off[i]
 template <int PASS>
 __global__ void k_join_candidates(const double *__restrict__ l4, const uint8_t *__restrict__ lhas, int64_t nl, const double *__restrict__ r4,
                                   JoinGrid jg, double ux1, double uy1, const int32_t *__restrict__ cell_start,

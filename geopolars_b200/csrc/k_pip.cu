@@ -2369,12 +2369,7 @@ extern "C" int gpl_contains_join_pairs(gpl_ctx *ctx, const gpl_pip_index *idx, c
     return GPL_OK;
 }
 
-// result of a join: defined in k_pairs.cu (gpl_spatial_join); the points-in-polygons join can return the same object
-struct gpl_pairs {
-    gpl_ctx *ctx = nullptr;
-    uint64_t *lhs = nullptr, *rhs = nullptr;  // device
-    int64_t n = 0;
-};
+// result of a join (struct gpl_pairs, common.cuh): the points-in-polygons join returns the same object as gpl_spatial_join
 extern "C" int gpl_contains_join_pairs_array(gpl_ctx *ctx, const gpl_pip_index *idx, const gpl_array *points, gpl_pairs **out) {
     GPL_REQUIRE(ctx && idx && points && out, GPL_ERR_INVALID_ARG, "gpl_contains_join_pairs_array: NULL argument");
     GPL_REQUIRE(points->type == GPL_POINT, GPL_ERR_INVALID_TYPE, "Expected Point (found geometry type %d)", points->type);

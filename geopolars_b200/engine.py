@@ -586,3 +586,74 @@ class PipIndex:
             self.free()
         except Exception:
             pass
+
+
+class NearestIndex:
+    """Right side of a nearest-geometry join (GeoPandas' sjoin_nearest): a grid over the rows of any geometry column.
+    The distance of a (point, row) pair is exactly what `distance` returns for it; see DESIGN.md §4.12."""
+
+    STATS = ("rows", "excluded", "everywhere", "grid_cells_per_axis", "cell_items", "bytes", "evaluations", "overflow_points")
+
+    def __init__(self, rhs: DeviceArray):
+        self.ctx = rhs.ctx
+        self.rhs = rhs  # keep alive: the index references its coordinates
+        h = C.c_void_p()
+        check(self.ctx.lib.gpl_nearest_index_build(self.ctx._h, rhs._h, C.byref(h)))
+        self._h = h
+
+    def stats(self) -> dict:
+        """row classes, grid shape and size; exact evaluations and overflow points of the last query"""
+        out = np.zeros(8, dtype=np.int64)
+        check(self.ctx.lib.gpl_nearest_index_stats(self.ctx._h, self._h, _np_ptr(out)))
+        return dict(zip(self.STATS, (int(v) for v in out)))
+
+    @staticmethod
+    def _maxd(max_distance) -> float:
+        return float("inf") if max_distance is None else float(max_distance)
+
+    def query(self, points_xy: np.ndarray, max_distance=None):
+        """(nearest_id int32 (-1: none), distance float64 (NaN: none), n_tied int32) for host points (n, 2)"""
+        pts = np.ascontiguousarray(points_xy, dtype=np.float64).reshape(-1, 2)
+        n = pts.shape[0]
+        nid = np.empty(n, dtype=np.int32)
+        dist = np.empty(n, dtype=np.float64)
+        tied = np.empty(n, dtype=np.int32)
+        check(self.ctx.lib.gpl_nearest_join(self.ctx._h, self._h, _np_ptr(pts), n, self._maxd(max_distance), _np_ptr(nid), _np_ptr(dist),
+                                            _np_ptr(tied), GPL_HOST))
+        return nid, dist, tied
+
+    def query_device(self, points_ptr: int, n: int, max_distance, nid_ptr: int, dist_ptr: int = 0, tied_ptr: int = 0) -> None:
+        """all buffers already in HBM: stream ordered, no host round trip"""
+        check(self.ctx.lib.gpl_nearest_join(self.ctx._h, self._h, C.c_void_p(points_ptr), n, self._maxd(max_distance), C.c_void_p(nid_ptr),
+                                            C.c_void_p(dist_ptr) if dist_ptr else None, C.c_void_p(tied_ptr) if tied_ptr else None,
+                                            GPL_DEVICE))
+
+    def query_array(self, points: DeviceArray, max_distance=None):
+        """the same for a Point column in HBM (null points match nothing)"""
+        n = len(points)
+        nid = np.empty(n, dtype=np.int32)
+        dist = np.empty(n, dtype=np.float64)
+        tied = np.empty(n, dtype=np.int32)
+        check(self.ctx.lib.gpl_nearest_join_array(self.ctx._h, self._h, points._h, self._maxd(max_distance), _np_ptr(nid), _np_ptr(dist),
+                                                  _np_ptr(tied), GPL_HOST))
+        return nid, dist, tied
+
+    def pairs_array(self, points: DeviceArray, max_distance=None, with_distance: bool = False):
+        """every tied (point, row) pair once, sorted by (lhs, rhs) [+ the dense distance of every point, NaN: no match]"""
+        h = C.c_void_p()
+        dist = np.empty(len(points), dtype=np.float64) if with_distance else None
+        check(self.ctx.lib.gpl_nearest_join_pairs_array(self.ctx._h, self._h, points._h, self._maxd(max_distance), C.byref(h), _np_ptr(dist),
+                                                        GPL_HOST))
+        lhs, rhs = _pairs_to_host(self.ctx, h)
+        return (lhs, rhs, dist) if with_distance else (lhs, rhs)
+
+    def free(self) -> None:
+        if getattr(self, "_h", None) and self.ctx._h:
+            self.ctx.lib.gpl_nearest_index_free(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass

@@ -310,3 +310,29 @@ def spatial_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", predicate: 
         order = np.lexsort((b, a))
         a, b = a[order], b[order]
     return a, b
+
+
+def nearest_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", max_distance: Optional[float] = None):
+    """Nearest-geometry join of a Point column against any geometry column (GeoPandas' sjoin_nearest with
+    max_distance / distance_col): (lhs_index int64, rhs_index int64, distance float64), sorted by (lhs, rhs).  Every right
+    row at the minimum distance is returned (ties are equal f64 distances, as GeoPandas returns all equidistant rows); the
+    distance is exactly what `lhs.geo.distance` computes for the pair.  max_distance is inclusive (None: unbounded).
+    how='inner' -> matched points only; how='left' -> unmatched points once, with rhs_index -1 and distance NaN."""
+    if how not in ("inner", "left"):
+        raise ValueError("how must be 'inner' or 'left'")
+    idx = E.NearestIndex(rhs.device)
+    try:
+        a, b, dist = idx.pairs_array(lhs.device, max_distance, with_distance=True)
+    finally:
+        idx.free()
+    a = a.astype(np.int64)
+    b = b.astype(np.int64)
+    d = dist[a]
+    if how == "left":
+        miss = np.nonzero(np.isnan(dist))[0]
+        a = np.concatenate([a, miss])
+        b = np.concatenate([b, np.full(len(miss), -1, dtype=np.int64)])
+        d = np.concatenate([d, np.full(len(miss), np.nan)])
+        order = np.lexsort((b, a))
+        a, b, d = a[order], b[order], d[order]
+    return a, b, d

@@ -70,6 +70,7 @@ typedef enum gpl_origin { GPL_ORIGIN_CENTROID = 0, GPL_ORIGIN_CENTER = 1, GPL_OR
 typedef struct gpl_ctx gpl_ctx;             /* one per (host thread, device) */
 typedef struct gpl_array gpl_array;         /* GeoArrow geometry array resident in HBM */
 typedef struct gpl_pip_index gpl_pip_index;
+typedef struct gpl_nearest_index gpl_nearest_index; /* right side of a nearest join */
 typedef struct gpl_pairs gpl_pairs;         /* (lhs_index, rhs_index) pair list of a join, resident on the device */ /* polygon-side index of a contains join */
 
 /* Raw GeoArrow buffers (the zero-dependency form of an Arrow array; replaces the WKB BinaryArray the
@@ -295,6 +296,36 @@ int gpl_spatial_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, i
 int64_t gpl_pairs_count(const gpl_pairs *pairs);
 int gpl_pairs_copy(gpl_ctx *ctx, const gpl_pairs *pairs, uint64_t *lhs, uint64_t *rhs, int mem);
 void gpl_pairs_free(gpl_pairs *pairs);
+
+/* ---------------------------------------------------------------- nearest join ----------- */
+/* Nearest-geometry join (GeoPandas sjoin_nearest; rstar's nearest_neighbor): for each point of a POINT column, the right
+ * rows at the smallest distance.  Right side: Point / LineString / Polygon / MultiPoint / MultiLineString / MultiPolygon,
+ * fewer than 2^31 rows.  Candidate rows R: non-null, with an envelope and only finite coordinates; no other row matches.
+ * d(i, j) is exactly the f64 value gpl_distance returns for the row pair (lhs[i], rhs[j]).  The nearest rows of point i
+ * are those of R at the minimum d <= max_distance (inclusive; +inf = unbounded; NaN or negative -> GPL_ERR_INVALID_ARG);
+ * rows tie when their distances are equal f64 values.  Null points and points with a non-finite coordinate match nothing.
+ * The index keeps a reference to `rhs` (must outlive it). */
+int gpl_nearest_index_build(gpl_ctx *ctx, const gpl_array *rhs, gpl_nearest_index **out);
+void gpl_nearest_index_free(gpl_nearest_index *idx);
+/* synchronises the context stream: out8[0] = rows in R, [1] = excluded rows, [2] = rows every query evaluates (an empty
+ * member, an empty ring or a 1-coordinate linestring / ring), [3] = grid cells per axis, [4] = cell items, [5] = index
+ * bytes, [6] = exact distance evaluations of the last query pass, [7] = points the last query pass sent to the overflow
+ * path.  [6] and [7] live in the index: gpl_nearest_join_pairs_array runs two passes and leaves the counts of its second,
+ * and queries of one index issued concurrently on different streams overwrite each other's counts (never their results). */
+int gpl_nearest_index_stats(gpl_ctx *ctx, const gpl_nearest_index *idx, int64_t *out8);
+/* dense form: nearest_id[i] = lowest tied row or -1, distance[i] (may be NULL) = its distance or NaN, n_tied[i] (may be
+ * NULL) = number of tied rows.  points_xy interleaved, n_points < 2^31 (else GPL_ERR_UNSUPPORTED), all buffers in `mem`. */
+int gpl_nearest_join(gpl_ctx *ctx, const gpl_nearest_index *idx, const double *points_xy, int64_t n_points, double max_distance,
+                     int32_t *nearest_id, double *distance, int32_t *n_tied, int mem);
+/* the same for a POINT gpl_array (any other type: GPL_ERR_INVALID_TYPE); outputs in `mem` */
+int gpl_nearest_join_array(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *points, double max_distance,
+                           int32_t *nearest_id, double *distance, int32_t *n_tied, int mem);
+/* every tied (point, row) pair once, sorted by (lhs, rhs), as a device-resident gpl_pairs; distance (may be NULL, in
+ * `mem`) receives the dense distance of every point (NaN: no match), which the pair list is built from.  The rows of one
+ * point are ordered by a rank sort of O(k^2) for k tied rows: fine for ties among a few thousand rows, slow for a point
+ * tied with ~1e5 or more rows (e.g. that many coincident geometries). */
+int gpl_nearest_join_pairs_array(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *points, double max_distance,
+                                 gpl_pairs **out, double *distance, int mem);
 
 /* ---------------------------------------------------------------- synthetic data --------- */
 /* device-side generators, bit-identical to geopolars_b200/synth.py (SURVEY.md §8d RNG) */

@@ -1,14 +1,16 @@
 #!/usr/bin/env python
 """Kernel-resident timings of the other §8 rows at BASELINE config sizes (3 and 5), with the HBM roofline
-fraction for the coordinate bytes read.  Not the flagship bench (that is bench.py, config 2); config 5 runs at
+fraction for the coordinate bytes read, and of the nearest join (100 M points against config 2's polygons, 1 M
+reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
 import json
 import os
+import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -39,6 +41,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
+    ap.add_argument("--only", choices=("all", "ops", "nearest"), default="all", help="run only the §8 rows or only the nearest join")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
@@ -55,9 +58,23 @@ def main():
         res["rows"].append(r)
         print(json.dumps(r), flush=True)
 
+    res["card"] = torch.cuda.get_device_name(0)
+    try:  # read-only query: the power limit is part of every number below
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True,
+                           timeout=30)
+        res["power_limit"] = q.stdout.strip().split(",")[-1].strip() if q.returncode == 0 else "unknown"
+    except (OSError, subprocess.SubprocessError):
+        res["power_limit"] = "unknown"
+    print(json.dumps({"card": res["card"], "power_limit": res["power_limit"]}), flush=True)
     with torch.cuda.stream(st):
         ctx = E.Context(0, st.cuda_stream)
         lib = ctx.lib
+        if args.only in ("all", "nearest"):
+            nearest_rows(args, ctx, dev, st, res)
+        if args.only == "nearest":
+            ctx.synchronize()
+            _write(args, res)
+            return
         # ---- config 5: G polygons x 257 coords: affine, area, centroid, convex_hull ----------------------
         G, NV = int(4_000_000 * args.scale), 256
         nc = G * (NV + 1)
@@ -156,10 +173,83 @@ def main():
         t = timed(st, lambda: E.check(lib.gpl_distance(ctx._h, A._h, B._h, C.c_void_p(dist.data_ptr()), None, E.GPL_DEVICE)), reps=3, warm=1)
         row("distance LineString pairs (config 3, includes the intersects test)", N, "pairs", 2 * N * K * 16 + 2 * (N + 1) * 8, N * 8, *t)
         res["intersect_fraction"] = float((dist == 0).float().mean().item())
-    os.makedirs(os.path.dirname(args.out), exist_ok=True)
+    _write(args, res)
+
+
+def _write(args, res):
+    if os.path.dirname(args.out):
+        os.makedirs(os.path.dirname(args.out), exist_ok=True)
     with open(args.out, "w") as f:
         json.dump(res, f, indent=1)
     print("wrote", args.out)
+
+
+def nearest_rows(args, ctx, dev, st, res):
+    """nearest join, kernel resident: build ms, query ms, G points/s and exact evaluations per point"""
+    from geopolars_b200 import synth
+
+    lib = ctx.lib
+    NP = int(100_000_000 * args.scale)
+    pts = torch.empty((NP, 2), dtype=torch.float64, device=dev)
+    E.check(lib.gpl_gen_uniform_points(ctx._h, 2, 0, NP, 1000.0, pts.data_ptr()))
+    nid = torch.empty(NP, dtype=torch.int32, device=dev)
+    dist = torch.empty(NP, dtype=torch.float64, device=dev)
+    tied = torch.empty(NP, dtype=torch.int32, device=dev)
+
+    def run(name, rhs, n_rhs):
+        tb = timed(st, lambda: E.NearestIndex(rhs).free(), reps=3, warm=1)
+        idx = E.NearestIndex(rhs)
+        t = timed(st, lambda: idx.query_device(pts.data_ptr(), NP, None, nid.data_ptr(), dist.data_ptr(), tied.data_ptr()), reps=3, warm=1)
+        s = idx.stats()
+        r = {"op": f"nearest join: {NP} uniform points x {name}", "points": NP, "rhs_rows": n_rhs, "build_ms_min": tb[0], "query_ms_min": t[0],
+             "query_ms_avg": t[1], "Gpoints_per_s": NP / (t[1] * 1e-3) / 1e9, "evals_per_point": s["evaluations"] / NP,
+             "overflow_points": s["overflow_points"], "grid_cells_per_axis": s["grid_cells_per_axis"], "index_bytes": s["bytes"],
+             "card": res["card"], "power_limit": res["power_limit"]}
+        idx.free()
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    # config 2's 10 k 64-vertex star polygons on a 100 x 100 lattice of 10-unit cells (the points' 1000 x 1000 square)
+    m, nv = 10_000, 64
+    xy, ro, go = synth.star_polygons(m, 100, 10.0, nv)
+    pxy, pro, pgo = (torch.from_numpy(a).to(dev) for a in (xy, ro, go))
+    polys = ctx.wrap_device(GeometryType.POLYGON, m, m * (nv + 1), pxy.data_ptr(), geom_off_ptr=pgo.data_ptr(), ring_off_ptr=pro.data_ptr(),
+                            n_rings=m, keepalive=(pxy, pro, pgo))
+    run("config 2's 10 k 64-vertex polygons", polys, m)
+    # CPU arm: the independent reference of the tests (its own ring search in Python, the C oracle's distances), one core
+    import time
+
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import nearest_reference as nr
+    from oracle import oracle as og
+
+    k = 2000
+    a = og.OGArray(og.POLYGON, xy, geom_off=go, ring_off=ro)
+    host_pts = pts[:k].cpu().numpy()
+    t0 = time.perf_counter()
+    nr.nearest_join(a, host_pts, use_grid=True)
+    dt = time.perf_counter() - t0
+    r = {"op": f"nearest join CPU arm: the test reference (Python ring search + C oracle distances, one core), {k}-point prefix x "
+               "config 2's polygons", "points": k, "seconds": dt, "points_per_s": k / dt}
+    res["rows"].append(r)
+    print(json.dumps(r), flush=True)
+    # 1 M uniform reference points in the same square
+    R = int(1_000_000 * max(args.scale, 0.01))
+    rxy = torch.empty((R, 2), dtype=torch.float64, device=dev)
+    E.check(lib.gpl_gen_uniform_points(ctx._h, 7, 0, R, 1000.0, rxy.data_ptr()))
+    refs = ctx.wrap_device(GeometryType.POINT, R, R, rxy.data_ptr(), keepalive=(rxy,))
+    run(f"{R} uniform reference points", refs, R)
+    # 1 M 16-vertex random-walk linestrings (config 3's generator)
+    K = 16
+    lxy = torch.empty((R * K, 2), dtype=torch.float64, device=dev)
+    loff = torch.empty(R + 1, dtype=torch.int64, device=dev)
+    E.check(lib.gpl_gen_walk_linestrings(ctx._h, 3, -1, 0, R, K, lxy.data_ptr(), loff.data_ptr()))
+    lines = ctx.wrap_device(GeometryType.LINESTRING, R, R * K, lxy.data_ptr(), geom_off_ptr=loff.data_ptr(), keepalive=(lxy, loff))
+    ctx.synchronize()
+    res["walk_linestring_extent"] = [float(v) for v in torch.cat([lxy.min(0).values, lxy.max(0).values]).cpu()]
+    run(f"{R} {K}-vertex walk linestrings", lines, R)
+    del pts, nid, dist, tied
+    torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":
