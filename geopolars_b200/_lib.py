@@ -147,6 +147,8 @@ SIGNATURES = {
     "gpl_pip_index_bytes": (_I64, [_P]),
     "gpl_pip_index_stats": (_INT, [_P, _P, _P]),
     "gpl_pip_index_phases": (_INT, [_P, _P, _P]),
+    "gpl_pip_index_timeline": (_INT, [_P, _P, _P]),
+    "gpl_pip_index_dump": (_INT, [_P, _P, _INT, _P, C.POINTER(_I64)]),
     "gpl_contains_join": (_INT, [_P, _P, _P, _I64, _P, _P, _INT]),
     "gpl_contains_join_counts": (_INT, [_P, _P, _P, _I64, _P, _P, _INT]),
     "gpl_contains_join_array": (_INT, [_P, _P, _P, _P, _P, _INT]),

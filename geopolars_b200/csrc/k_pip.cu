@@ -192,7 +192,9 @@ constexpr int kMaxBuildCtas = 1024;
 
 enum {  // BuildArgs::acc slots (unsigned long long each, zeroed by the host before the count kernel)
     ACC_XMIN = 0, ACC_YMIN, ACC_XMAX, ACC_YMAX,  // union bbox, order-preserving encodings (min as max of the complement)
-    ACC_HOLES, ACC_NOT_FAST, ACC_ITEMS, ACC_BUCKETS, ACC_ENTRIES, ACC_FAST, ACC_COUNT
+    ACC_HOLES, ACC_NOT_FAST, ACC_ITEMS, ACC_BUCKETS, ACC_ENTRIES, ACC_FAST,
+    ACC_RASTER_NEXT,  // the raster phase's work counter (next unclaimed item)
+    ACC_COUNT
 };
 
 struct BuildArgs {
@@ -203,6 +205,9 @@ struct BuildArgs {
     const uint8_t *validity;
     int slots_x100;
     int32_t G, rs;
+    int32_t raster_rows;     // fine rows per raster work item (8, 16 or 32)
+    int32_t build_legacy;    // 1: the previous work distribution (A/B): one thread per y-bucket in ph_bucket_finish,
+                             //    (part, 32-row chunk) raster items dealt out statically, it += nwarps
     int64_t n_cells, NB_cap;
     // phase 1 (scratch)
     PartHeader *hdr;
@@ -231,6 +236,7 @@ struct BuildArgs {
     uint2 *raster;          // per 16 fine cells: x = their 2-bit codes, y = the row of the coarse cell's candidate #0
     unsigned long long *n_deferred;
     unsigned long long *phase_t;  // 16 global-timer stamps (ns) taken by one thread at the phase boundaries of both kernels
+    const unsigned long long *count_t;  // fill kernel: the count kernel's stamps 0..4 (scratch), copied into phase_t
 };
 __device__ __forceinline__ unsigned long long global_ns() {
     unsigned long long t;
@@ -702,6 +708,119 @@ __device__ void ph_bucket_finish(const BuildArgs &a, const int32_t *__restrict__
     }
 }
 
+// The same bucket finishing with a GROUP of kFinishLanes lanes per y-bucket, one entry per lane: the edge ids are read
+// coalesced, the f64 records leave as contiguous runs, and each lane finds its slot in the two FP32 lists from a ballot
+// (prefix count of the earlier entries on that side), so every record lands where the serial loop above puts it.  On config 2
+// (110 k buckets of 9-20 entries) one thread per bucket issued every load and store of a bucket from one lane, ~30 partly
+// used sectors per warp instruction, and the phase took 0.48 ms on one H100.
+constexpr int kFinishLanes = 8;
+__device__ void ph_bucket_finish_groups(const BuildArgs &a, const int32_t *__restrict__ bstart) {
+    constexpr int GS = kFinishLanes, GPW = 32 / GS;  // lanes per bucket, buckets per warp
+    const int lane = threadIdx.x & 31, sub = lane & (GS - 1), grp = lane / GS;
+    const uint32_t gmask = ((1u << GS) - 1u) << (grp * GS), lt = (1u << lane) - 1u;
+    const int64_t warp = ((int64_t)blockIdx.x * kBuildThreads + threadIdx.x) >> 5;
+    const int64_t nwarps = ((int64_t)gridDim.x * kBuildThreads) >> 5;
+    const float inf = __int_as_float(0x7f800000);
+    const float4 sentinel = make_float4(0.0f, inf, 0.0f, inf);
+    // warp-uniform trip counts: every __ballot_sync / __shfl_sync below sees all 32 lanes
+    for (int64_t base = warp * GPW; base < a.n_buckets; base += nwarps * GPW) {
+        const int64_t gb = base + grp;
+        const bool have = gb < a.n_buckets;
+        int32_t e0 = 0, n = 0, p = 0;
+        if (have) e0 = bstart[gb], n = bstart[gb + 1] - e0, p = a.bucket_part[gb];
+        PartHeader h;
+        int64_t r0 = 0, r1 = 0;
+        if (have) {
+            h = a.hdr[p];
+            part_rings(a.type, p, a.geom_off, a.part_off, r0, r1);
+        } else {
+            h.flags = 0, h.bucket_base = 0;
+        }
+        // parts with holes: entries ascending by edge id (grouped by ring), as ph_bucket_finish orders them
+        if (have && (h.flags & 1) && sub == 0) {
+            int64_t *g = a.entry_edge + e0;
+            for (int32_t i = 1; i < n; ++i) {
+                const int64_t v = g[i];
+                int32_t j = i - 1;
+                while (j >= 0 && g[j] > v) {
+                    g[j + 1] = g[j];
+                    --j;
+                }
+                g[j + 1] = v;
+            }
+        }
+        __syncwarp();
+        const bool fast = have && a.fast_c[p] > 0;
+        const int32_t b = (int32_t)(gb - h.bucket_base);
+        float4 *fbase = nullptr, *list0 = nullptr, *list1 = nullptr;
+        int2 ovf = make_int2(0, 0);
+        double ox = 0.0, mx = 0.0, oy = 0.0, xm = 0.0;
+        if (fast) {
+            fbase = a.fast + (int64_t)a.fast_slots[p];
+            list0 = fbase + ((int64_t)b * 2) * kFastListRecs, list1 = list0 + kFastListRecs;
+            ovf = a.ovf_off[gb];
+            ox = (double)__double2float_rd(h.xmin), mx = (double)__double2float_ru(h.xmax), oy = h.by0;
+            xm = fast_split_x(h);
+        }
+        const int64_t ext0 = have ? a.ring_off[r0] : 0, ext1 = have ? a.ring_off[r0 + 1] : 0;
+        int32_t nmax = n;  // longest bucket of the warp
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) nmax = max(nmax, __shfl_xor_sync(0xffffffffu, nmax, o));
+        int32_t c0 = 0, c1 = 0;  // lengths of the two one-sided lists so far (same in every lane of the group)
+        for (int32_t k0 = 0; k0 < nmax; k0 += GS) {
+            const int32_t k = k0 + sub;
+            const bool act = have && k < n;
+            bool right = false, left = false;
+            float4 fr, fl;
+            if (act) {
+                const int64_t c = a.entry_edge[e0 + k];
+                int64_t r = r0, rc0 = ext0, rc1 = ext1;
+                if (h.flags & 1) {
+                    while (r + 1 < r1 && a.ring_off[r + 1] <= c) ++r;
+                    rc0 = a.ring_off[r], rc1 = a.ring_off[r + 1];
+                }
+                const double2 s = __ldg(a.xy + c);
+                const double2 e = c + 1 < rc1 ? __ldg(a.xy + c + 1) : (rc1 - rc0 == 1 ? s : __ldg(a.xy + rc0));
+                EdgeRec rec;
+                rec.sx = s.x, rec.sy = s.y, rec.ex = e.x, rec.ey = e.y;
+                a.entries[e0 + k] = rec;
+                if (a.entry_ring) a.entry_ring[e0 + k] = (int32_t)(r - r0);
+                if (fast) {
+                    right = fmax(s.x, e.x) >= xm;
+                    left = fmin(s.x, e.x) <= xm;
+                    fr = make_float4(__double2float_rn(s.x - ox), __double2float_rn(s.y - oy), __double2float_rn(e.x - ox),
+                                     __double2float_rn(e.y - oy));
+                    fl = make_float4(__double2float_rn(mx - s.x), __double2float_rn(s.y - oy), __double2float_rn(mx - e.x),
+                                     __double2float_rn(e.y - oy));
+                }
+            }
+            const uint32_t br = __ballot_sync(0xffffffffu, right) & gmask, bl = __ballot_sync(0xffffffffu, left) & gmask;
+            if (right) {
+                const int32_t pos = c0 + __popc(br & lt);
+                if (pos < kFastListRecs - 1) list0[1 + pos] = fr;
+                else fbase[ovf.x + pos - (kFastListRecs - 1)] = fr;
+            }
+            if (left) {
+                const int32_t pos = c1 + __popc(bl & lt);
+                if (pos < kFastListRecs - 1) list1[1 + pos] = fl;
+                else fbase[ovf.y + pos - (kFastListRecs - 1)] = fl;
+            }
+            c0 += __popc(br), c1 += __popc(bl);
+        }
+        if (fast) {
+            for (int32_t k = c0 + sub; k < kFastListRecs - 1; k += GS) list0[1 + k] = sentinel;
+            for (int32_t k = c1 + sub; k < kFastListRecs - 1; k += GS) list1[1 + k] = sentinel;
+            if (sub == 0) {
+                const int32_t n0 = max(c0 - (kFastListRecs - 1), 0), n1 = max(c1 - (kFastListRecs - 1), 0);
+                list0[0] = make_float4(__int_as_float(c0), __int_as_float(n0 ? ovf.x : 0), 0.0f, 0.0f);
+                list1[0] = make_float4(__int_as_float(c1), __int_as_float(n1 ? ovf.y : 0), 0.0f, 0.0f);
+                if (n0 & 1) fbase[ovf.x + n0] = sentinel;
+                if (n1 & 1) fbase[ovf.y + n1] = sentinel;
+            }
+        }
+    }
+}
+
 // one thread per segment: insertion sort (lists are a handful of items) — makes cell candidate lists
 // ascending by part id and bucket lists ascending by edge id (=> grouped by ring, deterministic).
 template <typename T>
@@ -936,11 +1055,20 @@ __device__ void ph_raster(const BuildArgs &a, const GridParams &g, const int32_t
     int32_t *cnt = sm.cnt[wid];
     uint32_t *list = sm.list[wid];
     double *row_y = sm.ry[wid];
-    // work item = (part, k): the chunks ra = fy0 + 32 (k + K j) of the part.  A part's bbox is about one coarse cell high,
-    // i.e. K = 2^rs / 32 chunks; they are independent (every raster write is an atomicOr), so config 4's 1 000 parts keep
-    // 4 000 warps busy instead of 1 000.
-    const int32_t K = max(1, min(8, (1 << g.rs) >> 5));
-    for (int64_t it = warp; it < a.P * K; it += nwarps) {
+    // work item = (part, k): the chunks ra = fy0 + R (k + K j) of the part, R = a.raster_rows fine rows each.  A part's bbox
+    // is about one coarse cell high, i.e. K = 2^rs / R chunks; they are independent (every raster write is an atomicOr).
+    // Items are claimed from a global counter: a warp that finishes early takes the next one, so the phase ends one small
+    // item after the work runs out instead of after a last, partly filled wave of a static deal.  Legacy (A/B): R = 32,
+    // K <= 8, item it to warp it mod nwarps.
+    const int32_t R = a.build_legacy ? 32 : a.raster_rows;
+    const int32_t K = a.build_legacy ? max(1, min(8, (1 << g.rs) >> 5)) : max(1, (1 << g.rs) / R);
+    auto claim = [&]() -> int64_t {
+        unsigned long long v = 0;
+        if (lane == 0) v = atomicAdd(a.acc + ACC_RASTER_NEXT, 1ULL);
+        return (int64_t)__shfl_sync(0xffffffffu, v, 0);
+    };
+    const int64_t n_items = a.P * K;
+    for (int64_t it = a.build_legacy ? warp : claim(); it < n_items; it = a.build_legacy ? it + nwarps : claim()) {
         const int64_t p = it / K;
         const int32_t kk = (int32_t)(it - p * K);
         const PartHeader h = a.hdr[p];
@@ -959,8 +1087,8 @@ __device__ void ph_raster(const BuildArgs &a, const GridParams &g, const int32_t
             for (int32_t k = lane; k < ncx * ncy; k += 32)
                 sm.code[wid][k] = (uint8_t)raster_rank_code(a, g, cell_start, cx0 + k % ncx, cy0 + k / ncx, (int32_t)p);
         __syncwarp();
-        for (int32_t ra = fy0 + 32 * kk; ra <= fy1; ra += 32 * K) {
-            const int32_t rb = min(ra + 31, fy1);
+        for (int32_t ra = fy0 + R * kk; ra <= fy1; ra += R * K) {
+            const int32_t rb = min(ra + R - 1, fy1);
             cnt[lane] = 0;
             row_y[lane] = g.y0 + ((double)(ra + lane) + 0.5) / g.inv_fh;
             __syncwarp();
@@ -1120,6 +1248,8 @@ __global__ void __launch_bounds__(kBuildThreads, 3) k_pip_build_fill(const Build
     const int64_t tid = (int64_t)blockIdx.x * kBuildThreads + threadIdx.x, nth = (int64_t)gridDim.x * kBuildThreads;
     const bool degenerate = g.inv_fw == 0.0 || g.inv_fh == 0.0;
     GPL_STAMP(a, 5);
+    if (blockIdx.x == 0 && threadIdx.x == 0 && a.phase_t && a.count_t)
+        for (int k = 0; k < 5; ++k) a.phase_t[k] = a.count_t[k];
     // T0: chunk-local scans (in place): cell counts -> cell starts, bucket counts -> bucket starts, FP32 slots ->
     // FP32 bases; raster cleared (all 3 on a degenerate grid: every point walks)
     grid_scan_local(a.cell_count, a.cell_count, a.n_cells, a.partial, sm_scan);
@@ -1163,9 +1293,10 @@ __global__ void __launch_bounds__(kBuildThreads, 3) k_pip_build_fill(const Build
     ph_buckets<1>(a, nullptr, 1);
     grid.sync();
     GPL_STAMP(a, 8);
-    // T3: candidate lists in ascending order; every y-bucket finished by one thread (sort, f64 records, FP32 lists)
+    // T3: candidate lists in ascending order; every y-bucket finished by a group of lanes (sort, f64 records, FP32 lists)
     ph_sort_segments<int32_t>(a.items, cell_start, a.n_cells);
-    ph_bucket_finish(a, bstart);
+    if (a.build_legacy) ph_bucket_finish(a, bstart);
+    else ph_bucket_finish_groups(a, bstart);
     ph_part_recs(a);
     for (int64_t b = tid; b < a.n_buckets; b += nth) a.bucket_range[b] = make_int2(bstart[b], bstart[b + 1]);
     grid.sync();
@@ -2067,6 +2198,42 @@ extern "C" int gpl_pip_index_phases(gpl_ctx *ctx, const gpl_pip_index *idx, doub
     for (int k = 0; k < 12; ++k) out12[k] = k >= 5 ? (double)(h[k] - h[5]) * 1e-3 : 0.0;
     return GPL_OK;
 }
+// the whole build timeline (diagnostics): out12[k] = microseconds from the COUNT kernel's start to stamp k — 0..4 = the count
+// kernel (start, after its barriers S0..S2, plan done), 5..11 as in gpl_pip_index_phases; synchronises the stream.
+extern "C" int gpl_pip_index_timeline(gpl_ctx *ctx, const gpl_pip_index *idx, double *out12) {
+    GPL_REQUIRE(ctx && idx && out12, GPL_ERR_INVALID_ARG, "gpl_pip_index_timeline: NULL argument");
+    GPL_CUDA(cudaSetDevice(ctx->device));
+    unsigned long long h[16];
+    GPL_CUDA(cudaMemcpyAsync(h, idx->phase_t, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    for (int k = 0; k < 12; ++k) out12[k] = (double)(long long)(h[k] - h[0]) * 1e-3;
+    return GPL_OK;
+}
+// read-only copy of one index table (diagnostics: two builds of the same polygons must agree byte for byte)
+extern "C" int gpl_pip_index_dump(gpl_ctx *ctx, const gpl_pip_index *idx, int which, void *dst, int64_t *nbytes) {
+    GPL_REQUIRE(ctx && idx && nbytes, GPL_ERR_INVALID_ARG, "gpl_pip_index_dump: NULL argument");
+    const int64_t n_cells = (int64_t)idx->grid.gx * idx->grid.gy;
+    const void *src = nullptr;
+    int64_t size = 0;
+    switch (which) {
+        case 0: src = idx->raster, size = (int64_t)sizeof(uint2) * idx->grid.fgy * idx->grid.wpr; break;
+        case 1: src = idx->cand01, size = (int64_t)sizeof(int2) * n_cells; break;
+        case 2: src = idx->cells, size = (int64_t)sizeof(CellRec) * n_cells; break;
+        case 3: src = idx->parts, size = (int64_t)sizeof(PartRec) * idx->n_parts; break;
+        default: GPL_REQUIRE(false, GPL_ERR_INVALID_ARG, "gpl_pip_index_dump: unknown table %d", which);
+    }
+    if (dst == nullptr) {
+        *nbytes = size;
+        return GPL_OK;
+    }
+    GPL_REQUIRE(*nbytes >= size, GPL_ERR_INVALID_ARG, "gpl_pip_index_dump: buffer of %lld bytes, table has %lld", (long long)*nbytes,
+                (long long)size);
+    GPL_CUDA(cudaSetDevice(ctx->device));
+    *nbytes = size;
+    if (size > 0) GPL_CUDA(cudaMemcpyAsync(dst, src, (size_t)size, cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    return GPL_OK;
+}
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -2135,6 +2302,16 @@ extern "C" int gpl_pip_index_build(gpl_ctx *ctx, const gpl_array *polys, gpl_pip
     a.xy = reinterpret_cast<const double2 *>(polys->xy);
     a.geom_off = polys->geom_off, a.part_off = polys->part_off, a.ring_off = polys->ring_off, a.validity = polys->validity;
     a.slots_x100 = slots_x100, a.G = (int32_t)G, a.rs = rs, a.n_cells = n_cells;
+    {
+        // GPL_PIP_BUILD_LEGACY=1: the previous build (static deal of (part, 32-row) raster items), for A/B measurements
+        static const bool build_legacy = env_int("GPL_PIP_BUILD_LEGACY", 0) != 0;
+        static const int raster_rows = [] {
+            const int v = env_int("GPL_PIP_RASTER_ROWS", 32);  // config 2 on one H100: 8 / 16 / 32 rows, raster phase 173 / 117 / 91 us
+            return v == 8 || v == 16 || v == 32 ? v : 32;
+        }();
+        a.build_legacy = build_legacy ? 1 : 0;
+        a.raster_rows = raster_rows;
+    }
     // sum of n_buckets <= P + n_coords * 100 / slots_x100 + 1 without a host round trip
     a.NB_cap = Pa + (polys->n_coords * 100) / slots_x100 + 1;
     Scratch<PartHeader> hdr;
@@ -2156,6 +2333,9 @@ extern "C" int gpl_pip_index_build(gpl_ctx *ctx, const gpl_array *polys, gpl_pip
     TRYF(fast_c.get(ctx, (size_t)Pa + 1));
     TRYF(fast_slots.get(ctx, (size_t)Pa + 1));
     TRYF(acc.get(ctx, ACC_COUNT));
+    Scratch<unsigned long long> count_t;  // the count kernel's phase stamps, until the slab exists
+    TRYF(count_t.get(ctx, 8));
+    a.phase_t = count_t.p;
     a.hdr = hdr.p, a.gp = gp.p, a.nb = nb.p, a.partial = partial.p, a.cell_count = cell_count.p, a.bcount = bcount.p;
     a.side_count = side_count.p, a.fast_c = fast_c.p, a.fast_slots = fast_slots.p, a.acc = acc.p;
     a.ovf_off = ovf_off.p, a.bucket_part = bucket_part.p;
@@ -2237,7 +2417,7 @@ extern "C" int gpl_pip_index_build(gpl_ctx *ctx, const gpl_array *polys, gpl_pip
     a.cell_cursor = cell_cursor.p, a.bcursor = bcursor.p, a.entry_edge = entry_edge.p;
     a.cells = idx->cells, a.cand01 = idx->cand01, a.items = idx->cell_overflow, a.parts = idx->parts;
     a.bucket_range = idx->bucket_range, a.entries = idx->entries, a.entry_ring = idx->entry_ring, a.fast = idx->fast;
-    a.raster = idx->raster, a.n_deferred = idx->n_deferred, a.phase_t = idx->phase_t;
+    a.raster = idx->raster, a.n_deferred = idx->n_deferred, a.phase_t = idx->phase_t, a.count_t = count_t.p;
     CUDAF(cudaMemsetAsync(idx->n_deferred, 0, 2 * sizeof(unsigned long long), st));
     {
         void *args[] = {&a};

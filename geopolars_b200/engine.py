@@ -517,6 +517,27 @@ class PipIndex:
         check(self.ctx.lib.gpl_pip_index_phases(self.ctx._h, self._h, _np_ptr(out)))
         return out[5:].tolist()
 
+    def timeline(self):
+        """microseconds from the start of the index count kernel to every build phase boundary (diagnostics): [0..4] count
+        kernel (start, after its three grid barriers, FP32 plan done), [5..11] fill kernel (start, after its barriers T0..T3,
+        cell records done, raster done)"""
+        out = np.zeros(12, dtype=np.float64)
+        check(self.ctx.lib.gpl_pip_index_timeline(self.ctx._h, self._h, _np_ptr(out)))
+        return out.tolist()
+
+    _DUMP_TABLES = {"raster": 0, "cand01": 1, "cells": 2, "parts": 3}
+
+    def dump(self, which: str) -> np.ndarray:
+        """read-only copy of one index table as raw bytes (uint8): "raster" (8 bytes per 16 fine cells), "cand01",
+        "cells" (32-byte records per coarse cell) or "parts" (32-byte records per part)"""
+        code = self._DUMP_TABLES[which]
+        n = C.c_int64(0)
+        check(self.ctx.lib.gpl_pip_index_dump(self.ctx._h, self._h, code, None, C.byref(n)))
+        out = np.empty(n.value, dtype=np.uint8)
+        if n.value:
+            check(self.ctx.lib.gpl_pip_index_dump(self.ctx._h, self._h, code, _np_ptr(out), C.byref(n)))
+        return out
+
     def query(self, points_xy: np.ndarray, with_count: bool = False):
         """first containing polygon row per point (-1 = none) [+ number of containing rows]."""
         pts = np.ascontiguousarray(points_xy, dtype=np.float64).reshape(-1, 2)

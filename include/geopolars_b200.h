@@ -255,6 +255,13 @@ int64_t gpl_pip_index_bytes(const gpl_pip_index *idx);
 int gpl_pip_index_stats(gpl_ctx *ctx, const gpl_pip_index *idx, int64_t *out8);
 /* diagnostics: microseconds from the start of the index fill kernel to each of its phase boundaries (out12[5..11]) */
 int gpl_pip_index_phases(gpl_ctx *ctx, const gpl_pip_index *idx, double *out12);
+/* diagnostics: microseconds from the start of the index COUNT kernel to each build phase boundary: out12[0..4] = the count
+ * kernel (start, after its three grid barriers, FP32 plan done), out12[5..11] = the fill kernel as above */
+int gpl_pip_index_timeline(gpl_ctx *ctx, const gpl_pip_index *idx, double *out12);
+/* diagnostics: read-only copy of one index table into host memory (synchronises the context stream).  which: 0 = raster
+ * words (8 bytes per 16 fine cells), 1 = cand01 (8 bytes per coarse cell), 2 = cell records (32 bytes per coarse cell),
+ * 3 = part records (32 bytes per part).  *nbytes: in = capacity of dst, out = size of the table; dst == NULL asks for the size. */
+int gpl_pip_index_dump(gpl_ctx *ctx, const gpl_pip_index *idx, int which, void *dst, int64_t *nbytes);
 /* spatial_join(points, polygons, Inner) candidate+exact test (spatial_index.rs:74-143):
  * first_id[p] = lowest polygon row containing point p, or -1; count[p] (may be NULL) = number of
  * containing rows.  points: xy interleaved, n points, in `mem`. */
