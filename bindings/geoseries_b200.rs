@@ -93,6 +93,8 @@ extern "C" {
     fn gpl_nearest_index_build(ctx: *mut GplCtx, rhs: *const GplArray, out: *mut *mut GplNearestIndex) -> c_int;
     fn gpl_nearest_index_free(idx: *mut GplNearestIndex);
     fn gpl_nearest_join_geom_pairs(ctx: *mut GplCtx, idx: *const GplNearestIndex, lhs: *const GplArray, max_distance: f64, out: *mut *mut GplPairs, distance: *mut f64, mem: c_int) -> c_int;
+    fn gpl_dwithin_join_pairs(ctx: *mut GplCtx, idx: *const GplNearestIndex, lhs: *const GplArray, distance: f64, with_distance: c_int, out: *mut *mut GplPairs) -> c_int;
+    fn gpl_pairs_copy_distance(ctx: *mut GplCtx, pairs: *const GplPairs, distance: *mut f64, mem: c_int) -> c_int;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -394,6 +396,10 @@ pub trait GeoSeriesB200Ext {
     /// unbounded), as (lhs_index, rhs_index, distance) sorted by (lhs, rhs); the distance is exactly what
     /// `self.distance(rhs)` computes for the pair
     fn nearest_join_pairs(&self, rhs: &Series, max_distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
+    /// distance-within join of this geometry column (any type) against any geometry column (GeoPandas'
+    /// `sjoin(predicate="dwithin", distance)`): every right row at distance <= `distance` (inclusive; finite and >= 0), as
+    /// (lhs_index, rhs_index, distance) sorted by (lhs, rhs); the distance is exactly what `self.distance(rhs)` computes
+    fn dwithin_join_pairs(&self, rhs: &Series, distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
 }
 
 impl GeoSeriesB200Ext for Series {
@@ -452,6 +458,32 @@ impl GeoSeriesB200Ext for Series {
         unsafe { gpl_pairs_free(pairs) };
         check(rc)?;
         let d = l.iter().map(|&i| dist[i as usize]).collect();
+        Ok((l, r, d))
+    }
+
+    fn dwithin_join_pairs(&self, rhs: &Series, distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let mut idx = std::ptr::null_mut();
+        check(unsafe { gpl_nearest_index_build(ctx, b.0, &mut idx) })?;
+        let mut pairs = std::ptr::null_mut();
+        let rc = unsafe { gpl_dwithin_join_pairs(ctx, idx, a.0, distance, 1, &mut pairs) };
+        unsafe { gpl_nearest_index_free(idx) };
+        if rc != 0 && !pairs.is_null() {
+            unsafe { gpl_pairs_free(pairs) };
+        }
+        check(rc)?;
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r, mut d) = (vec![0u64; n], vec![0u64; n], vec![0f64; n]);
+        let mut rc = 0;
+        if n > 0 {
+            rc = unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) };
+            if rc == 0 {
+                rc = unsafe { gpl_pairs_copy_distance(ctx, pairs, d.as_mut_ptr(), GPL_HOST) };
+            }
+        }
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
         Ok((l, r, d))
     }
 }

@@ -164,6 +164,9 @@ SIGNATURES = {
     "gpl_nearest_join_pairs_array": (_INT, [_P, _P, _P, _D, C.POINTER(_P), _P, _INT]),
     "gpl_nearest_join_geom": (_INT, [_P, _P, _P, _D, _P, _P, _P, _INT]),
     "gpl_nearest_join_geom_pairs": (_INT, [_P, _P, _P, _D, C.POINTER(_P), _P, _INT]),
+    "gpl_dwithin_count": (_INT, [_P, _P, _P, _D, _P, _INT]),
+    "gpl_dwithin_join_pairs": (_INT, [_P, _P, _P, _D, _INT, C.POINTER(_P)]),
+    "gpl_pairs_copy_distance": (_INT, [_P, _P, _P, _INT]),
     "gpl_gen_uniform_points": (_INT, [_P, C.c_uint64, _I64, _I64, _D, _P]),
     "gpl_gen_walk_linestrings": (_INT, [_P, C.c_uint64, _I64, _I64, _I64, C.c_int32, _P, _P]),
     "gpl_gen_blob_polygons": (_INT, [_P, C.c_uint64, _I64, _I64, C.c_int32, _P, _P, _P]),

@@ -127,10 +127,13 @@ struct gpl_array {
     int refcount = 1;
 };
 
-// result of a join (gpl_spatial_join, gpl_contains_join_pairs_array, gpl_nearest_join_pairs_array): (lhs, rhs) row pairs
+// result of a join (gpl_spatial_join, gpl_contains_join_pairs_array, gpl_nearest_join_pairs_array, gpl_dwithin_join_pairs):
+// (lhs, rhs) row pairs
 struct gpl_pairs {
     gpl_ctx *ctx = nullptr;
     uint64_t *lhs = nullptr, *rhs = nullptr;  // device
+    double *dist = nullptr;                   // device, the distance of each pair (gpl_dwithin_join_pairs with_distance only)
+    bool with_dist = false;                   // dist was asked for (it stays NULL when the list is empty)
     int64_t n = 0;
 };
 

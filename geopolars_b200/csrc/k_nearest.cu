@@ -24,6 +24,7 @@
 //     points have more than 256 candidates in all therefore sends some of them there (a speed cliff, not a wrong answer).
 // Pairs: the dense pass gives n_tied, a scan gives offsets, the same kernels in MODE 1 write the tied rows and
 // k_nearest_sort_pairs orders each point's rows.
+// The distance-within join (gpl_dwithin_*, DESIGN.md §4.14) queries the same index over a fixed window per left row.
 #include <math.h>
 #include <string.h>
 
@@ -737,6 +738,368 @@ static int check_geom_left(const gpl_array *lhs, double maxd) {
                 (long long)lhs->n_geoms);
     return check_query(lhs->n_geoms, maxd);
 }
+
+// ---- distance-within join (gpl_dwithin_*): every row of R within D of each left row, DESIGN.md §4.14 ------------------------
+// Kept in this file: it queries the nearest index through NearestView and reuses is_candidate, designated, row_distance,
+// geom_pair_distance and the left-row classification unchanged.  Instead of a ring search each left row walks a FIXED window:
+// the cells that can hold its box expanded by dw_margin(D, tau) on every side.  There is no overflow path: the walk runs in
+// warp-synchronous rounds, and a full queue is drained by the whole warp before the walk resumes.
+// MODE 0 writes the match count of each left row.  MODE 1 writes (rhs, d) into the row's slots [off[i], off[i+1]) in the
+// order they are found (k_dwithin_sort_* orders them) and adds to *bad each row whose write pass found a different number of
+// matches than its count pass; both passes evaluate the same pairs with the same routines, so the host treats bad != 0 as
+// an internal error.
+
+// Half-width of the window.  A row with computed lb <= D + tau has its designated cell at a coordinate within
+// lb * (1 + 4u) of the left box; the window edge fl(x - m) is within u * |x - m| of x - m.  (D + 2 tau)(1 + 2^-40) covers
+// both with tau to spare for any D (DESIGN.md §4.14 "Window").
+__device__ __forceinline__ double dw_margin(double D, double tau) { return (D + 2.0 * tau) * (1.0 + 0x1p-40); }
+
+// Point left side: persistent warps, one lane per point (k_nearest's tile loop and queue)
+template <int MODE>
+__global__ void __launch_bounds__(kNnWarps * 32) k_dwithin_pts(NearestView v, const double2 *__restrict__ pts, const uint8_t *__restrict__ pvalid,
+                                                              int64_t n, double D, int32_t *__restrict__ cnt, const int64_t *__restrict__ off,
+                                                              int32_t *__restrict__ raw_rhs, double *__restrict__ raw_d,
+                                                              unsigned long long *__restrict__ ctr, unsigned long long *__restrict__ bad) {
+    __shared__ int32_t s_row[kNnWarps][kNnQueue];
+    __shared__ uint8_t s_own[kNnWarps][kNnQueue];
+    __shared__ double2 s_pt[kNnWarps][32];
+    __shared__ int32_t s_cnt[kNnWarps][32];  // matches of each point so far (MODE 1: its next slot)
+    __shared__ int s_qn[kNnWarps];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int64_t nwarps = (int64_t)gridDim.x * kNnWarps;
+    const bool grid = v.jg.g > 0;
+    unsigned long long evals = 0;
+    int64_t t0 = ((int64_t)blockIdx.x * kNnWarps + wid) * 32;
+    double2 nxt = make_double2(0.0, 0.0);
+    if (t0 + lane < n) nxt = __ldcs(pts + t0 + lane);  // lane-contiguous: 512 B per warp-wide load
+    for (; t0 < n; t0 += nwarps * 32) {
+        const int64_t i = t0 + lane;
+        const double2 p = nxt;
+        if (t0 + nwarps * 32 + lane < n) nxt = __ldcs(pts + t0 + nwarps * 32 + lane);  // next tile in flight
+        const bool valid = i < n && bit_get(pvalid, i) && isfinite(p.x) && isfinite(p.y);
+        if (lane == 0) s_qn[wid] = 0;
+        s_pt[wid][lane] = p;
+        s_cnt[wid][lane] = 0;
+        __syncwarp();
+        // one evaluated pair, by one thread: count a match; MODE 1 also stores it in the owner's next slot
+        auto take = [&](int own, int32_t j, double d) {
+            if (!(d <= D)) return;
+            const int s = atomicAdd(&s_cnt[wid][own], 1);
+            if (MODE == 1) {
+                const int64_t b = off[t0 + own];
+                if (b + s < off[t0 + own + 1]) {
+                    raw_rhs[b + s] = j;
+                    if (raw_d) raw_d[b + s] = d;
+                }
+            }
+        };
+        // the everywhere rows, with the whole warp for each live point (never queued)
+        const unsigned live = __ballot_sync(0xffffffffu, valid);
+        for (int32_t e = 0; e < v.n_every; ++e) {
+            const int32_t j = v.every[e];
+            for (unsigned m = live; m; m &= m - 1) {
+                const int l = __ffs(m) - 1;
+                const double d = row_distance(v, j, s_pt[wid][l], lane);
+                if (lane == l) take(l, j, d), ++evals;
+            }
+        }
+        // the window, walked in rounds: each lane pushes its candidates until its window is done or the queue is full, the
+        // warp drains the queue, and the lanes resume where they stopped (the item that found the queue full is retried)
+        bool walking = valid && grid;
+        int32_t wx0 = 0, wx1 = 0, wy1 = 0, cx = 0, cy = 0, k = 0, k1 = 0;
+        double lim = 0.0;
+        if (walking) {
+            const double tau = slack(v, p), m = dw_margin(D, tau);
+            lim = D + tau;
+            wx0 = min(cell_x(v, p.x - m), v.gx - 1), wx1 = min(cell_x(v, p.x + m), v.gx - 1);
+            cy = min(cell_y(v, p.y - m), v.gy - 1), wy1 = min(cell_y(v, p.y + m), v.gy - 1);
+            cx = wx0;
+            const int64_t c = (int64_t)cy * v.jg.g + cx;
+            k = v.cell_start[c], k1 = v.cell_start[c + 1];
+        }
+        while (__any_sync(0xffffffffu, walking)) {
+            while (walking) {
+                if (k >= k1) {
+                    if (++cx > wx1) {
+                        cx = wx0;
+                        if (++cy > wy1) {
+                            walking = false;
+                            break;
+                        }
+                    }
+                    const int64_t c = (int64_t)cy * v.jg.g + cx;
+                    k = v.cell_start[c], k1 = v.cell_start[c + 1];
+                    continue;
+                }
+                if (is_candidate(v, k, p, lim, cx, cy)) {
+                    const int s = atomicAdd(&s_qn[wid], 1);
+                    if (s >= kNnQueue) break;  // full
+                    s_row[wid][s] = v.item_row[k], s_own[wid][s] = (uint8_t)lane;
+                }
+                ++k;
+            }
+            __syncwarp();
+            const int nq = min(s_qn[wid], kNnQueue);
+            if (lane_rows(v.type)) {
+                for (int e = lane; e < nq; e += 32) {
+                    const int own = s_own[wid][e];
+                    const int32_t j = s_row[wid][e];
+                    take(own, j, row_distance(v, j, s_pt[wid][own], lane));
+                    ++evals;
+                }
+            } else {
+                for (int e = 0; e < nq; ++e) {
+                    const int own = s_own[wid][e];
+                    const int32_t j = s_row[wid][e];
+                    const double d = row_distance(v, j, s_pt[wid][own], lane);
+                    if (lane == 0) take(own, j, d), ++evals;
+                }
+            }
+            __syncwarp();
+            if (lane == 0) s_qn[wid] = 0;
+            __syncwarp();
+        }
+        __syncwarp();
+        if (i < n) {
+            const int32_t got = s_cnt[wid][lane];
+            if (MODE == 0) cnt[i] = got;
+            else if (got != off[i + 1] - off[i]) atomicAdd(bad, 1ULL);
+        }
+        __syncwarp();  // s_pt / s_cnt are reused by the next tile
+    }
+    evals = (unsigned long long)warp_sum((double)evals);
+    if (lane == 0 && evals) atomicAdd(ctr, evals);
+}
+
+// any other left side: one warp per left row from an atomic cursor (k_nearest_geom's queue and dispatch)
+template <int MODE>
+__global__ void __launch_bounds__(kNgWarps * 32) k_dwithin_geom(NearestView v, Side L, const uint8_t *__restrict__ cls,
+                                                               const double *__restrict__ box4, int64_t n, double D, int32_t *__restrict__ cnt,
+                                                               const int64_t *__restrict__ off, int32_t *__restrict__ raw_rhs,
+                                                               double *__restrict__ raw_d, unsigned long long *__restrict__ ctr,
+                                                               unsigned long long *__restrict__ cursor, unsigned long long *__restrict__ bad) {
+    __shared__ int32_t s_row[kNgWarps][kNgQueue];
+    __shared__ double2 s_xy[kNgWarps][68];
+    __shared__ float4 s_box[kNgWarps][64];
+    __shared__ unsigned short s_q[kNgWarps][kPairQueue];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const LsLsScratch sc{s_xy[wid], s_box[wid], s_q[wid]};
+    unsigned long long evals = 0;
+    for (;;) {
+        unsigned long long t = 0;
+        if (lane == 0) t = atomicAdd(cursor, 1ULL);
+        const int64_t i = (int64_t)__shfl_sync(0xffffffffu, t, 0);
+        if (i >= n) break;
+        const uint8_t c = cls[i];
+        const int64_t b = MODE == 1 ? off[i] : 0, cap = MODE == 1 ? off[i + 1] - b : 0;
+        int64_t w = 0;  // matches so far (warp-uniform)
+        if (c != 0 && (MODE == 0 || cap > 0)) {
+            auto consider = [&](int32_t j) {  // warp-uniform
+                bool ok = true;
+                const double d = geom_pair_distance(L, i, v, j, sc, lane, ok);
+                ++evals;
+                if (!ok || !(d <= D)) return;
+                if (MODE == 1 && w < cap && lane == 0) {
+                    raw_rhs[b + w] = j;
+                    if (raw_d) raw_d[b + w] = d;
+                }
+                ++w;
+            };
+            for (int32_t e = 0; e < v.n_every; ++e) consider(v.every[e]);
+            if (v.jg.g > 0) {
+                const double lx0 = box4[4 * i], ly0 = box4[4 * i + 1], lx1 = box4[4 * i + 2], ly1 = box4[4 * i + 3];
+                const double tau = 0x1p-40 * fmax(v.M, fmax(fmax(fabs(lx0), fabs(ly0)), fmax(fabs(lx1), fabs(ly1))));
+                const double lim = D + tau, m = dw_margin(D, tau);
+                const bool prune = c == 1;  // irregular rows: every row of R
+                const int32_t lcx0 = cell_x(v, lx0), lcx1 = cell_x(v, lx1), lcy0 = cell_y(v, ly0), lcy1 = cell_y(v, ly1);
+                const int32_t wx0 = prune ? min(cell_x(v, lx0 - m), v.gx - 1) : 0, wx1 = prune ? min(cell_x(v, lx1 + m), v.gx - 1) : v.gx - 1;
+                const int32_t wy0 = prune ? min(cell_y(v, ly0 - m), v.gy - 1) : 0, wy1 = prune ? min(cell_y(v, ly1 + m), v.gy - 1) : v.gy - 1;
+                int qn = 0;  // warp-uniform
+                auto drain = [&]() {
+                    __syncwarp();
+                    for (int e = 0; e < qn; ++e) consider(s_row[wid][e]);
+                    qn = 0;
+                    __syncwarp();
+                };
+                for (int32_t cy = wy0; cy <= wy1; ++cy)
+                    for (int32_t cx = wx0; cx <= wx1; ++cx) {
+                        const int64_t cc = (int64_t)cy * v.jg.g + cx;
+                        const int32_t k0 = v.cell_start[cc], k1 = v.cell_start[cc + 1];
+                        for (int32_t kb = k0; kb < k1; kb += 32) {
+                            const int32_t k = kb + lane;
+                            bool cand = false;
+                            if (k < k1) {
+                                const double2 lo = v.recs[2 * (int64_t)k], hi = v.recs[2 * (int64_t)k + 1];
+                                cand = !prune || box_box_dist(lx0, ly0, lx1, ly1, lo.x, lo.y, hi.x, hi.y) <= lim;
+                                cand = cand && designated(cell_x(v, lo.x), cell_x(v, hi.x), lcx0, lcx1) == cx &&
+                                       designated(cell_y(v, lo.y), cell_y(v, hi.y), lcy0, lcy1) == cy;
+                            }
+                            const unsigned bm = __ballot_sync(0xffffffffu, cand);
+                            if (!bm) continue;
+                            if (qn + __popc(bm) > kNgQueue) drain();
+                            if (cand) s_row[wid][qn + __popc(bm & ((1u << lane) - 1u))] = v.item_row[k];
+                            qn += __popc(bm);
+                        }
+                    }
+                drain();
+            }
+        }
+        if (lane == 0) {
+            if (MODE == 0) cnt[i] = (int32_t)w;
+            else if (w != cap) atomicAdd(bad, 1ULL);
+        }
+    }
+    if (lane == 0 && evals) atomicAdd(ctr, evals);
+}
+
+// ---- per-row sort of the pair list by rhs, carrying d (the rows of a segment are distinct) -----------------------------------
+constexpr int kDwSortSmall = 256;  // segments up to this size are sorted on chip by one warp
+constexpr int kDwRadixThreads = 256;
+
+// one warp per segment of <= kDwSortSmall pairs: the row ids are staged in shared memory and each pair is written at its rank.
+// Larger segments are appended to big[] for k_dwithin_sort_large.
+__global__ void __launch_bounds__(256) k_dwithin_sort_small(int64_t n, const int64_t *__restrict__ off, const int32_t *__restrict__ raw,
+                                                            const double *__restrict__ raw_d, uint64_t *__restrict__ lhs,
+                                                            uint64_t *__restrict__ rhs, double *__restrict__ dist, int32_t *__restrict__ big,
+                                                            unsigned long long *__restrict__ n_big) {
+    __shared__ int32_t s_key[8][kDwSortSmall];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t i = warp; i < n; i += nwarps) {
+        const int64_t b = off[i], k = off[i + 1] - b;
+        if (k > kDwSortSmall) {
+            if (lane == 0) big[atomicAdd(n_big, 1ULL)] = (int32_t)i;
+            continue;
+        }
+        for (int q = lane; q < k; q += 32) s_key[wid][q] = raw[b + q];
+        __syncwarp();
+        for (int q = lane; q < k; q += 32) {
+            const int32_t j = s_key[wid][q];
+            int r = 0;
+            for (int t = 0; t < k; ++t) r += s_key[wid][t] < j;
+            lhs[b + r] = (uint64_t)i;
+            rhs[b + r] = (uint64_t)j;
+            if (dist) dist[b + r] = raw_d[b + q];
+        }
+        __syncwarp();
+    }
+}
+
+// one CTA per listed segment: a stable LSD radix sort of the row ids (< 2^31: four 8-bit digits), O(k) per segment, between
+// (raw, raw_d) and (tmp, tmp_d); the last pass scatters into the outputs.  Within a 256-pair tile a pair's place among equal
+// digits is its warp's offset plus its rank among the lanes of its warp with that digit (__match_any_sync), so the order of
+// equal digits is kept.
+__global__ void __launch_bounds__(kDwRadixThreads) k_dwithin_sort_large(const int32_t *__restrict__ big, int64_t n_big, const int64_t *__restrict__ off,
+                                                                       int32_t *__restrict__ raw, double *__restrict__ raw_d, int32_t *__restrict__ tmp,
+                                                                       double *__restrict__ tmp_d, uint64_t *__restrict__ lhs,
+                                                                       uint64_t *__restrict__ rhs, double *__restrict__ dist) {
+    constexpr int NW = kDwRadixThreads / 32;
+    __shared__ int32_t s_base[256];     // next place of each digit in this pass
+    __shared__ int32_t s_wcnt[NW][256];  // the tile's per-warp digit counts, then each warp's first place per digit
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    for (int64_t s = blockIdx.x; s < n_big; s += gridDim.x) {
+        const int64_t i = big[s], b = off[i], k = off[i + 1] - b;
+        for (int pass = 0; pass < 4; ++pass) {
+            const int shift = 8 * pass;
+            const int32_t *src = (pass & 1) ? tmp + b : raw + b;
+            const double *src_d = raw_d ? ((pass & 1) ? tmp_d + b : raw_d + b) : nullptr;
+            int32_t *dst = (pass & 1) ? raw + b : tmp + b;
+            double *dst_d = raw_d ? ((pass & 1) ? raw_d + b : tmp_d + b) : nullptr;
+            s_base[threadIdx.x] = 0;
+            __syncthreads();
+            for (int64_t q = threadIdx.x; q < k; q += kDwRadixThreads) atomicAdd(&s_base[(src[q] >> shift) & 255], 1);
+            __syncthreads();
+            if (threadIdx.x == 0)
+                for (int32_t d = 0, run = 0; d < 256; ++d) {
+                    const int32_t c = s_base[d];
+                    s_base[d] = run, run += c;
+                }
+            __syncthreads();
+            for (int64_t t0 = 0; t0 < k; t0 += kDwRadixThreads) {
+                const int64_t q = t0 + threadIdx.x;
+                const bool has = q < k;
+                const int32_t key = has ? src[q] : 0;
+                const int dg = has ? (key >> shift) & 255 : 256 + lane;  // absent pairs match nobody
+                for (int w = 0; w < NW; ++w) s_wcnt[w][threadIdx.x] = 0;
+                __syncthreads();
+                const unsigned peers = __match_any_sync(0xffffffffu, dg);
+                const int rank = __popc(peers & ((1u << lane) - 1u));
+                if (has && rank == 0) s_wcnt[wid][dg] = __popc(peers);
+                __syncthreads();
+                {
+                    int32_t run = s_base[threadIdx.x];  // thread d owns digit d
+                    for (int w = 0; w < NW; ++w) {
+                        const int32_t c = s_wcnt[w][threadIdx.x];
+                        s_wcnt[w][threadIdx.x] = run, run += c;
+                    }
+                    s_base[threadIdx.x] = run;
+                }
+                __syncthreads();
+                if (has) {
+                    const int32_t pos = s_wcnt[wid][dg] + rank;
+                    if (pass < 3) {
+                        dst[pos] = key;
+                        if (dst_d) dst_d[pos] = src_d[q];
+                    } else {
+                        lhs[b + pos] = (uint64_t)i;
+                        rhs[b + pos] = (uint64_t)key;
+                        if (dist) dist[b + pos] = src_d[q];
+                    }
+                }
+                __syncthreads();
+            }
+        }
+    }
+}
+
+static int check_dwithin(const gpl_array *lhs, double D) {
+    const int t = lhs->type;
+    GPL_REQUIRE(t == GPL_POINT || t == GPL_LINESTRING || t == GPL_POLYGON || t == GPL_MULTIPOINT || t == GPL_MULTILINESTRING ||
+                    t == GPL_MULTIPOLYGON,
+                GPL_ERR_INVALID_TYPE, "dwithin join: unsupported left geometry type %s", type_name_nn(t));
+    GPL_REQUIRE(lhs->n_geoms <= 0x7fffffffLL, GPL_ERR_UNSUPPORTED, "dwithin join: at most 2^31 - 1 left rows per call (got %lld)",
+                (long long)lhs->n_geoms);
+    GPL_REQUIRE(std::isfinite(D) && D >= 0.0, GPL_ERR_INVALID_ARG, "dwithin join: distance must be finite and >= 0 (got %g)", D);
+    return GPL_OK;
+}
+
+// one pass over the left rows (device buffers): a POINT column on k_dwithin_pts, any other on k_dwithin_geom (cls / box4 from
+// geom_classify).  MODE 0 (raw_rhs == NULL) writes cnt; MODE 1 writes the matches at off and fails when a row's write pass
+// disagrees with its count pass.
+static int dwithin_run(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, const uint8_t *cls, const double *box4, double D,
+                       int32_t *cnt, const int64_t *off, int32_t *raw_rhs, double *raw_d) {
+    GPL_CUDA(cudaMemsetAsync(idx->counters, 0, 2 * sizeof(unsigned long long), ctx->stream));
+    const int64_t n = lhs->n_geoms;
+    if (n == 0) return GPL_OK;
+    Scratch<unsigned long long> aux;  // [0] row cursor, [1] rows whose write pass disagreed with the count pass
+    GPL_TRY(aux.get(ctx, 2));
+    GPL_CUDA(cudaMemsetAsync(aux.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
+    const NearestView v = view_of(idx);
+    if (lhs->type == GPL_POINT) {
+        const double2 *pts = reinterpret_cast<const double2 *>(lhs->xy);
+        if (raw_rhs == nullptr)
+            GPL_LAUNCH(ctx, k_dwithin_pts<0>, nn_grid(n), kNnWarps * 32, 0, v, pts, lhs->validity, n, D, cnt, nullptr, nullptr, nullptr,
+                       idx->counters, aux.p + 1);
+        else
+            GPL_LAUNCH(ctx, k_dwithin_pts<1>, nn_grid(n), kNnWarps * 32, 0, v, pts, lhs->validity, n, D, nullptr, off, raw_rhs, raw_d,
+                       idx->counters, aux.p + 1);
+    } else {
+        const Side L{lhs->type, reinterpret_cast<const double2 *>(lhs->xy), lhs->geom_off, lhs->part_off, lhs->ring_off};
+        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, kNgWarps), (int64_t)kSMs * 8));
+        if (raw_rhs == nullptr)
+            GPL_LAUNCH(ctx, k_dwithin_geom<0>, grid, kNgWarps * 32, 0, v, L, cls, box4, n, D, cnt, nullptr, nullptr, nullptr, idx->counters,
+                       aux.p, aux.p + 1);
+        else
+            GPL_LAUNCH(ctx, k_dwithin_geom<1>, grid, kNgWarps * 32, 0, v, L, cls, box4, n, D, nullptr, off, raw_rhs, raw_d, idx->counters,
+                       aux.p, aux.p + 1);
+    }
+    unsigned long long bad = 0;
+    GPL_CUDA(cudaMemcpyAsync(&bad, aux.p + 1, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // aux returns to the cache when this scope ends
+    GPL_REQUIRE(bad == 0, GPL_ERR_CUDA, "dwithin join: the write pass found a different number of matches than the count pass on %llu rows",
+                bad);
+    return GPL_OK;
+}
 }  // namespace gpl
 
 using namespace gpl;
@@ -1063,5 +1426,81 @@ extern "C" int gpl_nearest_join_geom_pairs(gpl_ctx *ctx, const gpl_nearest_index
     GPL_LAUNCH(ctx, k_nearest_sort_pairs, (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 8), (int64_t)kSMs * 16)), 256, 0, n, off.p,
                raw.p, res->lhs, res->rhs);
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    return GPL_OK;
+}
+
+extern "C" int gpl_dwithin_count(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int32_t *count, int mem) {
+    GPL_REQUIRE(ctx && idx && lhs && (count || lhs->n_geoms == 0), GPL_ERR_INVALID_ARG, "gpl_dwithin_count: NULL argument");
+    GPL_TRY(check_dwithin(lhs, distance));
+    GPL_CUDA(cudaSetDevice(ctx->device));
+    const int64_t n = lhs->n_geoms;
+    Scratch<double> box4;
+    Scratch<uint8_t> cls;
+    Scratch<int32_t> dc;
+    if (n && lhs->type != GPL_POINT) GPL_TRY(geom_classify(ctx, lhs, box4, cls));
+    int32_t *out = count;
+    if (mem != GPL_DEVICE) {
+        GPL_TRY(dc.get(ctx, (size_t)n));
+        out = dc.p;
+    }
+    GPL_TRY(dwithin_run(ctx, idx, lhs, cls.p, box4.p, distance, out, nullptr, nullptr, nullptr));
+    if (mem != GPL_DEVICE) GPL_TRY(deliver(ctx, count, dc.p, sizeof(int32_t) * (size_t)n, mem));
+    return GPL_OK;
+}
+
+extern "C" int gpl_dwithin_join_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int with_distance,
+                                      gpl_pairs **out) {
+    GPL_REQUIRE(ctx && idx && lhs && out, GPL_ERR_INVALID_ARG, "gpl_dwithin_join_pairs: NULL argument");
+    GPL_TRY(check_dwithin(lhs, distance));
+    GPL_CUDA(cudaSetDevice(ctx->device));
+    gpl_pairs *res = new gpl_pairs();
+    res->ctx = ctx;
+    res->with_dist = with_distance != 0;
+    *out = res;
+    const int64_t n = lhs->n_geoms;
+    if (n == 0) return GPL_OK;
+    Scratch<double> box4, raw_d, tmp_d;
+    Scratch<uint8_t> cls;
+    Scratch<int32_t> cnt, raw, tmp, big;
+    Scratch<int64_t> off;
+    Scratch<unsigned long long> n_big;
+    if (lhs->type != GPL_POINT) GPL_TRY(geom_classify(ctx, lhs, box4, cls));
+    GPL_TRY(cnt.get(ctx, (size_t)n));
+    GPL_TRY(off.get(ctx, (size_t)n + 2));
+    GPL_TRY(dwithin_run(ctx, idx, lhs, cls.p, box4.p, distance, cnt.p, nullptr, nullptr, nullptr));
+    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n, off.p, off.p + n + 1)));
+    int64_t total = 0;
+    GPL_CUDA(cudaMemcpyAsync(&total, off.p + n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (total == 0) return GPL_OK;
+    GPL_TRY(raw.get(ctx, (size_t)total));
+    if (with_distance) GPL_TRY(raw_d.get(ctx, (size_t)total));
+    GPL_TRY(dwithin_run(ctx, idx, lhs, cls.p, box4.p, distance, nullptr, off.p, raw.p, raw_d.p));
+    void *pl = nullptr, *pr = nullptr, *pd = nullptr;
+    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pl));
+    res->lhs = (uint64_t *)pl;
+    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pr));
+    res->rhs = (uint64_t *)pr;
+    if (with_distance) {
+        GPL_TRY(ctx->alloc(sizeof(double) * (size_t)total, &pd));
+        res->dist = (double *)pd;
+    }
+    res->n = total;
+    // segments of more than kDwSortSmall pairs: at most total / (kDwSortSmall + 1) of them
+    GPL_TRY(big.get(ctx, (size_t)(total / (kDwSortSmall + 1) + 1)));
+    GPL_TRY(n_big.get(ctx, 1));
+    GPL_CUDA(cudaMemsetAsync(n_big.p, 0, sizeof(unsigned long long), ctx->stream));
+    GPL_LAUNCH(ctx, k_dwithin_sort_small, (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 8), (int64_t)kSMs * 16)), 256, 0, n, off.p,
+               raw.p, raw_d.p, res->lhs, res->rhs, res->dist, big.p, n_big.p);
+    unsigned long long h_big = 0;
+    GPL_CUDA(cudaMemcpyAsync(&h_big, n_big.p, sizeof(h_big), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (h_big > 0) {
+        GPL_TRY(tmp.get(ctx, (size_t)total));
+        if (with_distance) GPL_TRY(tmp_d.get(ctx, (size_t)total));
+        GPL_LAUNCH(ctx, k_dwithin_sort_large, (int)std::min<int64_t>((int64_t)h_big, (int64_t)kSMs * 8), kDwRadixThreads, 0, big.p, (int64_t)h_big,
+                   off.p, raw.p, raw_d.p, tmp.p, tmp_d.p, res->lhs, res->rhs, res->dist);
+    }
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
     return GPL_OK;
 }

@@ -817,9 +817,20 @@ extern "C" void gpl_pairs_free(gpl_pairs *p) {
     if (!p) return;
     p->ctx->release(p->lhs);
     p->ctx->release(p->rhs);
+    p->ctx->release(p->dist);
     delete p;
 }
 extern "C" int64_t gpl_pairs_count(const gpl_pairs *p) { return p ? p->n : 0; }
+extern "C" int gpl_pairs_copy_distance(gpl_ctx *ctx, const gpl_pairs *p, double *distance, int mem) {
+    GPL_REQUIRE(ctx && p && (p->n == 0 || distance), GPL_ERR_INVALID_ARG, "gpl_pairs_copy_distance: NULL argument");
+    GPL_REQUIRE(p->with_dist, GPL_ERR_INVALID_ARG, "gpl_pairs_copy_distance: this pair list carries no distances");
+    GPL_CUDA(cudaSetDevice(ctx->device));
+    if (p->n == 0) return GPL_OK;
+    const cudaMemcpyKind kind = mem == GPL_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+    GPL_CUDA(cudaMemcpyAsync(distance, p->dist, sizeof(double) * p->n, kind, ctx->stream));
+    if (mem == GPL_HOST) GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    return GPL_OK;
+}
 extern "C" int gpl_pairs_copy(gpl_ctx *ctx, const gpl_pairs *p, uint64_t *lhs, uint64_t *rhs, int mem) {
     GPL_REQUIRE(ctx && p && (p->n == 0 || (lhs && rhs)), GPL_ERR_INVALID_ARG, "gpl_pairs_copy: NULL argument");
     GPL_CUDA(cudaSetDevice(ctx->device));

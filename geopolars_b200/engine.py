@@ -691,6 +691,30 @@ class NearestIndex:
         lhs_rows, rhs_rows = _pairs_to_host(self.ctx, h)
         return (lhs_rows, rhs_rows, dist) if with_distance else (lhs_rows, rhs_rows)
 
+    def count_within(self, lhs: DeviceArray, distance: float) -> np.ndarray:
+        """number of right rows within `distance` (inclusive, finite, >= 0) of each left row of any geometry type (DESIGN.md
+        §4.14): int32 per left row; the distance of a pair is exactly what `distance(lhs, rhs)` returns for it"""
+        out = np.empty(len(lhs), dtype=np.int32)
+        check(self.ctx.lib.gpl_dwithin_count(self.ctx._h, self._h, lhs._h, float(distance), _np_ptr(out), GPL_HOST))
+        return out
+
+    def pairs_within(self, lhs: DeviceArray, distance: float, with_distance: bool = False):
+        """every (left row, right row) pair within `distance`, once, sorted by (lhs, rhs): (lhs uint64, rhs uint64[, d float64])"""
+        h = C.c_void_p()
+        check(self.ctx.lib.gpl_dwithin_join_pairs(self.ctx._h, self._h, lhs._h, float(distance), int(bool(with_distance)), C.byref(h)))
+        try:
+            n = int(self.ctx.lib.gpl_pairs_count(h))
+            a = np.empty(n, dtype=np.uint64)
+            b = np.empty(n, dtype=np.uint64)
+            d = np.empty(n, dtype=np.float64)
+            if n:
+                check(self.ctx.lib.gpl_pairs_copy(self.ctx._h, h, _np_ptr(a), _np_ptr(b), GPL_HOST))
+                if with_distance:
+                    check(self.ctx.lib.gpl_pairs_copy_distance(self.ctx._h, h, _np_ptr(d), GPL_HOST))
+        finally:
+            self.ctx.lib.gpl_pairs_free(h)
+        return (a, b, d) if with_distance else (a, b)
+
     def free(self) -> None:
         if getattr(self, "_h", None) and self.ctx._h:
             self.ctx.lib.gpl_nearest_index_free(self._h)

@@ -260,6 +260,11 @@ class GeoRustSeries:
         out, valid = E.distance(self._d(), other.device)
         return _f64(out, valid)
 
+    def dwithin(self, other: GeoSeries, distance: float):
+        """row-wise `distance(self, other) <= distance` (GeoPandas' GeoSeries.dwithin); a null distance gives False"""
+        out, valid = E.distance(self._d(), other.device)
+        return _pa().array(valid.astype(bool) & (out <= float(distance)))
+
     def translate(self, xoff: float = 0.0, yoff: float = 0.0) -> GeoSeries:
         return self._wrap(E.translate(self._d(), xoff, yoff))
 
@@ -336,6 +341,34 @@ def nearest_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", max_distanc
     d = dist[a]
     if how == "left":
         miss = np.nonzero(np.isnan(dist))[0]
+        a = np.concatenate([a, miss])
+        b = np.concatenate([b, np.full(len(miss), -1, dtype=np.int64)])
+        d = np.concatenate([d, np.full(len(miss), np.nan)])
+        order = np.lexsort((b, a))
+        a, b, d = a[order], b[order], d[order]
+    return a, b, d
+
+
+def dwithin_join(lhs: GeoSeries, rhs: GeoSeries, distance: float, how: str = "inner"):
+    """Distance-within join of any geometry column against any geometry column (GeoPandas' sjoin(predicate="dwithin",
+    distance=D)): (lhs_index int64, rhs_index int64, distance float64) for every right row whose distance to the left row is
+    <= `distance` (inclusive; finite and >= 0), sorted by (lhs, rhs).  The distance is exactly what `lhs.geo.distance`
+    computes for the pair, with the left row as the first operand; a null distance never matches.  Null left rows, and left
+    rows that are empty or have a non-finite coordinate, match nothing.  how='inner' -> matched left rows only; how='left' ->
+    unmatched left rows once, with rhs_index -1 and distance NaN (DESIGN.md §4.14)."""
+    if how not in ("inner", "left"):
+        raise ValueError("how must be 'inner' or 'left'")
+    idx = E.NearestIndex(rhs.device)
+    try:
+        a, b, d = idx.pairs_within(lhs.device, distance, with_distance=True)
+    finally:
+        idx.free()
+    a = a.astype(np.int64)
+    b = b.astype(np.int64)
+    if how == "left":
+        matched = np.zeros(len(lhs), dtype=bool)
+        matched[a] = True
+        miss = np.nonzero(~matched)[0]
         a = np.concatenate([a, miss])
         b = np.concatenate([b, np.full(len(miss), -1, dtype=np.int64)])
         d = np.concatenate([d, np.full(len(miss), np.nan)])

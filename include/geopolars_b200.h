@@ -317,7 +317,8 @@ void gpl_nearest_index_free(gpl_nearest_index *idx);
 /* synchronises the context stream: out8[0] = rows in R, [1] = excluded rows, [2] = rows every query evaluates (an empty
  * member, an empty ring or a 1-coordinate linestring / ring), [3] = grid cells per axis, [4] = cell items, [5] = index
  * bytes, [6] = exact distance evaluations of the last query pass, [7] = points the last query pass sent to the overflow
- * path.  [6] and [7] live in the index: gpl_nearest_join_pairs_array runs two passes and leaves the counts of its second,
+ * path.  The distance-within passes (gpl_dwithin_*) update [6] too and leave [7] at 0 (they have no overflow path).
+ * [6] and [7] live in the index: gpl_nearest_join_pairs_array runs two passes and leaves the counts of its second,
  * and queries of one index issued concurrently on different streams overwrite each other's counts (never their results). */
 int gpl_nearest_index_stats(gpl_ctx *ctx, const gpl_nearest_index *idx, int64_t *out8);
 /* dense form: nearest_id[i] = lowest tied row or -1, distance[i] (may be NULL) = its distance or NaN, n_tied[i] (may be
@@ -344,6 +345,24 @@ int gpl_nearest_join_geom(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_
                           double *distance, int32_t *n_tied, int mem);
 int gpl_nearest_join_geom_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double max_distance, gpl_pairs **out,
                                 double *distance, int mem);
+
+/* ---------------------------------------------------------------- distance-within join --- */
+/* Every row of R within `distance` of each left row (GeoPandas sjoin(predicate="dwithin", distance=D)), on a nearest index
+ * (DESIGN.md §4.14).  The eligible right rows R are those of the nearest index; a left row of any of the six types takes part
+ * only if it is non-null, has an envelope and only finite coordinates; no other row matches anything.  d(i, j) is exactly the
+ * f64 that gpl_distance(lhs, rhs) returns for the row pair, with lhs as the FIRST operand; a pair for which gpl_distance
+ * returns null never matches.  (i, j) matches when d(i, j) <= distance (inclusive).  distance must be finite and >= 0 (NaN,
+ * negative or +-inf -> GPL_ERR_INVALID_ARG); 0 means touching or intersecting, as `distance` computes it.  Fewer than 2^31
+ * left rows per call (else GPL_ERR_UNSUPPORTED); both checked before any launch or access.  A POINT left column runs one lane
+ * per point, any other type one warp per row.  Outputs are deterministic (two calls give byte-identical results). */
+/* count[i] (int32, in `mem`) = number of matching right rows of left row i */
+int gpl_dwithin_count(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int32_t *count, int mem);
+/* every matching pair once, sorted by (lhs, rhs), as a device-resident gpl_pairs (int64 total count); with_distance != 0
+ * also keeps d(i, j) of each pair (gpl_pairs_copy_distance) */
+int gpl_dwithin_join_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int with_distance,
+                           gpl_pairs **out);
+/* the distance of each pair of a list built with distances (any other list: GPL_ERR_INVALID_ARG); distance[n] in `mem` */
+int gpl_pairs_copy_distance(gpl_ctx *ctx, const gpl_pairs *pairs, double *distance, int mem);
 
 /* ---------------------------------------------------------------- synthetic data --------- */
 /* device-side generators, bit-identical to geopolars_b200/synth.py (SURVEY.md §8d RNG) */

@@ -4,7 +4,7 @@ fraction for the coordinate bytes read, and of the nearest join (100 M points ag
 reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
@@ -41,8 +41,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom"), default="all",
-                    help="run only the §8 rows, only the point nearest join or only the geometry nearest join")
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin"), default="all",
+                    help="run only the §8 rows, only the point nearest join, only the geometry nearest join or only the "
+                         "distance-within join")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
@@ -74,7 +75,9 @@ def main():
             nearest_rows(args, ctx, dev, st, res)
         if args.only in ("all", "nearest_geom"):
             nearest_geom_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom"):
+        if args.only in ("all", "dwithin"):
+            dwithin_rows(args, ctx, dev, st, res)
+        if args.only in ("nearest", "nearest_geom", "dwithin"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -310,6 +313,92 @@ def nearest_geom_rows(args, ctx, dev, st, res):
     res["rows"].append(r)
     print(json.dumps(r), flush=True)
     del lxy, loff, rxy
+    torch.cuda.empty_cache()
+
+
+def dwithin_rows(args, ctx, dev, st, res):
+    """distance-within join (DESIGN.md §4.14), kernel resident: build ms, count-pass ms (dense counts in HBM), pair-list ms
+    (device-resident gpl_pairs with distances, freed after each call), left rows/s, pairs/s, exact evaluations per left row of
+    the last pass and pairs returned; plus a cKDTree CPU arm for workload 1"""
+    import time
+
+    from geopolars_b200 import synth
+
+    lib = ctx.lib
+
+    def run(name, lhs, n_lhs, rhs, n_rhs, D):
+        tb = timed(st, lambda: E.NearestIndex(rhs).free(), reps=3, warm=1)
+        idx = E.NearestIndex(rhs)
+        cnt = torch.empty(max(n_lhs, 1), dtype=torch.int32, device=dev)
+        tc = timed(st, lambda: E.check(lib.gpl_dwithin_count(ctx._h, idx._h, lhs._h, D, C.c_void_p(cnt.data_ptr()), E.GPL_DEVICE)), reps=3, warm=1)
+        evals_count = idx.stats()["evaluations"]
+        n_pairs = [0]
+
+        def pairs():
+            h = C.c_void_p()
+            E.check(lib.gpl_dwithin_join_pairs(ctx._h, idx._h, lhs._h, D, 1, C.byref(h)))
+            n_pairs[0] = int(lib.gpl_pairs_count(h))
+            lib.gpl_pairs_free(h)
+
+        tp = timed(st, pairs, reps=3, warm=1)
+        s = idx.stats()
+        r = {"op": f"dwithin join: {name}, D = {D}", "left_rows": n_lhs, "rhs_rows": n_rhs, "distance": D, "build_ms_min": tb[0],
+             "count_ms_min": tc[0], "count_ms_avg": tc[1], "pairs_ms_min": tp[0], "pairs_ms_avg": tp[1],
+             "count_left_rows_per_s": n_lhs / (tc[1] * 1e-3), "pairs_left_rows_per_s": n_lhs / (tp[1] * 1e-3),
+             "pairs_per_s": n_pairs[0] / (tp[1] * 1e-3), "evals_per_left_row": evals_count / n_lhs,
+             "evals_per_left_row_write_pass": s["evaluations"] / n_lhs, "pairs": n_pairs[0], "total_count": int(cnt[:n_lhs].sum().item()),
+             "grid_cells_per_axis": s["grid_cells_per_axis"], "card": res["card"], "power_limit": res["power_limit"]}
+        idx.free()
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    NP, NR = int(10_000_000 * max(args.scale, 0.01)), int(1_000_000 * max(args.scale, 0.01))
+    lp = torch.empty((NP, 2), dtype=torch.float64, device=dev)
+    rp = torch.empty((NR, 2), dtype=torch.float64, device=dev)
+    E.check(lib.gpl_gen_uniform_points(ctx._h, 1, 0, NP, 1000.0, lp.data_ptr()))
+    E.check(lib.gpl_gen_uniform_points(ctx._h, 2, 0, NR, 1000.0, rp.data_ptr()))
+    left = ctx.wrap_device(GeometryType.POINT, NP, NP, lp.data_ptr(), keepalive=(lp,))
+    refs = ctx.wrap_device(GeometryType.POINT, NR, NR, rp.data_ptr(), keepalive=(rp,))
+    ctx.synchronize()
+    # 1: 10 M x 1 M uniform points, D = 1 (about pi matches per point)
+    run(f"{NP} uniform points x {NR} uniform points", left, NP, refs, NR, 1.0)
+    # 2: 10 M uniform points x config 2's 10 k 64-vertex polygons, D = 0.5
+    m, nv = 10_000, 64
+    xy, ro, go = synth.star_polygons(m, 100, 10.0, nv)
+    pxy, pro, pgo = (torch.from_numpy(a).to(dev) for a in (xy, ro, go))
+    polys = ctx.wrap_device(GeometryType.POLYGON, m, m * (nv + 1), pxy.data_ptr(), geom_off_ptr=pgo.data_ptr(), ring_off_ptr=pro.data_ptr(),
+                            n_rings=m, keepalive=(pxy, pro, pgo))
+    run(f"{NP} uniform points x config 2's 10 k 64-vertex polygons", left, NP, polys, m, 0.5)
+    # 3: 1 M 16-vertex walk linestrings x config 2's polygons, D = 1
+    K = 16
+    lxy = torch.empty((NR * K, 2), dtype=torch.float64, device=dev)
+    loff = torch.empty(NR + 1, dtype=torch.int64, device=dev)
+    E.check(lib.gpl_gen_walk_linestrings(ctx._h, 3, -1, 0, NR, K, lxy.data_ptr(), loff.data_ptr()))
+    lines = ctx.wrap_device(GeometryType.LINESTRING, NR, NR * K, lxy.data_ptr(), geom_off_ptr=loff.data_ptr(), keepalive=(lxy, loff))
+    ctx.synchronize()
+    run(f"{NR} {K}-vertex walk linestrings x config 2's polygons", lines, NR, polys, m, 1.0)
+    del lxy, loff, lines
+    # 4: workload 1 with the left side as one-member MultiPoint rows: the warp-per-row kernel on the same pairs
+    moff = torch.arange(NP + 1, dtype=torch.int64, device=dev)
+    mleft = ctx.wrap_device(GeometryType.MULTIPOINT, NP, NP, lp.data_ptr(), geom_off_ptr=moff.data_ptr(), keepalive=(lp, moff))
+    ctx.synchronize()
+    run(f"{NP} one-member MultiPoint rows x {NR} uniform points", mleft, NP, refs, NR, 1.0)
+    # CPU arm of workload 1: scipy's cKDTree.query_ball_point on every core of this host, on a prefix of the left points
+    from scipy.spatial import cKDTree
+
+    k = min(NP, 2_000_000)
+    L, R = lp[:k].cpu().numpy(), rp.cpu().numpy()
+    t0 = time.perf_counter()
+    tree = cKDTree(R)
+    t1 = time.perf_counter()
+    nb = tree.query_ball_point(L, 1.0, workers=-1, return_length=True)
+    t2 = time.perf_counter()
+    r = {"op": f"dwithin join CPU arm: scipy cKDTree.query_ball_point(workers=-1, return_length=True), {k}-point prefix of workload 1",
+         "left_rows": k, "nproc": os.cpu_count(), "build_s": t1 - t0, "query_s": t2 - t1, "left_rows_per_s": k / (t2 - t1),
+         "pairs": int(nb.sum()), "pairs_per_s": int(nb.sum()) / (t2 - t1)}
+    res["rows"].append(r)
+    print(json.dumps(r), flush=True)
+    del lp, rp, pxy, pro, pgo, moff
     torch.cuda.empty_cache()
 
 
