@@ -7,6 +7,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <algorithm>
 #include <map>
 #include <mutex>
 #include <string>
@@ -45,6 +46,24 @@ int cuda_fail(cudaError_t e, const char *what, const char *file, int line);
 constexpr int kSMs = 132;  // H100 SXM
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// CTAs for one warp per row, at most 16 per SM (the warps stride over the remaining rows)
+static int warp_grid(int64_t rows, int warps_per_cta) {
+    int64_t want = ceil_div(rows, warps_per_cta);
+    return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * 16));
+}
+
+static const char *type_name(int t) {
+    switch (t) {
+    case GPL_POINT: return "Point";
+    case GPL_LINESTRING: return "LineString";
+    case GPL_POLYGON: return "Polygon";
+    case GPL_MULTIPOINT: return "MultiPoint";
+    case GPL_MULTILINESTRING: return "MultiLineString";
+    case GPL_MULTIPOLYGON: return "MultiPolygon";
+    default: return "Unknown";
+    }
+}
 
 }  // namespace gpl
 

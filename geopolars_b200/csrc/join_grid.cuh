@@ -3,7 +3,12 @@
 // envelope overlaps.
 #pragma once
 
+#include <string.h>
+
+#include <cmath>
+
 #include "common.cuh"
+#include "scan.cuh"
 
 namespace gpl {
 
@@ -47,6 +52,60 @@ __global__ void k_join_cells(const double *__restrict__ b4, const uint8_t *__res
             if (PASS == 0) atomicAdd(&count_or_cursor[c], 1);
             else items[atomicAdd(&count_or_cursor[c], 1)] = (int32_t)i;
         }
+}
+
+// A built grid: the union box, the grid (g == 0 when no envelope is listed), and the cell lists (cell c holds
+// items[cell_start[c] .. cell_start[c + 1]), G * G + 1 offsets and n_items + 1 entries).
+struct GridBuild {
+    double ux0 = 0.0, uy0 = 0.0, ux1 = 0.0, uy1 = 0.0;
+    JoinGrid jg{0.0, 0.0, 0.0, 0.0, 0};
+    int64_t n_items = 0;
+    Scratch<int32_t> cell_start, items;
+};
+
+// The grid over the envelopes b4[i] with has[i] of n rows.  G = ceil(sqrt(n_g)) capped at 2048; a box without width
+// (height) gets inv_w = 0 (inv_h = 0), so every x (y) maps to cell 0.  More than 2^31 - 1 cell items: GPL_ERR_UNSUPPORTED
+// with the message "<what>: grid too dense".
+static int join_grid_build(gpl_ctx *ctx, const double *b4, const uint8_t *has, int64_t n, int64_t n_g, const char *what, GridBuild &out) {
+    Scratch<unsigned long long> acc;
+    GPL_TRY(acc.get(ctx, 4));
+    GPL_CUDA(cudaMemsetAsync(acc.p, 0, 4 * sizeof(unsigned long long), ctx->stream));
+    GPL_LAUNCH(ctx, k_join_union, (int)std::min<int64_t>(ceil_div(n, 256), kSMs * 8), 256, 0, b4, has, n, acc.p);
+    unsigned long long h_acc[4];
+    GPL_CUDA(cudaMemcpyAsync(h_acc, acc.p, sizeof(h_acc), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (h_acc[2] == 0ULL) return GPL_OK;  // no envelope listed
+    auto dec = [](unsigned long long u) {  // the inverse of k_join_union's order-preserving encoding
+        const unsigned long long b = (u >> 63) ? (u & 0x7fffffffffffffffULL) : ~u;
+        double d;
+        memcpy(&d, &b, sizeof(d));
+        return d;
+    };
+    out.ux0 = dec(~h_acc[0]), out.uy0 = dec(~h_acc[1]), out.ux1 = dec(h_acc[2]), out.uy1 = dec(h_acc[3]);
+    JoinGrid &jg = out.jg;
+    jg.g = (int32_t)std::min<int64_t>(2048, std::max<int64_t>(1, (int64_t)ceil(sqrt((double)n_g))));
+    jg.x0 = out.ux0, jg.y0 = out.uy0;
+    const double w = out.ux1 - out.ux0, h = out.uy1 - out.uy0;
+    jg.inv_w = (w > 0.0 && std::isfinite(w) && std::isfinite(jg.g / w)) ? jg.g / w : 0.0;
+    jg.inv_h = (h > 0.0 && std::isfinite(h) && std::isfinite(jg.g / h)) ? jg.g / h : 0.0;
+    const int64_t n_cells = (int64_t)jg.g * jg.g;
+    Scratch<int32_t> cell_count;
+    Scratch<int64_t> tot;
+    GPL_TRY(cell_count.get(ctx, (size_t)n_cells + 1));
+    GPL_TRY(out.cell_start.get(ctx, (size_t)n_cells + 1));
+    GPL_TRY(tot.get(ctx, 1));
+    GPL_CUDA(cudaMemsetAsync(cell_count.p, 0, sizeof(int32_t) * (n_cells + 1), ctx->stream));
+    GPL_LAUNCH(ctx, k_join_cells<0>, (int)ceil_div(n, 128), 128, 0, b4, has, n, jg, cell_count.p, nullptr);
+    GPL_TRY((exclusive_scan<int32_t, int32_t>(ctx, cell_count.p, n_cells, out.cell_start.p, tot.p)));
+    int64_t n_items = 0;
+    GPL_CUDA(cudaMemcpyAsync(&n_items, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    GPL_REQUIRE(n_items < (1LL << 31), GPL_ERR_UNSUPPORTED, "%s: grid too dense (%lld cell items)", what, (long long)n_items);
+    out.n_items = n_items;
+    GPL_TRY(out.items.get(ctx, (size_t)n_items + 1));
+    GPL_CUDA(cudaMemcpyAsync(cell_count.p, out.cell_start.p, sizeof(int32_t) * n_cells, cudaMemcpyDeviceToDevice, ctx->stream));  // cursors
+    GPL_LAUNCH(ctx, k_join_cells<1>, (int)ceil_div(n, 128), 128, 0, b4, has, n, jg, cell_count.p, out.items.p);
+    return GPL_OK;
 }
 
 }  // namespace gpl

@@ -22,14 +22,14 @@
 //   overflow: the queue is shared by the warp's 32 points; a lane whose push finds it full is flagged and
 //     k_nearest_overflow redoes that point with one warp, streaming the candidates instead of queueing them.  A warp whose
 //     points have more than 256 candidates in all therefore sends some of them there (a speed cliff, not a wrong answer).
-// Pairs: the dense pass gives n_tied, a scan gives offsets, the same kernels in MODE 1 write the tied rows and
-// k_nearest_sort_pairs orders each point's rows.
+// Pairs (pair_list): the dense pass gives n_tied, a scan gives offsets, the same kernels in MODE 1 write the tied rows and
+// k_sort_rows_* order each point's rows.
 // The distance-within join (gpl_dwithin_*, DESIGN.md §4.14) queries the same index over a fixed window per left row.
 #include <math.h>
-#include <string.h>
 
 #include <algorithm>
 #include <cmath>
+#include <memory>
 
 #include "common.cuh"
 #include "join_grid.cuh"
@@ -187,6 +187,10 @@ __device__ __forceinline__ double box_dist(double2 p, double x0, double y0, doub
 }
 __device__ __forceinline__ double slack(const NearestView &v, double2 p) {
     return 0x1p-40 * fmax(v.M, fmax(fabs(p.x), fabs(p.y)));
+}
+// tau of a left box (DESIGN.md §4.13 "Slack")
+__device__ __forceinline__ double box_slack(const NearestView &v, double lx0, double ly0, double lx1, double ly1) {
+    return 0x1p-40 * fmax(v.M, fmax(fmax(fabs(lx0), fabs(ly0)), fmax(fabs(lx1), fabs(ly1))));
 }
 __device__ __forceinline__ int32_t cell_x(const NearestView &v, double x) { return jg_cell(x, v.jg.x0, v.jg.inv_w, v.jg.g); }
 __device__ __forceinline__ int32_t cell_y(const NearestView &v, double y) { return jg_cell(y, v.jg.y0, v.jg.inv_h, v.jg.g); }
@@ -428,39 +432,72 @@ __global__ void __launch_bounds__(256) k_nearest_overflow(NearestView v, const d
     }
 }
 
-// each point's tied rows in ascending order: rank sort of the segment (rows of a point are distinct)
-__global__ void __launch_bounds__(256) k_nearest_sort_pairs(int64_t n, const int64_t *__restrict__ off, const int32_t *__restrict__ raw,
-                                                            uint64_t *__restrict__ lhs, uint64_t *__restrict__ rhs) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    for (int64_t i = warp; i < n; i += nwarps) {
-        const int64_t b = off[i], e = off[i + 1];
-        for (int64_t k = b + lane; k < e; k += 32) {
-            const int32_t j = raw[k];
-            int64_t rank = 0;
-            for (int64_t m = b; m < e; ++m) rank += raw[m] < j;
-            lhs[b + rank] = (uint64_t)i;
-            rhs[b + rank] = (uint64_t)j;
-        }
-    }
-}
-
-static const char *type_name_nn(int t) {
-    switch (t) {
-    case GPL_POINT: return "Point";
-    case GPL_LINESTRING: return "LineString";
-    case GPL_POLYGON: return "Polygon";
-    case GPL_MULTIPOINT: return "MultiPoint";
-    case GPL_MULTILINESTRING: return "MultiLineString";
-    case GPL_MULTIPOLYGON: return "MultiPolygon";
-    default: return "Unknown";
-    }
-}
-
 int envelope_raw(gpl_ctx *ctx, const gpl_array *in, double *out4_dev, uint8_t *valid_bytes_dev);
 int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
 
 static int nn_grid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, kNnWarps * 32), (int64_t)kSMs * 8)); }
+
+// a column of one of the six types with at most 2^31 - 1 rows (row ids are int32); `per` follows "rows" in the message
+static int check_column(const gpl_array *a, const char *join, const char *side, const char *per) {
+    const int t = a->type;
+    GPL_REQUIRE(t == GPL_POINT || t == GPL_LINESTRING || t == GPL_POLYGON || t == GPL_MULTIPOINT || t == GPL_MULTILINESTRING ||
+                    t == GPL_MULTIPOLYGON,
+                GPL_ERR_INVALID_TYPE, "%s: unsupported %s geometry type %s", join, side, type_name(t));
+    GPL_REQUIRE(a->n_geoms <= 0x7fffffffLL, GPL_ERR_UNSUPPORTED, "%s: at most 2^31 - 1 %s rows%s (got %lld)", join, side, per,
+                (long long)a->n_geoms);
+    return GPL_OK;
+}
+
+// the classes, boxes and representative vertices of a column's rows (k_nearest_classify), and the number of grid and everywhere
+// rows; the right side of the index and the left side of a query are classified alike
+struct RowClasses {
+    Scratch<double> box4;
+    Scratch<double2> rep;
+    Scratch<uint8_t> cls, grid_has;
+    int64_t n_grid = 0, n_every = 0;
+};
+static int classify_rows(gpl_ctx *ctx, const gpl_array *a, RowClasses &rc) {
+    const int64_t n = a->n_geoms;
+    Scratch<double> env4;
+    Scratch<uint8_t> has;
+    Scratch<unsigned long long> cnt;
+    GPL_TRY(env4.get(ctx, (size_t)n * 4));
+    GPL_TRY(rc.box4.get(ctx, (size_t)n * 4));
+    GPL_TRY(has.get(ctx, (size_t)n));
+    GPL_TRY(rc.cls.get(ctx, (size_t)n));
+    GPL_TRY(rc.grid_has.get(ctx, (size_t)n));
+    GPL_TRY(rc.rep.get(ctx, (size_t)n));
+    GPL_TRY(cnt.get(ctx, 2));
+    GPL_CUDA(cudaMemsetAsync(cnt.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
+    GPL_TRY(envelope_raw(ctx, a, env4.p, has.p));
+    GPL_LAUNCH(ctx, k_nearest_classify, (int)ceil_div(n, 256), 256, 0, a->type, n, reinterpret_cast<const double2 *>(a->xy), a->geom_off,
+               a->part_off, a->ring_off, a->validity, has.p, rc.box4.p, rc.rep.p, rc.cls.p, rc.grid_has.p, cnt.p);
+    unsigned long long h[2];
+    GPL_CUDA(cudaMemcpyAsync(h, cnt.p, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // env4 / has / cnt return to the cache when this scope ends
+    rc.n_grid = (int64_t)h[0], rc.n_every = (int64_t)h[1];
+    return GPL_OK;
+}
+
+// The dense outputs of a nearest pass: run(nid, dist, ntied) fills device buffers (dist / ntied may be NULL).  Outputs in host
+// memory are filled through scratch.
+template <class Run>
+static int dense_outputs(gpl_ctx *ctx, int64_t n, int mem, int32_t *nid, double *dist, int32_t *ntied, Run &&run) {
+    if (mem == GPL_DEVICE) return run(nid, dist, ntied);
+    Scratch<double> dd;
+    Scratch<int32_t> di, dt;
+    GPL_TRY(di.get(ctx, (size_t)n));
+    if (dist) GPL_TRY(dd.get(ctx, (size_t)n));
+    if (ntied) GPL_TRY(dt.get(ctx, (size_t)n));
+    GPL_TRY(run(di.p, dd.p, dt.p));
+    if (n) {
+        GPL_CUDA(cudaMemcpyAsync(nid, di.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+        if (dist) GPL_CUDA(cudaMemcpyAsync(dist, dd.p, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
+        if (ntied) GPL_CUDA(cudaMemcpyAsync(ntied, dt.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    return GPL_OK;
+}
 
 // one pass over the points (device buffers).  MODE 0 fills nid / dist / ntied; MODE 1 writes raw_rhs at off.
 static int nearest_run(gpl_ctx *ctx, const gpl_nearest_index *idx, const double2 *pts, const uint8_t *pvalid, int64_t n, double maxd,
@@ -470,7 +507,7 @@ static int nearest_run(gpl_ctx *ctx, const gpl_nearest_index *idx, const double2
     Scratch<uint8_t> flag;
     GPL_TRY(flag.get(ctx, (size_t)n));
     const NearestView v = view_of(idx);
-    const int ogrid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(ceil_div(n, 32), 8), (int64_t)kSMs * 16));
+    const int ogrid = warp_grid(ceil_div(n, 32), 8);  // one warp per 32-point block
     if (raw_rhs == nullptr) {
         GPL_LAUNCH(ctx, k_nearest<0>, nn_grid(n), kNnWarps * 32, 0, v, pts, pvalid, n, maxd, nid, dist, ntied, nullptr, nullptr, flag.p,
                    idx->counters);
@@ -498,6 +535,7 @@ static int check_query(int64_t n, double maxd) {
 // of all their coordinates.
 constexpr int kNgWarps = 4;     // warps per CTA
 constexpr int kNgQueue = 128;   // queued right rows per warp (a full queue is drained and the walk continues)
+static int ng_grid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, kNgWarps), (int64_t)kSMs * 8)); }
 
 // member views of a Multi* column (k_pairs.cu gpl_distance): MultiPoint -> POINT over coordinates, MultiLineString ->
 // LINESTRING over rings, MultiPolygon -> POLYGON over parts; a single type is its own view
@@ -623,7 +661,7 @@ __global__ void __launch_bounds__(kNgWarps * 32) k_nearest_geom(NearestView v, S
             for (int32_t e = 0; e < v.n_every; ++e) consider(v.every[e]);
             if (v.jg.g > 0) {
                 const double lx0 = box4[4 * i], ly0 = box4[4 * i + 1], lx1 = box4[4 * i + 2], ly1 = box4[4 * i + 3];
-                const double tau = 0x1p-40 * fmax(v.M, fmax(fmax(fabs(lx0), fabs(ly0)), fmax(fabs(lx1), fabs(ly1))));
+                const double tau = box_slack(v, lx0, ly0, lx1, ly1);
                 const bool prune = c == 1;  // irregular rows: every row of R
                 const int32_t lcx0 = cell_x(v, lx0), lcx1 = cell_x(v, lx1), lcy0 = cell_y(v, ly0), lcy1 = cell_y(v, ly1);
                 int qn = 0;  // warp-uniform
@@ -684,28 +722,6 @@ __global__ void __launch_bounds__(kNgWarps * 32) k_nearest_geom(NearestView v, S
     if (lane == 0 && evals) atomicAdd(ctr, evals);
 }
 
-// the left column's classes and boxes (k_nearest_classify, as for the right rows)
-static int geom_classify(gpl_ctx *ctx, const gpl_array *lhs, Scratch<double> &box4, Scratch<uint8_t> &cls) {
-    const int64_t n = lhs->n_geoms;
-    Scratch<double> env4;
-    Scratch<uint8_t> has, ghas;
-    Scratch<double2> rep;
-    Scratch<unsigned long long> cnt;
-    GPL_TRY(env4.get(ctx, (size_t)n * 4));
-    GPL_TRY(box4.get(ctx, (size_t)n * 4));
-    GPL_TRY(has.get(ctx, (size_t)n));
-    GPL_TRY(cls.get(ctx, (size_t)n));
-    GPL_TRY(ghas.get(ctx, (size_t)n));
-    GPL_TRY(rep.get(ctx, (size_t)n));
-    GPL_TRY(cnt.get(ctx, 2));
-    GPL_CUDA(cudaMemsetAsync(cnt.p, 0, 2 * sizeof(unsigned long long), ctx->stream));
-    GPL_TRY(envelope_raw(ctx, lhs, env4.p, has.p));
-    GPL_LAUNCH(ctx, k_nearest_classify, (int)ceil_div(n, 256), 256, 0, lhs->type, n, reinterpret_cast<const double2 *>(lhs->xy), lhs->geom_off,
-               lhs->part_off, lhs->ring_off, lhs->validity, has.p, box4.p, rep.p, cls.p, ghas.p, cnt.p);
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // env4 / has / ghas / rep / cnt return to the cache when this scope ends
-    return GPL_OK;
-}
-
 // one pass over the left rows (device buffers).  MODE 0 (raw_rhs == NULL) fills nid / dist / ntied; MODE 1 writes the rows at
 // dist_in[i] into raw_rhs at off.
 static int geom_run(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, const uint8_t *cls, const double *box4, double maxd,
@@ -718,34 +734,28 @@ static int geom_run(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array 
     GPL_CUDA(cudaMemsetAsync(cursor.p, 0, sizeof(unsigned long long), ctx->stream));
     const NearestView v = view_of(idx);
     const Side L{lhs->type, reinterpret_cast<const double2 *>(lhs->xy), lhs->geom_off, lhs->part_off, lhs->ring_off};
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, kNgWarps), (int64_t)kSMs * 8));
     if (raw_rhs == nullptr)
-        GPL_LAUNCH(ctx, k_nearest_geom<0>, grid, kNgWarps * 32, 0, v, L, cls, box4, n, maxd, nid, dist, ntied, nullptr, nullptr, nullptr,
+        GPL_LAUNCH(ctx, k_nearest_geom<0>, ng_grid(n), kNgWarps * 32, 0, v, L, cls, box4, n, maxd, nid, dist, ntied, nullptr, nullptr, nullptr,
                    idx->counters, cursor.p);
     else
-        GPL_LAUNCH(ctx, k_nearest_geom<1>, grid, kNgWarps * 32, 0, v, L, cls, box4, n, maxd, nullptr, nullptr, nullptr, dist_in, off, raw_rhs,
-                   idx->counters, cursor.p);
+        GPL_LAUNCH(ctx, k_nearest_geom<1>, ng_grid(n), kNgWarps * 32, 0, v, L, cls, box4, n, maxd, nullptr, nullptr, nullptr, dist_in, off,
+                   raw_rhs, idx->counters, cursor.p);
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the cursor returns to the cache when this scope ends
     return GPL_OK;
 }
 
 static int check_geom_left(const gpl_array *lhs, double maxd) {
-    const int t = lhs->type;
-    GPL_REQUIRE(t == GPL_POINT || t == GPL_LINESTRING || t == GPL_POLYGON || t == GPL_MULTIPOINT || t == GPL_MULTILINESTRING ||
-                    t == GPL_MULTIPOLYGON,
-                GPL_ERR_INVALID_TYPE, "nearest join: unsupported left geometry type %s", type_name_nn(t));
-    GPL_REQUIRE(lhs->n_geoms <= 0x7fffffffLL, GPL_ERR_UNSUPPORTED, "nearest join: at most 2^31 - 1 left rows per call (got %lld)",
-                (long long)lhs->n_geoms);
+    GPL_TRY(check_column(lhs, "nearest join", "left", " per call"));
     return check_query(lhs->n_geoms, maxd);
 }
 
 // ---- distance-within join (gpl_dwithin_*): every row of R within D of each left row, DESIGN.md §4.14 ------------------------
 // Kept in this file: it queries the nearest index through NearestView and reuses is_candidate, designated, row_distance,
-// geom_pair_distance and the left-row classification unchanged.  Instead of a ring search each left row walks a FIXED window:
+// geom_pair_distance, the left-row classification and the pair-list pipeline unchanged.  Instead of a ring search each left row walks a FIXED window:
 // the cells that can hold its box expanded by dw_margin(D, tau) on every side.  There is no overflow path: the walk runs in
 // warp-synchronous rounds, and a full queue is drained by the whole warp before the walk resumes.
 // MODE 0 writes the match count of each left row.  MODE 1 writes (rhs, d) into the row's slots [off[i], off[i+1]) in the
-// order they are found (k_dwithin_sort_* orders them) and adds to *bad each row whose write pass found a different number of
+// order they are found (k_sort_rows_* orders them) and adds to *bad each row whose write pass found a different number of
 // matches than its count pass; both passes evaluate the same pairs with the same routines, so the host treats bad != 0 as
 // an internal error.
 
@@ -908,7 +918,7 @@ __global__ void __launch_bounds__(kNgWarps * 32) k_dwithin_geom(NearestView v, S
             for (int32_t e = 0; e < v.n_every; ++e) consider(v.every[e]);
             if (v.jg.g > 0) {
                 const double lx0 = box4[4 * i], ly0 = box4[4 * i + 1], lx1 = box4[4 * i + 2], ly1 = box4[4 * i + 3];
-                const double tau = 0x1p-40 * fmax(v.M, fmax(fmax(fabs(lx0), fabs(ly0)), fmax(fabs(lx1), fabs(ly1))));
+                const double tau = box_slack(v, lx0, ly0, lx1, ly1);
                 const double lim = D + tau, m = dw_margin(D, tau);
                 const bool prune = c == 1;  // irregular rows: every row of R
                 const int32_t lcx0 = cell_x(v, lx0), lcx1 = cell_x(v, lx1), lcy0 = cell_y(v, ly0), lcy1 = cell_y(v, ly1);
@@ -952,22 +962,22 @@ __global__ void __launch_bounds__(kNgWarps * 32) k_dwithin_geom(NearestView v, S
     if (lane == 0 && evals) atomicAdd(ctr, evals);
 }
 
-// ---- per-row sort of the pair list by rhs, carrying d (the rows of a segment are distinct) -----------------------------------
-constexpr int kDwSortSmall = 256;  // segments up to this size are sorted on chip by one warp
-constexpr int kDwRadixThreads = 256;
+// ---- per-row sort of a pair list by rhs, carrying d when raw_d != NULL (the rows of a segment are distinct) -----------------
+constexpr int kSortSmall = 256;  // segments up to this size are sorted on chip by one warp
+constexpr int kSortRadixThreads = 256;
 
-// one warp per segment of <= kDwSortSmall pairs: the row ids are staged in shared memory and each pair is written at its rank.
-// Larger segments are appended to big[] for k_dwithin_sort_large.
-__global__ void __launch_bounds__(256) k_dwithin_sort_small(int64_t n, const int64_t *__restrict__ off, const int32_t *__restrict__ raw,
-                                                            const double *__restrict__ raw_d, uint64_t *__restrict__ lhs,
-                                                            uint64_t *__restrict__ rhs, double *__restrict__ dist, int32_t *__restrict__ big,
-                                                            unsigned long long *__restrict__ n_big) {
-    __shared__ int32_t s_key[8][kDwSortSmall];
+// one warp per segment of <= kSortSmall pairs: the row ids are staged in shared memory and each pair is written at its rank.
+// Larger segments are appended to big[] for k_sort_rows_large.
+__global__ void __launch_bounds__(256) k_sort_rows_small(int64_t n, const int64_t *__restrict__ off, const int32_t *__restrict__ raw,
+                                                         const double *__restrict__ raw_d, uint64_t *__restrict__ lhs,
+                                                         uint64_t *__restrict__ rhs, double *__restrict__ dist, int32_t *__restrict__ big,
+                                                         unsigned long long *__restrict__ n_big) {
+    __shared__ int32_t s_key[8][kSortSmall];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t i = warp; i < n; i += nwarps) {
         const int64_t b = off[i], k = off[i + 1] - b;
-        if (k > kDwSortSmall) {
+        if (k > kSortSmall) {
             if (lane == 0) big[atomicAdd(n_big, 1ULL)] = (int32_t)i;
             continue;
         }
@@ -989,11 +999,11 @@ __global__ void __launch_bounds__(256) k_dwithin_sort_small(int64_t n, const int
 // (raw, raw_d) and (tmp, tmp_d); the last pass scatters into the outputs.  Within a 256-pair tile a pair's place among equal
 // digits is its warp's offset plus its rank among the lanes of its warp with that digit (__match_any_sync), so the order of
 // equal digits is kept.
-__global__ void __launch_bounds__(kDwRadixThreads) k_dwithin_sort_large(const int32_t *__restrict__ big, int64_t n_big, const int64_t *__restrict__ off,
+__global__ void __launch_bounds__(kSortRadixThreads) k_sort_rows_large(const int32_t *__restrict__ big, int64_t n_big, const int64_t *__restrict__ off,
                                                                        int32_t *__restrict__ raw, double *__restrict__ raw_d, int32_t *__restrict__ tmp,
                                                                        double *__restrict__ tmp_d, uint64_t *__restrict__ lhs,
                                                                        uint64_t *__restrict__ rhs, double *__restrict__ dist) {
-    constexpr int NW = kDwRadixThreads / 32;
+    constexpr int NW = kSortRadixThreads / 32;
     __shared__ int32_t s_base[256];     // next place of each digit in this pass
     __shared__ int32_t s_wcnt[NW][256];  // the tile's per-warp digit counts, then each warp's first place per digit
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -1007,7 +1017,7 @@ __global__ void __launch_bounds__(kDwRadixThreads) k_dwithin_sort_large(const in
             double *dst_d = raw_d ? ((pass & 1) ? raw_d + b : tmp_d + b) : nullptr;
             s_base[threadIdx.x] = 0;
             __syncthreads();
-            for (int64_t q = threadIdx.x; q < k; q += kDwRadixThreads) atomicAdd(&s_base[(src[q] >> shift) & 255], 1);
+            for (int64_t q = threadIdx.x; q < k; q += kSortRadixThreads) atomicAdd(&s_base[(src[q] >> shift) & 255], 1);
             __syncthreads();
             if (threadIdx.x == 0)
                 for (int32_t d = 0, run = 0; d < 256; ++d) {
@@ -1015,7 +1025,7 @@ __global__ void __launch_bounds__(kDwRadixThreads) k_dwithin_sort_large(const in
                     s_base[d] = run, run += c;
                 }
             __syncthreads();
-            for (int64_t t0 = 0; t0 < k; t0 += kDwRadixThreads) {
+            for (int64_t t0 = 0; t0 < k; t0 += kSortRadixThreads) {
                 const int64_t q = t0 + threadIdx.x;
                 const bool has = q < k;
                 const int32_t key = has ? src[q] : 0;
@@ -1052,19 +1062,68 @@ __global__ void __launch_bounds__(kDwRadixThreads) k_dwithin_sort_large(const in
     }
 }
 
+// A pair list of n left rows: count(cnt) writes each left row's number of pairs, a scan turns the counts into int64 offsets,
+// write(off, raw, raw_d) writes each row's right rows (and, when raw_d != NULL, their distances) at its offsets in any order,
+// and k_sort_rows_* order each row's pairs by rhs.  The right rows of one left row are distinct, so the sorted list does not
+// depend on the order of the write pass.
+template <class Count, class Write>
+static int pair_list(gpl_ctx *ctx, int64_t n, bool with_dist, gpl_pairs **out, Count &&count, Write &&write) {
+    gpl_pairs *res = new gpl_pairs();
+    res->ctx = ctx;
+    res->with_dist = with_dist;
+    *out = res;
+    if (n == 0) return GPL_OK;
+    Scratch<double> raw_d, tmp_d;
+    Scratch<int32_t> cnt, raw, tmp, big;
+    Scratch<int64_t> off;
+    Scratch<unsigned long long> n_big;
+    GPL_TRY(cnt.get(ctx, (size_t)n));
+    GPL_TRY(off.get(ctx, (size_t)n + 2));
+    GPL_TRY(count(cnt.p));
+    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n, off.p, off.p + n + 1)));
+    int64_t total = 0;
+    GPL_CUDA(cudaMemcpyAsync(&total, off.p + n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (total == 0) return GPL_OK;
+    GPL_TRY(raw.get(ctx, (size_t)total));
+    if (with_dist) GPL_TRY(raw_d.get(ctx, (size_t)total));
+    GPL_TRY(write(off.p, raw.p, raw_d.p));
+    void *pl = nullptr, *pr = nullptr, *pd = nullptr;
+    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pl));
+    res->lhs = (uint64_t *)pl;
+    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pr));
+    res->rhs = (uint64_t *)pr;
+    if (with_dist) {
+        GPL_TRY(ctx->alloc(sizeof(double) * (size_t)total, &pd));
+        res->dist = (double *)pd;
+    }
+    res->n = total;
+    // segments of more than kSortSmall pairs: at most total / (kSortSmall + 1) of them
+    GPL_TRY(big.get(ctx, (size_t)(total / (kSortSmall + 1) + 1)));
+    GPL_TRY(n_big.get(ctx, 1));
+    GPL_CUDA(cudaMemsetAsync(n_big.p, 0, sizeof(unsigned long long), ctx->stream));
+    GPL_LAUNCH(ctx, k_sort_rows_small, warp_grid(n, 8), 256, 0, n, off.p, raw.p, raw_d.p, res->lhs, res->rhs, res->dist, big.p, n_big.p);
+    unsigned long long h_big = 0;
+    GPL_CUDA(cudaMemcpyAsync(&h_big, n_big.p, sizeof(h_big), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (h_big > 0) {
+        GPL_TRY(tmp.get(ctx, (size_t)total));
+        if (with_dist) GPL_TRY(tmp_d.get(ctx, (size_t)total));
+        GPL_LAUNCH(ctx, k_sort_rows_large, (int)std::min<int64_t>((int64_t)h_big, (int64_t)kSMs * 8), kSortRadixThreads, 0, big.p,
+                   (int64_t)h_big, off.p, raw.p, raw_d.p, tmp.p, tmp_d.p, res->lhs, res->rhs, res->dist);
+    }
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
+    return GPL_OK;
+}
+
 static int check_dwithin(const gpl_array *lhs, double D) {
-    const int t = lhs->type;
-    GPL_REQUIRE(t == GPL_POINT || t == GPL_LINESTRING || t == GPL_POLYGON || t == GPL_MULTIPOINT || t == GPL_MULTILINESTRING ||
-                    t == GPL_MULTIPOLYGON,
-                GPL_ERR_INVALID_TYPE, "dwithin join: unsupported left geometry type %s", type_name_nn(t));
-    GPL_REQUIRE(lhs->n_geoms <= 0x7fffffffLL, GPL_ERR_UNSUPPORTED, "dwithin join: at most 2^31 - 1 left rows per call (got %lld)",
-                (long long)lhs->n_geoms);
+    GPL_TRY(check_column(lhs, "dwithin join", "left", " per call"));
     GPL_REQUIRE(std::isfinite(D) && D >= 0.0, GPL_ERR_INVALID_ARG, "dwithin join: distance must be finite and >= 0 (got %g)", D);
     return GPL_OK;
 }
 
 // one pass over the left rows (device buffers): a POINT column on k_dwithin_pts, any other on k_dwithin_geom (cls / box4 from
-// geom_classify).  MODE 0 (raw_rhs == NULL) writes cnt; MODE 1 writes the matches at off and fails when a row's write pass
+// classify_rows).  MODE 0 (raw_rhs == NULL) writes cnt; MODE 1 writes the matches at off and fails when a row's write pass
 // disagrees with its count pass.
 static int dwithin_run(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, const uint8_t *cls, const double *box4, double D,
                        int32_t *cnt, const int64_t *off, int32_t *raw_rhs, double *raw_d) {
@@ -1085,12 +1144,11 @@ static int dwithin_run(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_arr
                        idx->counters, aux.p + 1);
     } else {
         const Side L{lhs->type, reinterpret_cast<const double2 *>(lhs->xy), lhs->geom_off, lhs->part_off, lhs->ring_off};
-        const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, kNgWarps), (int64_t)kSMs * 8));
         if (raw_rhs == nullptr)
-            GPL_LAUNCH(ctx, k_dwithin_geom<0>, grid, kNgWarps * 32, 0, v, L, cls, box4, n, D, cnt, nullptr, nullptr, nullptr, idx->counters,
+            GPL_LAUNCH(ctx, k_dwithin_geom<0>, ng_grid(n), kNgWarps * 32, 0, v, L, cls, box4, n, D, cnt, nullptr, nullptr, nullptr, idx->counters,
                        aux.p, aux.p + 1);
         else
-            GPL_LAUNCH(ctx, k_dwithin_geom<1>, grid, kNgWarps * 32, 0, v, L, cls, box4, n, D, nullptr, off, raw_rhs, raw_d, idx->counters,
+            GPL_LAUNCH(ctx, k_dwithin_geom<1>, ng_grid(n), kNgWarps * 32, 0, v, L, cls, box4, n, D, nullptr, off, raw_rhs, raw_d, idx->counters,
                        aux.p, aux.p + 1);
     }
     unsigned long long bad = 0;
@@ -1118,133 +1176,67 @@ extern "C" void gpl_nearest_index_free(gpl_nearest_index *idx) {
 
 extern "C" int gpl_nearest_index_build(gpl_ctx *ctx, const gpl_array *rhs, gpl_nearest_index **out) {
     GPL_REQUIRE(ctx && rhs && out, GPL_ERR_INVALID_ARG, "gpl_nearest_index_build: NULL argument");
-    const int t = rhs->type;
-    GPL_REQUIRE(t == GPL_POINT || t == GPL_LINESTRING || t == GPL_POLYGON || t == GPL_MULTIPOINT || t == GPL_MULTILINESTRING ||
-                    t == GPL_MULTIPOLYGON,
-                GPL_ERR_INVALID_TYPE, "nearest join: unsupported right geometry type %s", type_name_nn(t));
-    GPL_REQUIRE(rhs->n_geoms < (1LL << 31), GPL_ERR_UNSUPPORTED, "nearest join: at most 2^31 - 1 right rows (got %lld)",
-                (long long)rhs->n_geoms);
+    GPL_TRY(check_column(rhs, "nearest join", "right", ""));
     GPL_CUDA(cudaSetDevice(ctx->device));
-    gpl_nearest_index *idx = new gpl_nearest_index();
-    idx->ctx = ctx, idx->type = t, idx->xy = reinterpret_cast<const double2 *>(rhs->xy);
+    // freed on every early return; released to the caller at the end
+    std::unique_ptr<gpl_nearest_index, void (*)(gpl_nearest_index *)> idx(new gpl_nearest_index(), gpl_nearest_index_free);
+    idx->ctx = ctx, idx->type = rhs->type, idx->xy = reinterpret_cast<const double2 *>(rhs->xy);
     idx->go = rhs->geom_off, idx->po = rhs->part_off, idx->ro = rhs->ring_off;
     const int64_t n = rhs->n_geoms;
     idx->n_rows = n;
-    auto fail = [&](int rc) {
-        gpl_nearest_index_free(idx);
-        return rc;
-    };
-#define TRYF(expr)                             \
-    do {                                       \
-        int rc__ = (expr);                     \
-        if (rc__ != GPL_OK) return fail(rc__); \
-    } while (0)
-#define CUDAF(expr)                                                                     \
-    do {                                                                                \
-        cudaError_t e__ = (expr);                                                       \
-        if (e__ != cudaSuccess) return fail(cuda_fail(e__, #expr, __FILE__, __LINE__)); \
-    } while (0)
-    {
-        void *p = nullptr;
-        TRYF(ctx->alloc(2 * sizeof(unsigned long long), &p));
-        idx->counters = (unsigned long long *)p;
-        CUDAF(cudaMemsetAsync(idx->counters, 0, 2 * sizeof(unsigned long long), ctx->stream));
-    }
+    Scratch<unsigned long long> counters;
+    GPL_TRY(counters.get(ctx, 2));
+    idx->counters = counters.take();
+    GPL_CUDA(cudaMemsetAsync(idx->counters, 0, 2 * sizeof(unsigned long long), ctx->stream));
     if (n == 0) {
-        CUDAF(cudaStreamSynchronize(ctx->stream));
-        *out = idx;
+        GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+        *out = idx.release();
         return GPL_OK;
     }
-    Scratch<double> env4, box4;
-    Scratch<uint8_t> has, cls, ghas;
-    Scratch<double2> rep;
-    Scratch<unsigned long long> cnt;
-    TRYF(env4.get(ctx, (size_t)n * 4));
-    TRYF(box4.get(ctx, (size_t)n * 4));
-    TRYF(has.get(ctx, (size_t)n));
-    TRYF(cls.get(ctx, (size_t)n));
-    TRYF(ghas.get(ctx, (size_t)n));
-    TRYF(rep.get(ctx, (size_t)n));
-    TRYF(cnt.get(ctx, 8));
-    CUDAF(cudaMemsetAsync(cnt.p, 0, 8 * sizeof(unsigned long long), ctx->stream));
-    TRYF(envelope_raw(ctx, rhs, env4.p, has.p));
-    GPL_LAUNCH(ctx, k_nearest_classify, (int)ceil_div(n, 256), 256, 0, t, n, idx->xy, idx->go, idx->po, idx->ro, rhs->validity, has.p, box4.p,
-               rep.p, cls.p, ghas.p, cnt.p);
-    unsigned long long h[2];
-    CUDAF(cudaMemcpyAsync(h, cnt.p, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-    CUDAF(cudaStreamSynchronize(ctx->stream));
-    const int64_t n_grid = (int64_t)h[0];
-    idx->n_every = (int64_t)h[1];
-    idx->n_r = n_grid + idx->n_every;
+    RowClasses rc;
+    GPL_TRY(classify_rows(ctx, rhs, rc));
+    idx->n_every = rc.n_every;
+    idx->n_r = rc.n_grid + rc.n_every;
     size_t bytes = 2 * sizeof(unsigned long long);
     if (idx->n_every > 0) {
-        void *p = nullptr;
-        TRYF(ctx->alloc(sizeof(int32_t) * (size_t)idx->n_every, &p));
-        idx->every = (int32_t *)p;
+        Scratch<int32_t> every;
+        Scratch<unsigned long long> cursor;
+        GPL_TRY(every.get(ctx, (size_t)idx->n_every));
+        idx->every = every.take();
         bytes += sizeof(int32_t) * (size_t)idx->n_every;
-        GPL_LAUNCH(ctx, k_nearest_every, (int)ceil_div(n, 256), 256, 0, cls.p, n, cnt.p + 2, idx->every);
+        GPL_TRY(cursor.get(ctx, 1));
+        GPL_CUDA(cudaMemsetAsync(cursor.p, 0, sizeof(unsigned long long), ctx->stream));
+        GPL_LAUNCH(ctx, k_nearest_every, (int)ceil_div(n, 256), 256, 0, rc.cls.p, n, cursor.p, idx->every);
     }
-    if (n_grid > 0) {
-        // ---- the grid over the union box of the grid rows' boxes (same G rule as gpl_spatial_join) ----------------------------
-        unsigned long long *acc = cnt.p + 4;
-        GPL_LAUNCH(ctx, k_join_union, (int)std::min<int64_t>(ceil_div(n, 256), kSMs * 8), 256, 0, box4.p, ghas.p, n, acc);
-        unsigned long long ha[4];
-        CUDAF(cudaMemcpyAsync(ha, acc, sizeof(ha), cudaMemcpyDeviceToHost, ctx->stream));
-        CUDAF(cudaStreamSynchronize(ctx->stream));
-        auto dec = [](unsigned long long u) {
-            const unsigned long long b = (u >> 63) ? (u & 0x7fffffffffffffffULL) : ~u;
-            double d;
-            memcpy(&d, &b, sizeof(d));
-            return d;
-        };
-        idx->ux0 = dec(~ha[0]), idx->uy0 = dec(~ha[1]), idx->ux1 = dec(ha[2]), idx->uy1 = dec(ha[3]);
-        JoinGrid &jg = idx->jg;
-        jg.g = (int32_t)std::min<int64_t>(2048, std::max<int64_t>(1, (int64_t)ceil(sqrt((double)idx->n_r))));
-        jg.x0 = idx->ux0, jg.y0 = idx->uy0;
-        const double w = idx->ux1 - idx->ux0, hh = idx->uy1 - idx->uy0;
-        jg.inv_w = (w > 0.0 && std::isfinite(w) && std::isfinite(jg.g / w)) ? jg.g / w : 0.0;
-        jg.inv_h = (hh > 0.0 && std::isfinite(hh) && std::isfinite(jg.g / hh)) ? jg.g / hh : 0.0;
+    if (rc.n_grid > 0) {
+        // the grid over the union box of the grid rows' boxes, G from all rows of R
+        GridBuild grid;
+        GPL_TRY(join_grid_build(ctx, rc.box4.p, rc.grid_has.p, n, idx->n_r, "nearest join", grid));
+        const JoinGrid &jg = idx->jg = grid.jg;
+        idx->ux0 = grid.ux0, idx->uy0 = grid.uy0, idx->ux1 = grid.ux1, idx->uy1 = grid.uy1;
         // a box without width (height) maps every x (y) to cell 0: the search then has one column (row)
         idx->gx = jg.inv_w == 0.0 ? 1 : jg.g;
         idx->gy = jg.inv_h == 0.0 ? 1 : jg.g;
-        idx->cw = w / jg.g, idx->ch = hh / jg.g;
+        idx->cw = (idx->ux1 - idx->ux0) / jg.g, idx->ch = (idx->uy1 - idx->uy0) / jg.g;
         idx->M = std::max(std::max(std::fabs(idx->ux0), std::fabs(idx->uy0)), std::max(std::fabs(idx->ux1), std::fabs(idx->uy1)));
-        const int64_t n_cells = (int64_t)jg.g * jg.g;
-        Scratch<int32_t> cell_count, items;
-        Scratch<int64_t> tot;
-        TRYF(cell_count.get(ctx, (size_t)n_cells + 1));
-        TRYF(tot.get(ctx, 1));
-        void *p = nullptr;
-        TRYF(ctx->alloc(sizeof(int32_t) * ((size_t)n_cells + 1), &p));
-        idx->cell_start = (int32_t *)p;
-        bytes += sizeof(int32_t) * ((size_t)n_cells + 1);
-        CUDAF(cudaMemsetAsync(cell_count.p, 0, sizeof(int32_t) * (n_cells + 1), ctx->stream));
-        GPL_LAUNCH(ctx, k_join_cells<0>, (int)ceil_div(n, 128), 128, 0, box4.p, ghas.p, n, jg, cell_count.p, nullptr);
-        TRYF((exclusive_scan<int32_t, int32_t>(ctx, cell_count.p, n_cells, idx->cell_start, tot.p)));
-        int64_t n_items = 0;
-        CUDAF(cudaMemcpyAsync(&n_items, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        CUDAF(cudaStreamSynchronize(ctx->stream));
-        GPL_REQUIRE(n_items < (1LL << 31), fail(GPL_ERR_UNSUPPORTED), "nearest join: grid too dense (%lld cell items)", (long long)n_items);
-        idx->n_items = n_items;
-        TRYF(ctx->alloc(sizeof(int32_t) * ((size_t)n_items + 1), &p));
-        idx->item_row = (int32_t *)p;
-        TRYF(ctx->alloc(sizeof(double2) * 2 * ((size_t)n_items + 1), &p));
-        idx->recs = (double2 *)p;
-        TRYF(ctx->alloc(sizeof(double2) * ((size_t)n_items + 1), &p));
-        idx->item_rep = (double2 *)p;
+        const int64_t n_items = idx->n_items = grid.n_items;
+        idx->cell_start = grid.cell_start.take();
+        idx->item_row = grid.items.take();
+        bytes += sizeof(int32_t) * ((size_t)jg.g * jg.g + 1);
+        Scratch<double2> recs, item_rep;
+        GPL_TRY(recs.get(ctx, 2 * ((size_t)n_items + 1)));
+        idx->recs = recs.take();
+        GPL_TRY(item_rep.get(ctx, (size_t)n_items + 1));
+        idx->item_rep = item_rep.take();
         bytes += (size_t)n_items * (sizeof(int32_t) + 3 * sizeof(double2));
-        CUDAF(cudaMemcpyAsync(cell_count.p, idx->cell_start, sizeof(int32_t) * n_cells, cudaMemcpyDeviceToDevice, ctx->stream));  // cursors
-        GPL_LAUNCH(ctx, k_join_cells<1>, (int)ceil_div(n, 128), 128, 0, box4.p, ghas.p, n, jg, cell_count.p, idx->item_row);
         if (n_items > 0)
-            GPL_LAUNCH(ctx, k_nearest_records, (int)ceil_div(n_items, 256), 256, 0, idx->item_row, n_items, box4.p, rep.p, idx->recs,
+            GPL_LAUNCH(ctx, k_nearest_records, (int)ceil_div(n_items, 256), 256, 0, idx->item_row, n_items, rc.box4.p, rc.rep.p, idx->recs,
                        idx->item_rep);
     }
     idx->bytes = (int64_t)bytes;
-    CUDAF(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
-    *out = idx;
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
+    *out = idx.release();
     return GPL_OK;
-#undef TRYF
-#undef CUDAF
 }
 
 extern "C" int gpl_nearest_index_stats(gpl_ctx *ctx, const gpl_nearest_index *idx, int64_t *out8) {
@@ -1271,95 +1263,53 @@ extern "C" int gpl_nearest_join(gpl_ctx *ctx, const gpl_nearest_index *idx, cons
     GPL_TRY(check_query(n_points, max_distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const double2 *pts = reinterpret_cast<const double2 *>(points_xy);
-    if (mem == GPL_DEVICE) {
-        GPL_TRY(nearest_run(ctx, idx, pts, nullptr, n_points, max_distance, nearest_id, distance, n_tied, nullptr, nullptr));
-        return GPL_OK;
+    Scratch<double2> dp;
+    if (mem != GPL_DEVICE) {  // the points are in the caller's memory too
+        GPL_TRY(dp.get(ctx, (size_t)n_points));
+        if (n_points) GPL_CUDA(cudaMemcpyAsync(dp.p, points_xy, sizeof(double2) * n_points, cudaMemcpyHostToDevice, ctx->stream));
+        pts = dp.p;
     }
-    const size_t n = (size_t)n_points;
-    Scratch<double> dp, dd;
-    Scratch<int32_t> di, dt;
-    GPL_TRY(dp.get(ctx, n * 2));
-    GPL_TRY(di.get(ctx, n));
-    if (distance) GPL_TRY(dd.get(ctx, n));
-    if (n_tied) GPL_TRY(dt.get(ctx, n));
-    if (n) GPL_CUDA(cudaMemcpyAsync(dp.p, points_xy, sizeof(double) * 2 * n, cudaMemcpyHostToDevice, ctx->stream));
-    GPL_TRY(nearest_run(ctx, idx, reinterpret_cast<const double2 *>(dp.p), nullptr, n_points, max_distance, di.p, distance ? dd.p : nullptr,
-                        n_tied ? dt.p : nullptr, nullptr, nullptr));
-    if (n) {
-        GPL_CUDA(cudaMemcpyAsync(nearest_id, di.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-        if (distance) GPL_CUDA(cudaMemcpyAsync(distance, dd.p, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
-        if (n_tied) GPL_CUDA(cudaMemcpyAsync(n_tied, dt.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    return GPL_OK;
+    return dense_outputs(ctx, n_points, mem, nearest_id, distance, n_tied, [&](int32_t *nid, double *dist, int32_t *ntied) {
+        return nearest_run(ctx, idx, pts, nullptr, n_points, max_distance, nid, dist, ntied, nullptr, nullptr);
+    });
 }
 
 extern "C" int gpl_nearest_join_array(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *points, double max_distance,
                                       int32_t *nearest_id, double *distance, int32_t *n_tied, int mem) {
     GPL_REQUIRE(ctx && idx && points && nearest_id, GPL_ERR_INVALID_ARG, "gpl_nearest_join_array: NULL argument");
     GPL_REQUIRE(points->type == GPL_POINT, GPL_ERR_INVALID_TYPE, "nearest join: the left side must be Point (found %s)",
-                type_name_nn(points->type));
+                type_name(points->type));
     GPL_TRY(check_query(points->n_geoms, max_distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
-    const int64_t n = points->n_geoms;
     const double2 *pts = reinterpret_cast<const double2 *>(points->xy);
-    if (mem == GPL_DEVICE) return nearest_run(ctx, idx, pts, points->validity, n, max_distance, nearest_id, distance, n_tied, nullptr, nullptr);
-    Scratch<double> dd;
-    Scratch<int32_t> di, dt;
-    GPL_TRY(di.get(ctx, (size_t)n));
-    if (distance) GPL_TRY(dd.get(ctx, (size_t)n));
-    if (n_tied) GPL_TRY(dt.get(ctx, (size_t)n));
-    GPL_TRY(nearest_run(ctx, idx, pts, points->validity, n, max_distance, di.p, distance ? dd.p : nullptr, n_tied ? dt.p : nullptr, nullptr,
-                        nullptr));
-    if (n) {
-        GPL_CUDA(cudaMemcpyAsync(nearest_id, di.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-        if (distance) GPL_CUDA(cudaMemcpyAsync(distance, dd.p, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
-        if (n_tied) GPL_CUDA(cudaMemcpyAsync(n_tied, dt.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    return GPL_OK;
+    return dense_outputs(ctx, points->n_geoms, mem, nearest_id, distance, n_tied, [&](int32_t *nid, double *dist, int32_t *ntied) {
+        return nearest_run(ctx, idx, pts, points->validity, points->n_geoms, max_distance, nid, dist, ntied, nullptr, nullptr);
+    });
 }
 
 extern "C" int gpl_nearest_join_pairs_array(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *points, double max_distance,
                                             gpl_pairs **out, double *distance, int mem) {
     GPL_REQUIRE(ctx && idx && points && out, GPL_ERR_INVALID_ARG, "gpl_nearest_join_pairs_array: NULL argument");
     GPL_REQUIRE(points->type == GPL_POINT, GPL_ERR_INVALID_TYPE, "nearest join: the left side must be Point (found %s)",
-                type_name_nn(points->type));
+                type_name(points->type));
     GPL_TRY(check_query(points->n_geoms, max_distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
-    gpl_pairs *res = new gpl_pairs();
-    res->ctx = ctx;
-    *out = res;
     const int64_t n = points->n_geoms;
-    if (n == 0) return GPL_OK;
     const double2 *pts = reinterpret_cast<const double2 *>(points->xy);
-    Scratch<int32_t> ids, cnt, raw;
-    Scratch<double> dist;
-    Scratch<int64_t> off;
-    GPL_TRY(ids.get(ctx, (size_t)n));
-    GPL_TRY(cnt.get(ctx, (size_t)n));
-    GPL_TRY(dist.get(ctx, (size_t)n));
-    GPL_TRY(off.get(ctx, (size_t)n + 2));
-    GPL_CUDA(cudaMemsetAsync(cnt.p, 0, sizeof(int32_t) * (size_t)n, ctx->stream));  // the offsets below never see stale counts
-    GPL_TRY(nearest_run(ctx, idx, pts, points->validity, n, max_distance, ids.p, dist.p, cnt.p, nullptr, nullptr));
-    if (distance) GPL_TRY(deliver(ctx, distance, dist.p, sizeof(double) * (size_t)n, mem));  // the dense distances, for free
-    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n, off.p, off.p + n + 1)));
-    int64_t total = 0;
-    GPL_CUDA(cudaMemcpyAsync(&total, off.p + n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (total == 0) return GPL_OK;
-    GPL_TRY(raw.get(ctx, (size_t)total));
-    GPL_TRY(nearest_run(ctx, idx, pts, points->validity, n, max_distance, nullptr, dist.p, nullptr, off.p, raw.p));
-    void *pl = nullptr, *pr = nullptr;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pl));
-    res->lhs = (uint64_t *)pl;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pr));
-    res->rhs = (uint64_t *)pr;
-    res->n = total;
-    GPL_LAUNCH(ctx, k_nearest_sort_pairs, (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 8), (int64_t)kSMs * 16)), 256, 0, n, off.p,
-               raw.p, res->lhs, res->rhs);
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    return GPL_OK;
+    Scratch<int32_t> ids;
+    Scratch<double> dist;  // the dense distance: MODE 1 writes the rows at it
+    auto count = [&](int32_t *cnt) -> int {
+        GPL_TRY(ids.get(ctx, (size_t)n));
+        GPL_TRY(dist.get(ctx, (size_t)n));
+        GPL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (size_t)n, ctx->stream));  // the offsets never see stale counts
+        GPL_TRY(nearest_run(ctx, idx, pts, points->validity, n, max_distance, ids.p, dist.p, cnt, nullptr, nullptr));
+        if (distance) GPL_TRY(deliver(ctx, distance, dist.p, sizeof(double) * (size_t)n, mem));  // the dense distances, for free
+        return GPL_OK;
+    };
+    auto write = [&](const int64_t *off, int32_t *raw, double *) {
+        return nearest_run(ctx, idx, pts, points->validity, n, max_distance, nullptr, dist.p, nullptr, off, raw);
+    };
+    return pair_list(ctx, n, false, out, count, write);
 }
 
 extern "C" int gpl_nearest_join_geom(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double max_distance,
@@ -1368,24 +1318,11 @@ extern "C" int gpl_nearest_join_geom(gpl_ctx *ctx, const gpl_nearest_index *idx,
     GPL_TRY(check_geom_left(lhs, max_distance));
     if (lhs->type == GPL_POINT) return gpl_nearest_join_array(ctx, idx, lhs, max_distance, nearest_id, distance, n_tied, mem);
     GPL_CUDA(cudaSetDevice(ctx->device));
-    const int64_t n = lhs->n_geoms;
-    Scratch<double> box4, dd;
-    Scratch<uint8_t> cls;
-    Scratch<int32_t> di, dt;
-    if (n) GPL_TRY(geom_classify(ctx, lhs, box4, cls));
-    if (mem == GPL_DEVICE) return geom_run(ctx, idx, lhs, cls.p, box4.p, max_distance, nearest_id, distance, n_tied, nullptr, nullptr, nullptr);
-    GPL_TRY(di.get(ctx, (size_t)n));
-    if (distance) GPL_TRY(dd.get(ctx, (size_t)n));
-    if (n_tied) GPL_TRY(dt.get(ctx, (size_t)n));
-    GPL_TRY(geom_run(ctx, idx, lhs, cls.p, box4.p, max_distance, di.p, distance ? dd.p : nullptr, n_tied ? dt.p : nullptr, nullptr, nullptr,
-                     nullptr));
-    if (n) {
-        GPL_CUDA(cudaMemcpyAsync(nearest_id, di.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-        if (distance) GPL_CUDA(cudaMemcpyAsync(distance, dd.p, sizeof(double) * n, cudaMemcpyDeviceToHost, ctx->stream));
-        if (n_tied) GPL_CUDA(cudaMemcpyAsync(n_tied, dt.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    return GPL_OK;
+    RowClasses lc;
+    if (lhs->n_geoms) GPL_TRY(classify_rows(ctx, lhs, lc));
+    return dense_outputs(ctx, lhs->n_geoms, mem, nearest_id, distance, n_tied, [&](int32_t *nid, double *dist, int32_t *ntied) {
+        return geom_run(ctx, idx, lhs, lc.cls.p, lc.box4.p, max_distance, nid, dist, ntied, nullptr, nullptr, nullptr);
+    });
 }
 
 extern "C" int gpl_nearest_join_geom_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double max_distance,
@@ -1394,39 +1331,22 @@ extern "C" int gpl_nearest_join_geom_pairs(gpl_ctx *ctx, const gpl_nearest_index
     GPL_TRY(check_geom_left(lhs, max_distance));
     if (lhs->type == GPL_POINT) return gpl_nearest_join_pairs_array(ctx, idx, lhs, max_distance, out, distance, mem);
     GPL_CUDA(cudaSetDevice(ctx->device));
-    gpl_pairs *res = new gpl_pairs();
-    res->ctx = ctx;
-    *out = res;
     const int64_t n = lhs->n_geoms;
-    if (n == 0) return GPL_OK;
-    Scratch<double> box4, dist;
-    Scratch<uint8_t> cls;
-    Scratch<int32_t> ids, cnt, raw;
-    Scratch<int64_t> off;
-    GPL_TRY(geom_classify(ctx, lhs, box4, cls));
-    GPL_TRY(ids.get(ctx, (size_t)n));
-    GPL_TRY(cnt.get(ctx, (size_t)n));
-    GPL_TRY(dist.get(ctx, (size_t)n));
-    GPL_TRY(off.get(ctx, (size_t)n + 2));
-    GPL_TRY(geom_run(ctx, idx, lhs, cls.p, box4.p, max_distance, ids.p, dist.p, cnt.p, nullptr, nullptr, nullptr));
-    if (distance) GPL_TRY(deliver(ctx, distance, dist.p, sizeof(double) * (size_t)n, mem));
-    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n, off.p, off.p + n + 1)));
-    int64_t total = 0;
-    GPL_CUDA(cudaMemcpyAsync(&total, off.p + n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (total == 0) return GPL_OK;
-    GPL_TRY(raw.get(ctx, (size_t)total));
-    GPL_TRY(geom_run(ctx, idx, lhs, cls.p, box4.p, max_distance, nullptr, nullptr, nullptr, dist.p, off.p, raw.p));
-    void *pl = nullptr, *pr = nullptr;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pl));
-    res->lhs = (uint64_t *)pl;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pr));
-    res->rhs = (uint64_t *)pr;
-    res->n = total;
-    GPL_LAUNCH(ctx, k_nearest_sort_pairs, (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 8), (int64_t)kSMs * 16)), 256, 0, n, off.p,
-               raw.p, res->lhs, res->rhs);
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    return GPL_OK;
+    RowClasses lc;
+    Scratch<int32_t> ids;
+    Scratch<double> dist;  // the dense distance: MODE 1 writes the rows at it
+    auto count = [&](int32_t *cnt) -> int {
+        GPL_TRY(classify_rows(ctx, lhs, lc));
+        GPL_TRY(ids.get(ctx, (size_t)n));
+        GPL_TRY(dist.get(ctx, (size_t)n));
+        GPL_TRY(geom_run(ctx, idx, lhs, lc.cls.p, lc.box4.p, max_distance, ids.p, dist.p, cnt, nullptr, nullptr, nullptr));
+        if (distance) GPL_TRY(deliver(ctx, distance, dist.p, sizeof(double) * (size_t)n, mem));
+        return GPL_OK;
+    };
+    auto write = [&](const int64_t *off, int32_t *raw, double *) {
+        return geom_run(ctx, idx, lhs, lc.cls.p, lc.box4.p, max_distance, nullptr, nullptr, nullptr, dist.p, off, raw);
+    };
+    return pair_list(ctx, n, false, out, count, write);
 }
 
 extern "C" int gpl_dwithin_count(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int32_t *count, int mem) {
@@ -1434,16 +1354,15 @@ extern "C" int gpl_dwithin_count(gpl_ctx *ctx, const gpl_nearest_index *idx, con
     GPL_TRY(check_dwithin(lhs, distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = lhs->n_geoms;
-    Scratch<double> box4;
-    Scratch<uint8_t> cls;
+    RowClasses lc;
     Scratch<int32_t> dc;
-    if (n && lhs->type != GPL_POINT) GPL_TRY(geom_classify(ctx, lhs, box4, cls));
+    if (n && lhs->type != GPL_POINT) GPL_TRY(classify_rows(ctx, lhs, lc));
     int32_t *out = count;
     if (mem != GPL_DEVICE) {
         GPL_TRY(dc.get(ctx, (size_t)n));
         out = dc.p;
     }
-    GPL_TRY(dwithin_run(ctx, idx, lhs, cls.p, box4.p, distance, out, nullptr, nullptr, nullptr));
+    GPL_TRY(dwithin_run(ctx, idx, lhs, lc.cls.p, lc.box4.p, distance, out, nullptr, nullptr, nullptr));
     if (mem != GPL_DEVICE) GPL_TRY(deliver(ctx, count, dc.p, sizeof(int32_t) * (size_t)n, mem));
     return GPL_OK;
 }
@@ -1453,54 +1372,13 @@ extern "C" int gpl_dwithin_join_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx
     GPL_REQUIRE(ctx && idx && lhs && out, GPL_ERR_INVALID_ARG, "gpl_dwithin_join_pairs: NULL argument");
     GPL_TRY(check_dwithin(lhs, distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
-    gpl_pairs *res = new gpl_pairs();
-    res->ctx = ctx;
-    res->with_dist = with_distance != 0;
-    *out = res;
-    const int64_t n = lhs->n_geoms;
-    if (n == 0) return GPL_OK;
-    Scratch<double> box4, raw_d, tmp_d;
-    Scratch<uint8_t> cls;
-    Scratch<int32_t> cnt, raw, tmp, big;
-    Scratch<int64_t> off;
-    Scratch<unsigned long long> n_big;
-    if (lhs->type != GPL_POINT) GPL_TRY(geom_classify(ctx, lhs, box4, cls));
-    GPL_TRY(cnt.get(ctx, (size_t)n));
-    GPL_TRY(off.get(ctx, (size_t)n + 2));
-    GPL_TRY(dwithin_run(ctx, idx, lhs, cls.p, box4.p, distance, cnt.p, nullptr, nullptr, nullptr));
-    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n, off.p, off.p + n + 1)));
-    int64_t total = 0;
-    GPL_CUDA(cudaMemcpyAsync(&total, off.p + n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (total == 0) return GPL_OK;
-    GPL_TRY(raw.get(ctx, (size_t)total));
-    if (with_distance) GPL_TRY(raw_d.get(ctx, (size_t)total));
-    GPL_TRY(dwithin_run(ctx, idx, lhs, cls.p, box4.p, distance, nullptr, off.p, raw.p, raw_d.p));
-    void *pl = nullptr, *pr = nullptr, *pd = nullptr;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pl));
-    res->lhs = (uint64_t *)pl;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pr));
-    res->rhs = (uint64_t *)pr;
-    if (with_distance) {
-        GPL_TRY(ctx->alloc(sizeof(double) * (size_t)total, &pd));
-        res->dist = (double *)pd;
-    }
-    res->n = total;
-    // segments of more than kDwSortSmall pairs: at most total / (kDwSortSmall + 1) of them
-    GPL_TRY(big.get(ctx, (size_t)(total / (kDwSortSmall + 1) + 1)));
-    GPL_TRY(n_big.get(ctx, 1));
-    GPL_CUDA(cudaMemsetAsync(n_big.p, 0, sizeof(unsigned long long), ctx->stream));
-    GPL_LAUNCH(ctx, k_dwithin_sort_small, (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 8), (int64_t)kSMs * 16)), 256, 0, n, off.p,
-               raw.p, raw_d.p, res->lhs, res->rhs, res->dist, big.p, n_big.p);
-    unsigned long long h_big = 0;
-    GPL_CUDA(cudaMemcpyAsync(&h_big, n_big.p, sizeof(h_big), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (h_big > 0) {
-        GPL_TRY(tmp.get(ctx, (size_t)total));
-        if (with_distance) GPL_TRY(tmp_d.get(ctx, (size_t)total));
-        GPL_LAUNCH(ctx, k_dwithin_sort_large, (int)std::min<int64_t>((int64_t)h_big, (int64_t)kSMs * 8), kDwRadixThreads, 0, big.p, (int64_t)h_big,
-                   off.p, raw.p, raw_d.p, tmp.p, tmp_d.p, res->lhs, res->rhs, res->dist);
-    }
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
-    return GPL_OK;
+    RowClasses lc;
+    auto count = [&](int32_t *cnt) -> int {
+        if (lhs->type != GPL_POINT) GPL_TRY(classify_rows(ctx, lhs, lc));
+        return dwithin_run(ctx, idx, lhs, lc.cls.p, lc.box4.p, distance, cnt, nullptr, nullptr, nullptr);
+    };
+    auto write = [&](const int64_t *off, int32_t *raw, double *raw_d) {
+        return dwithin_run(ctx, idx, lhs, lc.cls.p, lc.box4.p, distance, nullptr, off, raw, raw_d);
+    };
+    return pair_list(ctx, lhs->n_geoms, with_distance != 0, out, count, write);
 }

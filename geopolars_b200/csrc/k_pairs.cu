@@ -602,23 +602,7 @@ __global__ void k_point_point_dist(int64_t n, const double2 *__restrict__ a, con
 int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n);
 int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
 
-static int warp_grid(int64_t rows, int warps_per_cta) {
-    int64_t want = ceil_div(rows, warps_per_cta);
-    return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * 16));
-}
-
 static int side_class_host(int t) { return (t == GPL_POINT || t == GPL_MULTIPOINT) ? 0 : (t == GPL_LINESTRING || t == GPL_MULTILINESTRING) ? 1 : 2; }
-static const char *type_name(int t) {
-    switch (t) {
-    case GPL_POINT: return "Point";
-    case GPL_LINESTRING: return "LineString";
-    case GPL_POLYGON: return "Polygon";
-    case GPL_MULTIPOINT: return "MultiPoint";
-    case GPL_MULTILINESTRING: return "MultiLineString";
-    case GPL_MULTIPOLYGON: return "MultiPolygon";
-    default: return "Unknown";
-    }
-}
 
 // bool result: bytes on device -> Arrow bitmap in the caller's memory
 static int finish_bitmap(gpl_ctx *ctx, const uint8_t *bytes_dev, int64_t n, uint8_t *out_bitmap, int mem) {
@@ -762,7 +746,7 @@ extern "C" int gpl_distance(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b
 // the intersection box); count -> scan -> write gives the candidate list, a warp per candidate evaluates the
 // dispatched predicate, and a second scan compacts the hits.  Points x (Multi)Polygons with millions of points should
 // use gpl_pip_index_build + gpl_contains_join (the north-star path); this entry point is the general one.
-// JoinGrid, jg_cell, k_join_union, k_join_cells: join_grid.cuh; struct gpl_pairs: common.cuh
+// JoinGrid, jg_cell and the grid build (join_grid_build): join_grid.cuh; struct gpl_pairs: common.cuh
 namespace gpl {
 
 int envelope_raw(gpl_ctx *ctx, const gpl_array *in, double *out4_dev, uint8_t *valid_bytes_dev);
@@ -889,58 +873,27 @@ extern "C" int gpl_spatial_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_ar
     GPL_TRY(envelope_raw(ctx, lhs, l4.p, lh.p));
     GPL_TRY(envelope_raw(ctx, rhs, r4.p, rh.p));
     // ---- grid over the right side's union box ------------------------------------------------------------------------------
-    Scratch<unsigned long long> acc;
-    GPL_TRY(acc.get(ctx, 4));
-    GPL_CUDA(cudaMemsetAsync(acc.p, 0, 4 * sizeof(unsigned long long), ctx->stream));
-    GPL_LAUNCH(ctx, k_join_union, (int)std::min<int64_t>(ceil_div(nr, 256), kSMs * 8), 256, 0, r4.p, rh.p, nr, acc.p);
-    unsigned long long h_acc[4];
-    GPL_CUDA(cudaMemcpyAsync(h_acc, acc.p, sizeof(h_acc), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (h_acc[2] == 0ULL) return GPL_OK;  // no right row has an envelope
-    auto dec = [](unsigned long long u) {
-        const unsigned long long b = (u >> 63) ? (u & 0x7fffffffffffffffULL) : ~u;
-        double d;
-        memcpy(&d, &b, sizeof(d));
-        return d;
-    };
-    const double ux0 = dec(~h_acc[0]), uy0 = dec(~h_acc[1]), ux1 = dec(h_acc[2]), uy1 = dec(h_acc[3]);
-    JoinGrid jg;
-    jg.g = (int32_t)std::min<int64_t>(2048, std::max<int64_t>(1, (int64_t)ceil(sqrt((double)nr))));
-    jg.x0 = ux0, jg.y0 = uy0;
-    const double w = ux1 - ux0, h = uy1 - uy0;
-    jg.inv_w = (w > 0.0 && std::isfinite(w) && std::isfinite(jg.g / w)) ? jg.g / w : 0.0;
-    jg.inv_h = (h > 0.0 && std::isfinite(h) && std::isfinite(jg.g / h)) ? jg.g / h : 0.0;
-    const int64_t n_cells = (int64_t)jg.g * jg.g;
-    Scratch<int32_t> cell_count, cell_start, items, cand_count;
-    Scratch<int64_t> tot, cand_off;
-    GPL_TRY(cell_count.get(ctx, (size_t)n_cells + 1));
-    GPL_TRY(cell_start.get(ctx, (size_t)n_cells + 1));
-    GPL_TRY(tot.get(ctx, 2));
-    GPL_CUDA(cudaMemsetAsync(cell_count.p, 0, sizeof(int32_t) * (n_cells + 1), ctx->stream));
-    GPL_LAUNCH(ctx, k_join_cells<0>, (int)ceil_div(nr, 128), 128, 0, r4.p, rh.p, nr, jg, cell_count.p, nullptr);
-    GPL_TRY((exclusive_scan<int32_t, int32_t>(ctx, cell_count.p, n_cells, cell_start.p, tot.p)));
-    int64_t n_items = 0;
-    GPL_CUDA(cudaMemcpyAsync(&n_items, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    GPL_REQUIRE(n_items < (1LL << 31), GPL_ERR_UNSUPPORTED, "gpl_spatial_join: grid too dense (%lld cell items)", (long long)n_items);
-    GPL_TRY(items.get(ctx, (size_t)n_items + 1));
-    GPL_CUDA(cudaMemcpyAsync(cell_count.p, cell_start.p, sizeof(int32_t) * n_cells, cudaMemcpyDeviceToDevice, ctx->stream));  // cursors
-    GPL_LAUNCH(ctx, k_join_cells<1>, (int)ceil_div(nr, 128), 128, 0, r4.p, rh.p, nr, jg, cell_count.p, items.p);
+    GridBuild grid;
+    GPL_TRY(join_grid_build(ctx, r4.p, rh.p, nr, nr, "gpl_spatial_join", grid));
+    if (grid.jg.g == 0) return GPL_OK;  // no right row has an envelope
     // ---- candidates: count -> scan -> write ----------------------------------------------------------------------------------
+    Scratch<int32_t> cand_count;
+    Scratch<int64_t> tot, cand_off;
+    GPL_TRY(tot.get(ctx, 1));
     GPL_TRY(cand_count.get(ctx, (size_t)nl + 1));
     GPL_TRY(cand_off.get(ctx, (size_t)nl + 2));
-    GPL_LAUNCH(ctx, k_join_candidates<0>, (int)ceil_div(nl, 128), 128, 0, l4.p, lh.p, nl, r4.p, jg, ux1, uy1, cell_start.p, items.p, cand_count.p,
-               nullptr, nullptr, nullptr);
-    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cand_count.p, nl, cand_off.p, tot.p + 1)));
+    GPL_LAUNCH(ctx, k_join_candidates<0>, (int)ceil_div(nl, 128), 128, 0, l4.p, lh.p, nl, r4.p, grid.jg, grid.ux1, grid.uy1, grid.cell_start.p,
+               grid.items.p, cand_count.p, nullptr, nullptr, nullptr);
+    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cand_count.p, nl, cand_off.p, tot.p)));
     int64_t n_cand = 0;
-    GPL_CUDA(cudaMemcpyAsync(&n_cand, tot.p + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaMemcpyAsync(&n_cand, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));
     if (n_cand == 0) return GPL_OK;
     Scratch<uint64_t> cl, cr;
     GPL_TRY(cl.get(ctx, (size_t)n_cand));
     GPL_TRY(cr.get(ctx, (size_t)n_cand));
-    GPL_LAUNCH(ctx, k_join_candidates<1>, (int)ceil_div(nl, 128), 128, 0, l4.p, lh.p, nl, r4.p, jg, ux1, uy1, cell_start.p, items.p, nullptr,
-               cand_off.p, cl.p, cr.p);
+    GPL_LAUNCH(ctx, k_join_candidates<1>, (int)ceil_div(nl, 128), 128, 0, l4.p, lh.p, nl, r4.p, grid.jg, grid.ux1, grid.uy1, grid.cell_start.p,
+               grid.items.p, nullptr, cand_off.p, cl.p, cr.p);
     // ---- exact predicate per candidate ------------------------------------------------------------------------------------------
     Scratch<uint8_t> hit;
     GPL_TRY(hit.get(ctx, (size_t)n_cand));

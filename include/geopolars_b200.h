@@ -329,9 +329,7 @@ int gpl_nearest_join(gpl_ctx *ctx, const gpl_nearest_index *idx, const double *p
 int gpl_nearest_join_array(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *points, double max_distance,
                            int32_t *nearest_id, double *distance, int32_t *n_tied, int mem);
 /* every tied (point, row) pair once, sorted by (lhs, rhs), as a device-resident gpl_pairs; distance (may be NULL, in
- * `mem`) receives the dense distance of every point (NaN: no match), which the pair list is built from.  The rows of one
- * point are ordered by a rank sort of O(k^2) for k tied rows: fine for ties among a few thousand rows, slow for a point
- * tied with ~1e5 or more rows (e.g. that many coincident geometries). */
+ * `mem`) receives the dense distance of every point (NaN: no match), which the pair list is built from. */
 int gpl_nearest_join_pairs_array(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *points, double max_distance,
                                  gpl_pairs **out, double *distance, int mem);
 /* Nearest join for a left column of ANY of the six types (DESIGN.md §4.13), fewer than 2^31 rows (else GPL_ERR_UNSUPPORTED,

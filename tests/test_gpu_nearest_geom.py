@@ -203,6 +203,9 @@ def test_overlaps_touches_and_lattice_ties(ctx):
                                     [sq(x + 1.0, y + 1.0, 0.0) for x in range(3) for y in range(3)])
     _, nid, dist, tied = check_geom(ctx, lhs, rhs, sample=np.r_[0:40, 361:370])
     assert (dist == 0.0).all() and (tied[:361] == 1).all()
+    # one square over the whole lattice: 400 rows tied at 0, more than the on-chip per-row sort takes
+    _, nid, dist, tied = check_geom(ctx, GeoArrowArray.from_shapes(GeometryType.POLYGON, [sq(-1.0, -1.0, 22.0)]), rhs)
+    assert nid[0] == 0 and dist[0] == 0.0 and tied[0] == 400
     # lattice of points, left segments centred between 4 of them: 4-way ties at equal f64 distances
     g = np.arange(25, dtype=np.float64)
     X, Y = np.meshgrid(g, g)
