@@ -97,11 +97,8 @@ static_assert(sizeof(CellRec) == 32, "CellRec must be one sector");
 
 constexpr int32_t kFastBit = 1 << 30;  // PartLite::nb_flags: the CellRec points at the FP32 fast table
 constexpr int kFastCShift = 24;        // bits 24..29: C/2 (C = 16-byte records per bucket incl. header, even)
-#ifndef GPL_FAST_LIST
-#define GPL_FAST_LIST 6
-#endif
-constexpr int kFastListRecs = GPL_FAST_LIST;  // records per fast list: header + edges, even (see the FP32 fast table below)
-static_assert(GPL_FAST_LIST % 2 == 0 && GPL_FAST_LIST >= 2 && GPL_FAST_LIST <= 8, "fast list = 1..4 sectors");
+constexpr int kFastListRecs = 6;  // records per fast list: header + edges, even (see the FP32 fast table below)
+static_assert(kFastListRecs % 2 == 0 && kFastListRecs >= 2 && kFastListRecs <= 8, "fast list = 1..4 sectors");
 constexpr int kFastMaxCount = 120;  // longest bucket list a fast part may have
 
 struct __align__(32) EdgeRec {  // one L2 sector
@@ -205,9 +202,8 @@ struct BuildArgs {
     const uint8_t *validity;
     int slots_x100;
     int32_t G, rs;
-    int32_t raster_rows;     // fine rows per raster work item (8, 16 or 32)
     int32_t build_legacy;    // 1: the previous work distribution (A/B): one thread per y-bucket in ph_bucket_finish,
-                             //    (part, 32-row chunk) raster items dealt out statically, it += nwarps
+                             //    raster items dealt out statically, it += nwarps
     int64_t n_cells, NB_cap;
     // phase 1 (scratch)
     PartHeader *hdr;
@@ -1055,13 +1051,13 @@ __device__ void ph_raster(const BuildArgs &a, const GridParams &g, const int32_t
     int32_t *cnt = sm.cnt[wid];
     uint32_t *list = sm.list[wid];
     double *row_y = sm.ry[wid];
-    // work item = (part, k): the chunks ra = fy0 + R (k + K j) of the part, R = a.raster_rows fine rows each.  A part's bbox
-    // is about one coarse cell high, i.e. K = 2^rs / R chunks; they are independent (every raster write is an atomicOr).
-    // Items are claimed from a global counter: a warp that finishes early takes the next one, so the phase ends one small
-    // item after the work runs out instead of after a last, partly filled wave of a static deal.  Legacy (A/B): R = 32,
-    // K <= 8, item it to warp it mod nwarps.
-    const int32_t R = a.build_legacy ? 32 : a.raster_rows;
-    const int32_t K = a.build_legacy ? max(1, min(8, (1 << g.rs) >> 5)) : max(1, (1 << g.rs) / R);
+    // work item = (part, k): the chunks ra = fy0 + R (k + K j) of the part, R = 32 fine rows each (one lane per row).  A
+    // part's bbox is about one coarse cell high, i.e. K = 2^rs / R chunks; they are independent (every raster write is an
+    // atomicOr).  Items are claimed from a global counter: a warp that finishes early takes the next one, so the phase ends
+    // one small item after the work runs out instead of after a last, partly filled wave of a static deal.  Legacy (A/B):
+    // item it to warp it mod nwarps.
+    constexpr int32_t R = 32;
+    const int32_t K = max(1, (1 << g.rs) / R);
     auto claim = [&]() -> int64_t {
         unsigned long long v = 0;
         if (lane == 0) v = atomicAdd(a.acc + ACC_RASTER_NEXT, 1ULL);
@@ -1334,18 +1330,10 @@ __device__ __forceinline__ int64_t coarse_cell(const GridParams &g, double px, d
 
 // One 32-byte record (one L2 sector, 32-byte aligned) as two back-to-back 128-bit loads: sm_90 has no 256-bit
 // LDG, and both halves come from the same sector.
-#ifndef GPL_PIP_NOALLOC
-#define GPL_PIP_NOALLOC 0
-#endif
 __device__ __forceinline__ void ld256(const void *p, double &a, double &b, double &c, double &d) {
     const double *q = static_cast<const double *>(p);
-#if GPL_PIP_NOALLOC
-    asm("ld.global.nc.L1::no_allocate.v2.f64 {%0,%1}, [%2];" : "=d"(a), "=d"(b) : "l"(q));
-    asm("ld.global.nc.L1::no_allocate.v2.f64 {%0,%1}, [%2];" : "=d"(c), "=d"(d) : "l"(q + 2));
-#else
     asm("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(a), "=d"(b) : "l"(q));
     asm("ld.global.nc.v2.f64 {%0,%1}, [%2];" : "=d"(c), "=d"(d) : "l"(q + 2));
-#endif
 }
 __device__ __forceinline__ void ld256(const void *p, int32_t (&r)[8]) {
     const int32_t *q = static_cast<const int32_t *>(p);
@@ -1377,13 +1365,7 @@ __device__ __forceinline__ void edge_rule_fast(double sx, double sy, double ex, 
     wn += (int)(a && !b && det > 0.0) - (int)(!a && b && det < 0.0);
 }
 
-#ifndef GPL_PIP_MINB
-#define GPL_PIP_MINB 3
-#endif
-#ifndef GPL_PIP_THREADS
-#define GPL_PIP_THREADS 256
-#endif
-constexpr int kQueryThreads = GPL_PIP_THREADS;
+constexpr int kQueryThreads = 256;
 constexpr int32_t kDeferred = -2;  // first_id marker: "the fast filter could not decide, see k_pip_deferred"
 
 __device__ __forceinline__ void unpack_lite(const int32_t *r, PartLite &l) {
@@ -1642,22 +1624,14 @@ __device__ __forceinline__ void walk_point(const IndexView &ix, const double2 p,
     }
 }
 
-#ifndef GPL_PIP_LEAN_MINB
-#define GPL_PIP_LEAN_MINB 4
-#endif
-// Round-1 kernel, kept for MODE 1 (pair lists) and as the A/B baseline (GPL_PIP_LEGACY=1): one thread per point,
-// every point walks.  32 consecutive points per warp (coalesced 512-byte read, software-prefetched one grid stride
-// ahead).
-template <int MODE, bool LEAN = false>
-__global__ void __launch_bounds__(kQueryThreads, LEAN ? GPL_PIP_LEAN_MINB : GPL_PIP_MINB) k_pip_query(const IndexView ix, const double2 *__restrict__ pts,
-                                                                           const uint8_t *__restrict__ pts_validity,
-                                                                           int64_t n_pts, int32_t *__restrict__ first_id,
-                                                                           int32_t *__restrict__ count,
-                                                                           const int64_t *__restrict__ pair_off,
-                                                                           uint64_t *__restrict__ lhs, uint64_t *__restrict__ rhs,
-                                                                           int64_t point_base,
-                                                                           unsigned long long *__restrict__ n_deferred,
-                                                                           uint32_t *__restrict__ deferred_list, uint32_t list_cap) {
+constexpr int kQueryMinBlocks = 3;  // resident CTAs per SM of both query kernels (80 registers per thread)
+
+// Pair lists (the write pass after count -> scan): one thread per point, every point walks and writes its pairs from slot
+// pair_off[i] on.  32 consecutive points per warp (coalesced 512-byte read, software-prefetched one grid stride ahead).
+__global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_pairs(const IndexView ix, const double2 *__restrict__ pts,
+                                                                              const uint8_t *__restrict__ pts_validity, int64_t n_pts,
+                                                                              const int64_t *__restrict__ pair_off,
+                                                                              uint64_t *__restrict__ lhs, uint64_t *__restrict__ rhs) {
     const GridParams &g = ix.grid;
     const int64_t stride = (int64_t)gridDim.x * kQueryThreads;
     int64_t i = (int64_t)blockIdx.x * kQueryThreads + threadIdx.x;
@@ -1670,22 +1644,11 @@ __global__ void __launch_bounds__(kQueryThreads, LEAN ? GPL_PIP_LEAN_MINB : GPL_
         if (ok && pts_validity) ok = bit_get(pts_validity, i);
         int32_t first = -1, cnt = 0;
         bool undecided = false;
-        if (ok)
-            walk_point<MODE, LEAN>(ix, p, count != nullptr, first, cnt, undecided, (uint64_t)(point_base + i), MODE == 1 ? pair_off[i] : 0, lhs,
-                                   rhs);
-        if (MODE == 0) {
-            if (undecided) {
-                first = kDeferred;
-                const unsigned long long slot = atomicAdd(n_deferred, 1ULL);
-                if (slot < list_cap) deferred_list[slot] = (uint32_t)i;  // chunk-relative index (chunks are < 2^32 points)
-            }
-            __stcs(first_id + i, first);
-            if (count) __stcs(count + i, cnt);
-        }
+        if (ok) walk_point<1, false>(ix, p, false, first, cnt, undecided, (uint64_t)i, pair_off[i], lhs, rhs);
     }
 }
 
-// ---- the streaming kernel (MODE 0 of round 2) --------------------------------------------------------------
+// ---- the streaming kernel: ids and counts ---------------------------------------------------------------------
 // Persistent warps; a warp takes tiles of 128 consecutive points (2 KB; lane l holds points l, l+32, l+64, l+96, so that
 // every warp-wide 16-byte load covers 512 contiguous bytes; the next tile is prefetched into registers).  Per point: closed bbox test, fine cell by arithmetic, ONE 64-bit load of the raster
 // word (four independent loads in flight per lane), then
@@ -1702,11 +1665,10 @@ struct __align__(16) StreamSmem {
     double2 q_pts[kStreamWarps][kQueueCap];
     uint32_t q_idx[kStreamWarps][kQueueCap];
 };
-#ifndef GPL_PIP_STREAM_MINB
-#define GPL_PIP_STREAM_MINB 3
-#endif
 // cache-hint variants (GPL_PIP_LD_HINTS, A/B switch): the point stream without an L1 line (L2: evict first), the raster gather
 // (20 MB of random 8-byte words: no reuse an L1 could catch) without one — leaves the L1 to the cell / part / edge records.
+// `hints` stays a kernel argument: with the default fixed at compile time, ptxas allocates the registers of both
+// instantiations differently, and on config 2 (one H100 80GB HBM3, 700 W) the LEAN kernel took 1 % and the full walk 9 % longer.
 __device__ __forceinline__ double2 ld_pt_na(const double2 *p, unsigned long long pol) {
     double2 a;
     asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v2.f64 {%0,%1}, [%2], %3;" : "=d"(a.x), "=d"(a.y) : "l"(p), "l"(pol));
@@ -1722,34 +1684,17 @@ __device__ __forceinline__ uint2 ldg_na(const uint2 *p) {
     asm("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p));
     return v;
 }
-// HIST: per-polygon hit counts (config 4's all-reduce input) in the same pass: 32-bit bins privatised per CTA in shared
-// memory behind the queues, flushed with one 64-bit global atomic per non-zero bin when the CTA retires.
-// CSM: the rows of candidate #0 of every coarse cell (raster code 1: 36 % of config 2's points) staged in shared memory —
-// the 8-byte gather from the L1-resident table cost L1/TEX tag wavefronts, which can limit this kernel.
-template <bool LEAN, bool HIST, bool CSM>
-__global__ void __launch_bounds__(kQueryThreads, GPL_PIP_STREAM_MINB) k_pip_stream(const IndexView ix, const double2 *__restrict__ pts,
-                                                                                  const uint8_t *__restrict__ pts_validity, int64_t n_pts,
-                                                                                  int32_t *__restrict__ first_id, int32_t *__restrict__ count,
-                                                                                  unsigned long long *__restrict__ n_deferred,
-                                                                                  uint32_t *__restrict__ deferred_list, uint32_t list_cap,
-                                                                                  unsigned long long *__restrict__ hist, int32_t n_bins,
-                                                                                  int hints) {
+template <bool LEAN>
+__global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_stream(const IndexView ix, const double2 *__restrict__ pts,
+                                                                               const uint8_t *__restrict__ pts_validity, int64_t n_pts,
+                                                                               int32_t *__restrict__ first_id, int32_t *__restrict__ count,
+                                                                               unsigned long long *__restrict__ n_deferred,
+                                                                               uint32_t *__restrict__ deferred_list, uint32_t list_cap, int hints) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     unsigned long long pol_ef = 0ULL;
     if (hints & 2) asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol_ef));
     const bool raster_na = (hints & 1) != 0, pts_na = (hints & 2) != 0;
     StreamSmem &sm = *reinterpret_cast<StreamSmem *>(smem_raw);
-    unsigned int *bins = reinterpret_cast<unsigned int *>(smem_raw + sizeof(StreamSmem));
-    int32_t *cand0 = reinterpret_cast<int32_t *>(smem_raw + sizeof(StreamSmem));  // HIST and CSM are never combined
-    if (HIST) {
-        for (int32_t b = threadIdx.x; b < n_bins; b += kQueryThreads) bins[b] = 0u;
-        __syncthreads();
-    }
-    if (CSM) {
-        const int32_t n_cells = ix.grid.gx * ix.grid.gy;
-        for (int32_t c = threadIdx.x; c < n_cells; c += kQueryThreads) cand0[c] = __ldg(&ix.cand01[c].x);
-        __syncthreads();
-    }
     const GridParams &g = ix.grid;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     double2 *q_pts = sm.q_pts[wid];
@@ -1776,7 +1721,6 @@ __global__ void __launch_bounds__(kQueryThreads, GPL_PIP_STREAM_MINB) k_pip_stre
             }
             first_id[idx] = first;
             if (want_count) count[idx] = cnt;
-            if (HIST && first >= 0 && first < n_bins) atomicAdd(&bins[first], 1u);
         }
     };
 
@@ -1826,13 +1770,10 @@ __global__ void __launch_bounds__(kQueryThreads, GPL_PIP_STREAM_MINB) k_pip_stre
                 const int64_t cc = (int64_t)(fy[k] >> g.rs) * g.gx + (fx[k] >> g.rs);
                 if (code[k] == 1u && word[k].y != 0xfffffffeu) {
                     id[k] = (int32_t)word[k].y;  // the candidate's row travels with the codes: no second gather
-                } else if (CSM && code[k] == 1u) {
-                    id[k] = cand0[cc];
                 } else {
                     const int2 cand = __ldg(ix.cand01 + cc);
                     id[k] = code[k] == 1u ? cand.x : cand.y;
                 }
-                if (HIST && id[k] >= 0 && id[k] < n_bins) atomicAdd(&bins[id[k]], 1u);
             }
         }
         // stage 3: ids out (the queued ones are overwritten by the walk)
@@ -1863,13 +1804,6 @@ __global__ void __launch_bounds__(kQueryThreads, GPL_PIP_STREAM_MINB) k_pip_stre
         }
     }
     if (qn > 0) walk_queued(lane, lane < qn);
-    if (HIST) {
-        __syncthreads();
-        for (int32_t b = threadIdx.x; b < n_bins; b += kQueryThreads) {
-            const unsigned int v = bins[b];
-            if (v) atomicAdd(hist + b, (unsigned long long)v);
-        }
-    }
 }
 
 // Exact re-evaluation of the points the walk marked kDeferred (those whose filters could not
@@ -1878,8 +1812,7 @@ __global__ void __launch_bounds__(kQueryThreads, GPL_PIP_STREAM_MINB) k_pip_stre
 // counter is zero.  One thread per deferred point, taken from the list the query kernel appended to; if
 // the list overflowed, the id column is scanned for the marker instead.
 __device__ __forceinline__ void deferred_point(const IndexView &ix, const double2 *__restrict__ pts, int64_t i,
-                                               int32_t *__restrict__ first_id, int32_t *__restrict__ count,
-                                               unsigned long long *__restrict__ hist) {
+                                               int32_t *__restrict__ first_id, int32_t *__restrict__ count) {
     const double2 p = pts[i];
     const CellRec cell = ix.cells[coarse_cell(ix.grid, p.x, p.y)];
     int32_t first = -1, cnt = 0, last_geom = -1;
@@ -1897,23 +1830,21 @@ __device__ __forceinline__ void deferred_point(const IndexView &ix, const double
     }
     first_id[i] = first;
     if (count) count[i] = cnt;
-    if (hist && first >= 0) atomicAdd(hist + first, 1ULL);  // the streaming kernel counted decided points only
 }
 __global__ void __launch_bounds__(256) k_pip_deferred(const IndexView ix, const double2 *__restrict__ pts, int64_t n_pts,
                                                       int32_t *__restrict__ first_id, int32_t *__restrict__ count,
                                                       unsigned long long *__restrict__ n_deferred,
                                                       const uint32_t *__restrict__ deferred_list, uint32_t list_cap,
-                                                      unsigned long long *__restrict__ n_deferred_total,
-                                                      unsigned long long *__restrict__ hist) {
+                                                      unsigned long long *__restrict__ n_deferred_total) {
     const unsigned long long nd = *n_deferred;
     if (nd == 0ULL) return;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     if (nd <= list_cap) {
         for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < (int64_t)nd; k += stride)
-            deferred_point(ix, pts, (int64_t)deferred_list[k], first_id, count, hist);
+            deferred_point(ix, pts, (int64_t)deferred_list[k], first_id, count);
     } else {
         for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_pts; i += stride)
-            if (first_id[i] == kDeferred) deferred_point(ix, pts, i, first_id, count, hist);
+            if (first_id[i] == kDeferred) deferred_point(ix, pts, i, first_id, count);
     }
     if (blockIdx.x == 0 && threadIdx.x == 0 && n_deferred_total) atomicAdd(n_deferred_total, nd);
 }
@@ -1968,61 +1899,48 @@ static int env_int(const char *name, int dflt) {
     return e ? atoi(e) : dflt;
 }
 
-static int query_grid(int64_t n, bool lean = false) {
+static int query_grid(int64_t n) {
     // persistent-style: 132 SMs x resident CTAs, grid-stride over the point stream
-    static const int per_sm_full = env_int("GPL_PIP_CTAS_PER_SM", 8);
-    static const int per_sm_lean = env_int("GPL_PIP_LEAN_CTAS_PER_SM", 2 * GPL_PIP_LEAN_MINB);  // two waves of the resident CTAs
-    const int per_sm = lean ? per_sm_lean : per_sm_full;
+    static const int per_sm = env_int("GPL_PIP_CTAS_PER_SM", 8);
     int64_t want = ceil_div(n, kQueryThreads);
     return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * per_sm));
 }
-// streaming kernel: exactly the resident CTAs (persistent warps, one tile of 128 points per warp and iteration)
-constexpr int32_t kHistFuseMaxBins = 12288;  // 48 KB of bins per CTA: three CTAs per SM still fit next to the queues
-template <bool LEAN, bool HIST, bool CSM>
-static int stream_grid(int64_t n, size_t smem_bytes) {
-    static size_t attr_bytes = 0;
-    if (smem_bytes > attr_bytes) {
-        cudaFuncSetAttribute(k_pip_stream<LEAN, HIST, CSM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
-        attr_bytes = smem_bytes;
-    }
-    int occ = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pip_stream<LEAN, HIST, CSM>, kQueryThreads, smem_bytes) != cudaSuccess || occ < 1) occ = 1;
-    (void)cudaGetLastError();
-    static const int cap = env_int("GPL_PIP_STREAM_CTAS_PER_SM", 0);
-    const int per_sm = cap > 0 ? std::min(cap, occ) : occ;
-    const int64_t want = ceil_div(ceil_div(n, kTilePts), kStreamWarps);
-    return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * per_sm));
-}
-constexpr int32_t kCandSmemMaxCells = 12288;  // 48 KB of candidate rows per CTA
-template <bool LEAN, bool HIST>
+// the streaming kernel on exactly the resident CTAs (persistent warps, one tile of 128 points per warp and iteration)
+template <bool LEAN>
 static void launch_stream(const IndexView &v, const double2 *pts, const uint8_t *val, int64_t m, int32_t *first, int32_t *cnt,
-                          const gpl_pip_index *idx, unsigned long long *hist, int32_t n_bins, cudaStream_t stream) {
-    static const bool csm_enabled = env_int("GPL_PIP_CAND_SMEM", 0) != 0;  // candidate rows staged in shared memory: opt-in
+                          const gpl_pip_index *idx, cudaStream_t stream) {
     // bit 0: raster gather without an L1 line; bit 2: the point stream too; bit 1: the point stream too, plus an L2 evict-first
     // policy.  On config 2 (one H100) 0, 1 and 5 are within 1 % of each other.
     static const int hints = env_int("GPL_PIP_LD_HINTS", 5);
-    const int64_t n_cells = (int64_t)v.grid.gx * v.grid.gy;
-    if (!HIST && csm_enabled && n_cells <= kCandSmemMaxCells) {
-        const size_t smem = sizeof(StreamSmem) + sizeof(int32_t) * (size_t)n_cells;
-        k_pip_stream<LEAN, false, true><<<stream_grid<LEAN, false, true>(m, smem), kQueryThreads, smem, stream>>>(
-            v, pts, val, m, first, cnt, idx->n_deferred, idx->deferred_list, idx->deferred_cap, nullptr, 0, hints);
-        return;
-    }
-    const size_t smem = sizeof(StreamSmem) + (HIST ? sizeof(unsigned int) * (size_t)n_bins : 0);
-    k_pip_stream<LEAN, HIST, false><<<stream_grid<LEAN, HIST, false>(m, smem), kQueryThreads, smem, stream>>>(
-        v, pts, val, m, first, cnt, idx->n_deferred, idx->deferred_list, idx->deferred_cap, hist, n_bins, hints);
+    const size_t smem = sizeof(StreamSmem);
+    int occ = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pip_stream<LEAN>, kQueryThreads, smem) != cudaSuccess || occ < 1) occ = 1;
+    (void)cudaGetLastError();
+    static const int cap = env_int("GPL_PIP_STREAM_CTAS_PER_SM", 0);
+    const int per_sm = cap > 0 ? std::min(cap, occ) : occ;
+    const int64_t want = ceil_div(ceil_div(m, kTilePts), kStreamWarps);
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * per_sm));
+    k_pip_stream<LEAN><<<grid, kQueryThreads, smem, stream>>>(v, pts, val, m, first, cnt, idx->n_deferred, idx->deferred_list,
+                                                              idx->deferred_cap, hints);
+}
+// counts[id] += number of ids equal to id, for every id in [0, n_polys)
+static int launch_histogram(gpl_ctx *ctx, const int32_t *ids, int64_t n, unsigned long long *counts, int64_t n_polys,
+                            cudaStream_t stream) {
+    const bool use_smem = n_polys <= kHistSmemBins;
+    const size_t dyn = use_smem ? sizeof(unsigned int) * (size_t)n_polys : 0;
+    if (dyn > 48 * 1024) GPL_CUDA(cudaFuncSetAttribute(k_histogram, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
+    const int per_sm = use_smem ? (int)std::max<size_t>(1, std::min<size_t>(4, (200 * 1024) / std::max<size_t>(dyn, 1))) : 4;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 2048), (int64_t)kSMs * per_sm));
+    k_histogram<<<grid, 512, dyn, stream>>>(ids, n, counts, n_polys, use_smem ? 1 : 0);
+    ctx->launches++;
+    return GPL_OK;
 }
 // hist (optional, device, n_geoms u64): += number of points whose first containing row is that polygon
 int pip_query(gpl_ctx *ctx, const gpl_pip_index *idx, const double *pts_dev, const uint8_t *validity_dev, int64_t n,
               int32_t *first_dev, int32_t *count_dev, cudaStream_t stream, unsigned long long *hist = nullptr) {
     if (n == 0) return GPL_OK;
-    // Per-polygon counts: a separate pass over the id column (k_histogram) by default; the variant fused into the streaming
-    // kernel (shared-memory bins) is opt-in.
-    static const bool fuse_enabled = env_int("GPL_PIP_FUSE_HIST", 0) != 0;
-    const bool fuse_hist = fuse_enabled && hist != nullptr && idx->n_geoms <= kHistFuseMaxBins;
     const double2 *pts = reinterpret_cast<const double2 *>(pts_dev);
     const IndexView v = view_of(idx);
-    static const bool legacy = env_int("GPL_PIP_LEGACY", 0) != 0;  // round-1 kernel: every point walks (A/B measurements)
     // the deferred list holds chunk-relative uint32 indices: process at most 2^31 points per launch pair
     const int64_t kMaxChunk = 1LL << 31;
     for (int64_t lo = 0; lo < n; lo += kMaxChunk) {
@@ -2039,41 +1957,15 @@ int pip_query(gpl_ctx *ctx, const gpl_pip_index *idx, const double *pts_dev, con
         GPL_CUDA(cudaMemsetAsync(idx->n_deferred, 0, sizeof(unsigned long long), stream));
         const uint8_t *val = validity_dev ? validity_dev + lo / 8 : nullptr;
         int32_t *cnt = count_dev ? count_dev + lo : nullptr;
-        if (legacy) {
-            if (idx->lean_ok)
-                k_pip_query<0, true><<<query_grid(m, true), kQueryThreads, 0, stream>>>(v, pts + lo, val, m, first_dev + lo, cnt, nullptr, nullptr,
-                                                                                    nullptr, lo, idx->n_deferred, idx->deferred_list,
-                                                                                    idx->deferred_cap);
-            else
-                k_pip_query<0, false><<<query_grid(m), kQueryThreads, 0, stream>>>(v, pts + lo, val, m, first_dev + lo, cnt, nullptr, nullptr,
-                                                                                     nullptr, lo, idx->n_deferred, idx->deferred_list,
-                                                                                     idx->deferred_cap);
-        } else {
-            cudaEvent_t t0 = nullptr, t1 = nullptr;
-            if (ctx->kt_on && ctx->kernel_timing_pair(&t0, &t1)) GPL_CUDA(cudaEventRecord(t0, stream));
-            const int32_t nb = (int32_t)idx->n_geoms;
-            if (idx->lean_ok) {
-                if (fuse_hist) launch_stream<true, true>(v, pts + lo, val, m, first_dev + lo, cnt, idx, hist, nb, stream);
-                else launch_stream<true, false>(v, pts + lo, val, m, first_dev + lo, cnt, idx, nullptr, 0, stream);
-            } else {
-                if (fuse_hist) launch_stream<false, true>(v, pts + lo, val, m, first_dev + lo, cnt, idx, hist, nb, stream);
-                else launch_stream<false, false>(v, pts + lo, val, m, first_dev + lo, cnt, idx, nullptr, 0, stream);
-            }
-            if (t1) GPL_CUDA(cudaEventRecord(t1, stream));
-        }
-        const bool fused_here = fuse_hist && !legacy;
+        cudaEvent_t t0 = nullptr, t1 = nullptr;
+        if (ctx->kt_on && ctx->kernel_timing_pair(&t0, &t1)) GPL_CUDA(cudaEventRecord(t0, stream));
+        if (idx->lean_ok) launch_stream<true>(v, pts + lo, val, m, first_dev + lo, cnt, idx, stream);
+        else launch_stream<false>(v, pts + lo, val, m, first_dev + lo, cnt, idx, stream);
+        if (t1) GPL_CUDA(cudaEventRecord(t1, stream));
         k_pip_deferred<<<kSMs * 8, 256, 0, stream>>>(v, pts + lo, m, first_dev + lo, cnt, idx->n_deferred, idx->deferred_list, idx->deferred_cap,
-                                                     idx->n_deferred + 1, fused_here ? hist : nullptr);
+                                                     idx->n_deferred + 1);
         ctx->launches += 2;
-        if (hist && !fused_here) {  // many polygons (or the legacy kernel): count from the id column
-            const bool use_smem = idx->n_geoms <= kHistSmemBins;
-            const size_t dyn = use_smem ? sizeof(unsigned int) * (size_t)idx->n_geoms : 0;
-            if (dyn > 48 * 1024) GPL_CUDA(cudaFuncSetAttribute(k_histogram, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-            const int per_sm = use_smem ? (int)std::max<size_t>(1, std::min<size_t>(4, (200 * 1024) / std::max<size_t>(dyn, 1))) : 4;
-            const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(m, 2048), (int64_t)kSMs * per_sm));
-            k_histogram<<<grid, 512, dyn, stream>>>(first_dev + lo, m, hist, idx->n_geoms, use_smem ? 1 : 0);
-            ctx->launches++;
-        }
+        if (hist) GPL_TRY(launch_histogram(ctx, first_dev + lo, m, hist, idx->n_geoms, stream));  // counts from the id column
     }
     GPL_CUDA(cudaGetLastError());
     return GPL_OK;
@@ -2084,8 +1976,8 @@ int pip_query(gpl_ctx *ctx, const gpl_pip_index *idx, const double *pts_dev, con
 using namespace gpl;
 
 // Keep the hot part of the index slab resident in the 50 MB L2 while 1.6 GB of points stream past it: mark it
-// as a persisting access-policy window on the context stream (the point loads are ld.global.cs,
-// i.e. evict-first).  Best effort: failures only cost performance.  The device-wide carve-out only ever grows while
+// as a persisting access-policy window on the context stream (each point is read once, without an L1
+// line).  Best effort: failures only cost performance.  The device-wide carve-out only ever grows while
 // the context lives and is restored by gpl_ctx_destroy; the window is dropped and the persisting lines are released
 // when the index that set them is freed (neither call waits for running kernels: they are cache hints).
 static void l2_pin(gpl_pip_index *idx, bool on) {
@@ -2302,16 +2194,9 @@ extern "C" int gpl_pip_index_build(gpl_ctx *ctx, const gpl_array *polys, gpl_pip
     a.xy = reinterpret_cast<const double2 *>(polys->xy);
     a.geom_off = polys->geom_off, a.part_off = polys->part_off, a.ring_off = polys->ring_off, a.validity = polys->validity;
     a.slots_x100 = slots_x100, a.G = (int32_t)G, a.rs = rs, a.n_cells = n_cells;
-    {
-        // GPL_PIP_BUILD_LEGACY=1: the previous build (static deal of (part, 32-row) raster items), for A/B measurements
-        static const bool build_legacy = env_int("GPL_PIP_BUILD_LEGACY", 0) != 0;
-        static const int raster_rows = [] {
-            const int v = env_int("GPL_PIP_RASTER_ROWS", 32);  // config 2 on one H100: 8 / 16 / 32 rows, raster phase 173 / 117 / 91 us
-            return v == 8 || v == 16 || v == 32 ? v : 32;
-        }();
-        a.build_legacy = build_legacy ? 1 : 0;
-        a.raster_rows = raster_rows;
-    }
+    // GPL_PIP_BUILD_LEGACY=1: the previous build (static deal of (part, 32-row) raster items), for A/B measurements
+    static const bool build_legacy = env_int("GPL_PIP_BUILD_LEGACY", 0) != 0;
+    a.build_legacy = build_legacy ? 1 : 0;
     // sum of n_buckets <= P + n_coords * 100 / slots_x100 + 1 without a host round trip
     a.NB_cap = Pa + (polys->n_coords * 100) / slots_x100 + 1;
     Scratch<PartHeader> hdr;
@@ -2497,6 +2382,31 @@ extern "C" int gpl_contains_join_array(gpl_ctx *ctx, const gpl_pip_index *idx, c
     return GPL_OK;
 }
 
+// (point, polygon) pairs of n device points, sorted by point: the count pass, the scan of the counts into write offsets, the
+// total (one host round trip), then the write pass.  `outputs(total, &lhs, &rhs)` provides device buffers for `total` pairs,
+// or leaves them NULL to stop after the count.
+template <class Outputs>
+static int pip_pairs(gpl_ctx *ctx, const gpl_pip_index *idx, const double *pts, const uint8_t *validity, int64_t n, Outputs &&outputs) {
+    Scratch<int32_t> ids, cnt;
+    Scratch<int64_t> off;
+    GPL_TRY(ids.get(ctx, (size_t)n));
+    GPL_TRY(cnt.get(ctx, (size_t)n));
+    GPL_TRY(off.get(ctx, (size_t)n + 2));
+    GPL_TRY(pip_query(ctx, idx, pts, validity, n, ids.p, cnt.p, ctx->stream));
+    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n, off.p, off.p + n + 1)));
+    int64_t total = 0;
+    GPL_CUDA(cudaMemcpyAsync(&total, off.p + n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    uint64_t *lhs = nullptr, *rhs = nullptr;
+    GPL_TRY(outputs(total, &lhs, &rhs));
+    if (total == 0 || lhs == nullptr) return GPL_OK;
+    k_pip_pairs<<<query_grid(n), kQueryThreads, 0, ctx->stream>>>(view_of(idx), reinterpret_cast<const double2 *>(pts), validity, n, off.p,
+                                                                  lhs, rhs);
+    ctx->launches++;
+    GPL_CUDA(cudaGetLastError());
+    return GPL_OK;
+}
+
 extern "C" int gpl_contains_join_pairs(gpl_ctx *ctx, const gpl_pip_index *idx, const double *points_xy, int64_t n_points,
                                        uint64_t *lhs, uint64_t *rhs, int64_t *n_pairs, int mem) {
     GPL_REQUIRE(ctx && idx && n_pairs, GPL_ERR_INVALID_ARG, "gpl_contains_join_pairs: NULL argument");
@@ -2512,38 +2422,29 @@ extern "C" int gpl_contains_join_pairs(gpl_ctx *ctx, const gpl_pip_index *idx, c
         GPL_CUDA(cudaMemcpyAsync(pts.p, points_xy, sizeof(double) * 2 * n_points, cudaMemcpyHostToDevice, ctx->stream));
         pdev = pts.p;
     }
-    Scratch<int32_t> ids, cnt;
-    Scratch<int64_t> off;
-    GPL_TRY(ids.get(ctx, (size_t)n_points));
-    GPL_TRY(cnt.get(ctx, (size_t)n_points));
-    GPL_TRY(off.get(ctx, (size_t)n_points + 2));
-    GPL_TRY(pip_query(ctx, idx, pdev, nullptr, n_points, ids.p, cnt.p, ctx->stream));
-    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n_points, off.p, off.p + n_points + 1)));
-    int64_t total = 0;
-    GPL_CUDA(cudaMemcpyAsync(&total, off.p + n_points + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (lhs == nullptr || rhs == nullptr) {
-        *n_pairs = total;
-        return GPL_OK;
-    }
-    GPL_REQUIRE(*n_pairs >= total, GPL_ERR_INVALID_ARG, "pair buffers too small: need %lld, have %lld", (long long)total,
-                (long long)*n_pairs);
-    *n_pairs = total;
-    if (total == 0) return GPL_OK;
     Scratch<uint64_t> dl, dr;
-    uint64_t *pl = lhs, *pr = rhs;
+    int64_t total = 0;
+    GPL_TRY(pip_pairs(ctx, idx, pdev, nullptr, n_points, [&](int64_t t, uint64_t **pl, uint64_t **pr) -> int {
+        total = t;
+        if (lhs == nullptr || rhs == nullptr) {  // the caller asks for the count only
+            *n_pairs = total;
+            return GPL_OK;
+        }
+        GPL_REQUIRE(*n_pairs >= total, GPL_ERR_INVALID_ARG, "pair buffers too small: need %lld, have %lld", (long long)total,
+                    (long long)*n_pairs);
+        *n_pairs = total;
+        *pl = lhs, *pr = rhs;
+        if (mem == GPL_HOST && total > 0) {
+            GPL_TRY(dl.get(ctx, (size_t)total));
+            GPL_TRY(dr.get(ctx, (size_t)total));
+            *pl = dl.p, *pr = dr.p;
+        }
+        return GPL_OK;
+    }));
+    if (lhs == nullptr || rhs == nullptr || total == 0) return GPL_OK;
     if (mem == GPL_HOST) {
-        GPL_TRY(dl.get(ctx, (size_t)total));
-        GPL_TRY(dr.get(ctx, (size_t)total));
-        pl = dl.p, pr = dr.p;
-    }
-    k_pip_query<1><<<query_grid(n_points), kQueryThreads, 0, ctx->stream>>>(view_of(idx), reinterpret_cast<const double2 *>(pdev), nullptr,
-                                                                      n_points, nullptr, nullptr, off.p, pl, pr, 0, nullptr, nullptr, 0);
-    ctx->launches++;
-    GPL_CUDA(cudaGetLastError());
-    if (mem == GPL_HOST) {
-        GPL_CUDA(cudaMemcpyAsync(lhs, pl, sizeof(uint64_t) * total, cudaMemcpyDeviceToHost, ctx->stream));
-        GPL_CUDA(cudaMemcpyAsync(rhs, pr, sizeof(uint64_t) * total, cudaMemcpyDeviceToHost, ctx->stream));
+        GPL_CUDA(cudaMemcpyAsync(lhs, dl.p, sizeof(uint64_t) * total, cudaMemcpyDeviceToHost, ctx->stream));
+        GPL_CUDA(cudaMemcpyAsync(rhs, dr.p, sizeof(uint64_t) * total, cudaMemcpyDeviceToHost, ctx->stream));
     }
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));
     return GPL_OK;
@@ -2559,27 +2460,16 @@ extern "C" int gpl_contains_join_pairs_array(gpl_ctx *ctx, const gpl_pip_index *
     *out = res;
     const int64_t n = points->n_geoms;
     if (n == 0) return GPL_OK;
-    Scratch<int32_t> ids, cnt;
-    Scratch<int64_t> off;
-    GPL_TRY(ids.get(ctx, (size_t)n));
-    GPL_TRY(cnt.get(ctx, (size_t)n));
-    GPL_TRY(off.get(ctx, (size_t)n + 2));
-    GPL_TRY(pip_query(ctx, idx, points->xy, points->validity, n, ids.p, cnt.p, ctx->stream));
-    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n, off.p, off.p + n + 1)));
-    int64_t total = 0;
-    GPL_CUDA(cudaMemcpyAsync(&total, off.p + n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (total == 0) return GPL_OK;
-    void *pl = nullptr, *pr = nullptr;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pl));
-    res->lhs = (uint64_t *)pl;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pr));
-    res->rhs = (uint64_t *)pr;
-    res->n = total;
-    k_pip_query<1><<<query_grid(n), kQueryThreads, 0, ctx->stream>>>(view_of(idx), reinterpret_cast<const double2 *>(points->xy), points->validity, n,
-                                                                nullptr, nullptr, off.p, res->lhs, res->rhs, 0, nullptr, nullptr, 0);
-    ctx->launches++;
-    GPL_CUDA(cudaGetLastError());
+    GPL_TRY(pip_pairs(ctx, idx, points->xy, points->validity, n, [&](int64_t total, uint64_t **pl, uint64_t **pr) -> int {
+        if (total == 0) return GPL_OK;
+        void *q = nullptr;
+        GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &q));
+        res->lhs = *pl = (uint64_t *)q;
+        GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &q));
+        res->rhs = *pr = (uint64_t *)q;
+        res->n = total;
+        return GPL_OK;
+    }));
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));
     return GPL_OK;
 }
@@ -2653,14 +2543,7 @@ extern "C" int gpl_join_histogram(gpl_ctx *ctx, const int32_t *first_id, int64_t
     GPL_REQUIRE(mem == GPL_DEVICE, GPL_ERR_UNSUPPORTED, "gpl_join_histogram: device buffers only");
     GPL_CUDA(cudaSetDevice(ctx->device));
     if (n_points == 0) return GPL_OK;
-    const bool use_smem = n_polygons <= kHistSmemBins;
-    const size_t dyn = use_smem ? sizeof(unsigned int) * (size_t)n_polygons : 0;
-    if (dyn > 48 * 1024) GPL_CUDA(cudaFuncSetAttribute(k_histogram, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-    const int per_sm = use_smem ? (int)std::max<size_t>(1, std::min<size_t>(4, (200 * 1024) / std::max<size_t>(dyn, 1))) : 4;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_points, 2048), (int64_t)kSMs * per_sm));
-    k_histogram<<<grid, 512, dyn, ctx->stream>>>(first_id, n_points, reinterpret_cast<unsigned long long *>(counts), n_polygons,
-                                                 use_smem ? 1 : 0);
-    ctx->launches++;
+    GPL_TRY(launch_histogram(ctx, first_id, n_points, reinterpret_cast<unsigned long long *>(counts), n_polygons, ctx->stream));
     GPL_CUDA(cudaGetLastError());
     return GPL_OK;
 }

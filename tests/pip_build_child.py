@@ -1,7 +1,7 @@
 """Builds the points-in-polygons index of a fixed set of polygon columns and saves its tables; a helper of
 test_gpu_pip_build.py, not a test module.
 
-The build's switches (GPL_PIP_BUILD_LEGACY, GPL_PIP_RASTER_ROWS) are read once per process, so each variant of the build
+The build's switch GPL_PIP_BUILD_LEGACY is read once per process, so each variant of the build
 runs in a fresh process: the test starts this script with the variant's environment and compares what it wrote.
 
     python tests/pip_build_child.py OUTDIR

@@ -1,7 +1,7 @@
 """Runs every entry point of the points-in-polygons join on a fixed set of indexes and saves the outputs; a helper of
 test_gpu_pip_regimes.py, not a test module.
 
-The join's A/B switches (GPL_PIP_LEAN, GPL_PIP_LEGACY, GPL_PIP_CAND_SMEM, GPL_PIP_FUSE_HIST, GPL_PIP_LD_HINTS, ...) are
+The join's A/B switches (GPL_PIP_LEAN, GPL_PIP_LD_HINTS, GPL_PIP_RASTER_LOG2, GPL_PIP_STREAM_CTAS_PER_SM, ...) are
 read once per process, so each kernel variant needs a fresh process: the test starts this script with the variant's
 environment and compares what it wrote with the oracle.
 
@@ -47,12 +47,12 @@ def cases():
     from test_gpu_pip_regimes import field_points, star_field
 
     out = {}
-    out["stars2500"] = star_field(2500, holes=False, seed=1)  # <= 12288 coarse cells and rows: CSM and fused bins eligible
+    out["stars2500"] = star_field(2500, holes=False, seed=1)  # POLYGON rows without holes
     out["field2500"] = star_field(2500, holes=True, seed=2)
     out["multi2500"] = star_field(2500, holes=True, seed=2, multi=True)
     out["holes_multis"] = GeoArrowArray.from_shapes(GeometryType.MULTIPOLYGON, _holes_and_multis())
     out["nested"] = _nested()
-    xy, ro, go = synth.star_polygons(16_900, 130)  # above the fused-histogram bin limit
+    xy, ro, go = synth.star_polygons(16_900, 130)  # the largest case: 16 900 rows
     out["stars16900"] = GeoArrowArray.polygons(xy, ro, go)
     out["one"] = GeoArrowArray.from_shapes(GeometryType.POLYGON, [[[(0.0, 0.0), (4.0, 1.0), (5.0, 5.0), (1.0, 3.5), (0.0, 0.0)]]])
     # one million points on the 16 900 stars: several tiles per warp, so the walk queue carries points across tiles

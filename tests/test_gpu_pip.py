@@ -294,11 +294,9 @@ def test_reference_golden_envelope_queries_gpu(ctx, og, conv):
                               og.envelope_query(conv(mixed), (-1.0, -1.0, 16.0, 16.0), mode))
 
 
-def test_join_counts_fused_histogram(ctx, og, conv):
-    """gpl_contains_join_counts: ids + per-polygon hit counts; boundary points (deferred to the exact kernel) must be counted
-    exactly once.  With the default environment the counts come from the id-column histogram (k_histogram) at both sizes; the
-    bins fused into the streaming kernel (GPL_PIP_FUSE_HIST=1, up to 12288 rows) are tested in a child process by
-    test_gpu_pip_regimes.py::test_kernel_variants_vs_oracle."""
+def test_join_counts_histogram(ctx, og, conv):
+    """gpl_contains_join_counts: ids + per-polygon hit counts from the id-column histogram (k_histogram) at two sizes;
+    boundary points (deferred to the exact kernel) must be counted exactly once."""
     from geopolars_b200.engine import PipIndex
 
     for m, grid in ((400, 20), (16_900, 130)):

@@ -20,12 +20,10 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-_SWITCHES = ("GPL_PIP_BUILD_LEGACY", "GPL_PIP_RASTER_ROWS", "GPL_PIP_RASTER_LOG2", "GPL_PIP_RASTER_MCELLS", "GPL_PIP_SLOTS_X100")
+_SWITCHES = ("GPL_PIP_BUILD_LEGACY", "GPL_PIP_RASTER_LOG2", "GPL_PIP_RASTER_MCELLS", "GPL_PIP_SLOTS_X100")
 VARIANTS = {
     "default": {},
     "legacy": {"GPL_PIP_BUILD_LEGACY": "1"},
-    "rows8": {"GPL_PIP_RASTER_ROWS": "8"},
-    "rows16": {"GPL_PIP_RASTER_ROWS": "16"},
 }
 
 
@@ -44,7 +42,7 @@ def legacy(tmp_path_factory):
     return run_build(tmp_path_factory, "legacy")
 
 
-@pytest.mark.parametrize("variant", ["default", "rows8", "rows16"])
+@pytest.mark.parametrize("variant", ["default"])
 def test_index_identical_to_legacy_build(variant, legacy, tmp_path_factory):
     tables, meta = run_build(tmp_path_factory, variant)
     want_tables, want_meta = legacy

@@ -217,10 +217,6 @@ def test_index_regimes_vs_oracle(ctx, og, conv, form, P, rs, G):
 VARIANTS = {
     "default": {},
     "lean0": {"GPL_PIP_LEAN": "0"},
-    "legacy": {"GPL_PIP_LEGACY": "1"},
-    "legacy-lean0": {"GPL_PIP_LEGACY": "1", "GPL_PIP_LEAN": "0"},
-    "cand-smem": {"GPL_PIP_CAND_SMEM": "1"},
-    "fuse-hist": {"GPL_PIP_FUSE_HIST": "1"},
     **{f"ld-hints{h}": {"GPL_PIP_LD_HINTS": str(h)} for h in (0, 1, 2, 3, 4, 6, 7)},
     "one-cta-per-sm": {"GPL_PIP_STREAM_CTAS_PER_SM": "1", "GPL_PIP_CTAS_PER_SM": "1"},
     **{f"raster-log2-{k}": {"GPL_PIP_RASTER_LOG2": str(k)} for k in (0, 1, 2, 3)},
@@ -229,7 +225,7 @@ VARIANTS = {
     "slots-6400": {"GPL_PIP_SLOTS_X100": "6400"},
     "no-l2-pin": {"GPL_L2_PIN": "0"},
 }
-_SWITCHES = sorted({k for v in VARIANTS.values() for k in v} | {"GPL_PIP_LEAN_CTAS_PER_SM", "GPL_PIP_NOALLOC"})
+_SWITCHES = sorted({k for v in VARIANTS.values() for k in v})
 
 
 def run_variant(tmp_path_factory, name):
@@ -262,9 +258,9 @@ def control(tmp_path_factory):
 @pytest.mark.parametrize("variant", list(VARIANTS))
 def test_kernel_variants_vs_oracle(variant, variant_oracle, control, tmp_path_factory):
     """every entry point under every A/B switch.  Where the ABI shows the path taken, the test asserts it: raster_log2 and
-    fine_cells_per_axis for the raster switches, the index bytes for the bucket sizing, one launch fewer for query_counts
-    with fused bins, no kernel-timing pair for the round-1 kernel.  Nothing in the ABI shows whether the LEAN walk, the
-    shared-memory candidate rows or a cache-hint variant ran; those variants are checked on their outputs only."""
+    fine_cells_per_axis for the raster switches, the index bytes for the bucket sizing, the launches of query_counts and
+    one kernel-timing pair per query.  Nothing in the ABI shows whether the LEAN walk, a cache-hint variant or one CTA per SM
+    ran; those variants are checked on their outputs only."""
     res, meta = control if variant == "default" else run_variant(tmp_path_factory, variant)
     _, cmeta = control
     for name, o in variant_oracle.items():
@@ -296,12 +292,8 @@ def test_kernel_variants_vs_oracle(variant, variant_oracle, control, tmp_path_fa
             assert st["bytes"] <= cst["bytes"] and (st["bytes"] < cst["bytes"] or name in ("one", "holes_multis")), (name, st["bytes"])
         elif st["raster_log2"] == cst["raster_log2"]:
             assert st["bytes"] == cst["bytes"], name
-        fused = variant == "fuse-hist" and o["n_geoms"] <= 12288
-        assert meta[name]["launches_counts"] == cmeta[name]["launches_counts"] - int(fused), (name, meta[name], cmeta[name])
-        legacy = "GPL_PIP_LEGACY" in env
-        assert meta[name]["timed_stream_launches"] == (0 if legacy else 1), (name, meta[name])
-    if variant == "fuse-hist":
-        assert any(o["n_geoms"] <= 12288 for o in variant_oracle.values())
+        assert meta[name]["launches_counts"] == cmeta[name]["launches_counts"], (name, meta[name], cmeta[name])
+        assert meta[name]["timed_stream_launches"] == 1, (name, meta[name])
     if "GPL_PIP_RASTER_MCELLS" in VARIANTS[variant]:  # the budget, not the 2^7 cap, set the resolution somewhere
         assert any(meta[k]["stats"]["raster_log2"] < cmeta[k]["stats"]["raster_log2"] for k in meta)
 

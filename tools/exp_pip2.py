@@ -1,6 +1,6 @@
 """PIP experiments on one GPU: build time, query time, raster census for the config-2 workload.
 Knobs are read by the library at load time (environment): GPL_PIP_RASTER_LOG2, GPL_PIP_RASTER_MCELLS,
-GPL_PIP_SLOTS_X100, GPL_PIP_LEGACY, GPL_PIP_STREAM_CTAS_PER_SM, GPL_L2_PIN.  One JSON line per run.
+GPL_PIP_SLOTS_X100, GPL_PIP_LEAN, GPL_PIP_STREAM_CTAS_PER_SM, GPL_L2_PIN.  One JSON line per run.
 
   python tools/exp_pip2.py [--points N] [--polys M --grid G] [--reps R] [--tag TAG]
 """
