@@ -202,8 +202,6 @@ struct BuildArgs {
     const uint8_t *validity;
     int slots_x100;
     int32_t G, rs;
-    int32_t build_legacy;    // 1: the previous work distribution (A/B): one thread per y-bucket in ph_bucket_finish,
-                             //    raster items dealt out statically, it += nwarps
     int64_t n_cells, NB_cap;
     // phase 1 (scratch)
     PartHeader *hdr;
@@ -599,116 +597,13 @@ __device__ void ph_fast_plan(const BuildArgs &a) {
         if (not_fast) atomicAdd(a.acc + ACC_NOT_FAST, not_fast);
     }
 }
-// One THREAD per y-bucket finishes it: orders the bucket's edge ids where a consumer needs it (parts with holes),
-// materialises the 32-byte f64 records (+ ring index when holes exist) and writes the bucket's two FP32 lists (header, float
-// edges relative to the part origin, sentinels, overflow records).  Round 2's first build did these as three warp-per-part
-// phases separated by grid barriers; a part's ~22 buckets then cost ~44 dependent L2 round trips per warp.  Here every
-// load of a bucket (edge ids, coordinates) is independent of the others and 227 k buckets run side by side.
-__device__ void ph_bucket_finish(const BuildArgs &a, const int32_t *__restrict__ bstart) {
-    const int64_t tid = (int64_t)blockIdx.x * kBuildThreads + threadIdx.x, nth = (int64_t)gridDim.x * kBuildThreads;
-    const float inf = __int_as_float(0x7f800000);
-    const float4 sentinel = make_float4(0.0f, inf, 0.0f, inf);  // inert: +inf ordinates never straddle a finite p.y
-    for (int64_t gb = tid; gb < a.n_buckets; gb += nth) {
-        const int32_t e0 = bstart[gb], n = bstart[gb + 1] - e0;
-        const int32_t p = a.bucket_part[gb];
-        const PartHeader h = a.hdr[p];
-        int64_t r0, r1;
-        part_rings(a.type, p, a.geom_off, a.part_off, r0, r1);
-        // ---- order: parts WITH holes need their entries grouped by ring (ascending edge id does it: the bucket walk switches
-        // ring when the ring index changes).  For a hole-free part the order in which the atomic cursors filled the bucket is
-        // irrelevant to every consumer (winding sums and the two one-sided lists are order-independent), so it is kept.
-        if (h.flags & 1) {
-            int64_t *g = a.entry_edge + e0;
-            for (int32_t i = 1; i < n; ++i) {
-                const int64_t v = g[i];
-                int32_t j = i - 1;
-                while (j >= 0 && g[j] > v) {
-                    g[j + 1] = g[j];
-                    --j;
-                }
-                g[j + 1] = v;
-            }
-        }
-        // ---- FP32 lists of this bucket (plain parts only)
-        const bool fast = a.fast_c[p] > 0;
-        const int32_t b = (int32_t)(gb - h.bucket_base);
-        float4 *base = nullptr, *list0 = nullptr, *list1 = nullptr;
-        int2 ovf = make_int2(0, 0);
-        double ox = 0.0, mx = 0.0, oy = 0.0, xm = 0.0;
-        if (fast) {
-            base = a.fast + (int64_t)a.fast_slots[p];
-            list0 = base + ((int64_t)b * 2) * kFastListRecs, list1 = list0 + kFastListRecs;
-            ovf = a.ovf_off[gb];
-            ox = (double)__double2float_rd(h.xmin), mx = (double)__double2float_ru(h.xmax), oy = h.by0;
-            xm = fast_split_x(h);  // == 0.5 * (ox + mx); the query kernel forms it from PartLite
-        }
-        int32_t c0 = 0, c1 = 0;  // lengths of the two one-sided lists
-        const int64_t ext0 = a.ring_off[r0], ext1 = a.ring_off[r0 + 1];
-        // four entries at a time: their edge ids, then their coordinates, are loaded together (read-only path) before
-        // anything is stored — one entry per iteration cost two dependent L2 round trips each
-        for (int32_t k0 = 0; k0 < n; k0 += 4) {
-            const int32_t mm = min(4, n - k0);
-            int64_t cc[4], rr[4];
-            double2 ss[4], ee[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) cc[j] = j < mm ? __ldg(a.entry_edge + e0 + k0 + j) : ext0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                int64_t r = r0, rc0 = ext0, rc1 = ext1;
-                if (h.flags & 1) {  // ring of coordinate c: rings of a part are few; linear search from the exterior
-                    while (r + 1 < r1 && a.ring_off[r + 1] <= cc[j]) ++r;
-                    rc0 = a.ring_off[r], rc1 = a.ring_off[r + 1];
-                }
-                rr[j] = r - r0;
-                // edge_of_slot on the read-only path: (c -> c+1), or the closing edge back to the ring's first coordinate,
-                // or the degenerate edge of a 1-coordinate ring (entries never name a "no edge" slot)
-                ss[j] = __ldg(a.xy + cc[j]);
-                ee[j] = cc[j] + 1 < rc1 ? __ldg(a.xy + cc[j] + 1) : (rc1 - rc0 == 1 ? ss[j] : __ldg(a.xy + rc0));
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                if (j >= mm) break;
-                const double2 s = ss[j], e = ee[j];
-                const int32_t k = k0 + j;
-                EdgeRec rec;
-                rec.sx = s.x, rec.sy = s.y, rec.ex = e.x, rec.ey = e.y;
-                a.entries[e0 + k] = rec;
-                if (a.entry_ring) a.entry_ring[e0 + k] = (int32_t)rr[j];
-                if (fast) {
-                    if (fmax(s.x, e.x) >= xm) {  // right-hand list: coordinates relative to (xminf, yminf)
-                        const float4 f = make_float4(__double2float_rn(s.x - ox), __double2float_rn(s.y - oy), __double2float_rn(e.x - ox),
-                                                     __double2float_rn(e.y - oy));
-                        if (c0 < kFastListRecs - 1) list0[1 + c0] = f;
-                        else base[ovf.x + c0 - (kFastListRecs - 1)] = f;
-                        ++c0;
-                    }
-                    if (fmin(s.x, e.x) <= xm) {  // left-hand list, mirrored in x
-                        const float4 f = make_float4(__double2float_rn(mx - s.x), __double2float_rn(s.y - oy), __double2float_rn(mx - e.x),
-                                                     __double2float_rn(e.y - oy));
-                        if (c1 < kFastListRecs - 1) list1[1 + c1] = f;
-                        else base[ovf.y + c1 - (kFastListRecs - 1)] = f;
-                        ++c1;
-                    }
-                }
-            }
-        }
-        if (fast) {
-            for (int32_t k = c0; k < kFastListRecs - 1; ++k) list0[1 + k] = sentinel;
-            for (int32_t k = c1; k < kFastListRecs - 1; ++k) list1[1 + k] = sentinel;
-            const int32_t n0 = max(c0 - (kFastListRecs - 1), 0), n1 = max(c1 - (kFastListRecs - 1), 0);
-            list0[0] = make_float4(__int_as_float(c0), __int_as_float(n0 ? ovf.x : 0), 0.0f, 0.0f);
-            list1[0] = make_float4(__int_as_float(c1), __int_as_float(n1 ? ovf.y : 0), 0.0f, 0.0f);
-            if (n0 & 1) base[ovf.x + n0] = sentinel;  // overflow runs are padded to an even number of records
-            if (n1 & 1) base[ovf.y + n1] = sentinel;
-        }
-    }
-}
-
-// The same bucket finishing with a GROUP of kFinishLanes lanes per y-bucket, one entry per lane: the edge ids are read
-// coalesced, the f64 records leave as contiguous runs, and each lane finds its slot in the two FP32 lists from a ballot
-// (prefix count of the earlier entries on that side), so every record lands where the serial loop above puts it.  On config 2
-// (110 k buckets of 9-20 entries) one thread per bucket issued every load and store of a bucket from one lane, ~30 partly
-// used sectors per warp instruction, and the phase took 0.48 ms on one H100.
+// Finishes every y-bucket: orders the bucket's edge ids where a consumer needs it (parts with holes), materialises the
+// 32-byte f64 records (+ ring index when holes exist) and writes the bucket's two FP32 lists (header, float edges relative
+// to the part origin, sentinels, overflow records).  A GROUP of kFinishLanes lanes takes one bucket, one entry per lane: the
+// edge ids are read coalesced, the f64 records leave as contiguous runs, and each lane finds its slot in the two FP32 lists
+// from a ballot (prefix count of the group's earlier entries on that side), so within each list the entries keep their
+// order in the bucket.  On config 2 (110 k buckets of 9-20 entries) one thread per bucket issued every load and store of a
+// bucket from one lane, ~30 partly used sectors per warp instruction, and the phase took 0.48 ms on one H100.
 constexpr int kFinishLanes = 8;
 __device__ void ph_bucket_finish_groups(const BuildArgs &a, const int32_t *__restrict__ bstart) {
     constexpr int GS = kFinishLanes, GPW = 32 / GS;  // lanes per bucket, buckets per warp
@@ -717,7 +612,7 @@ __device__ void ph_bucket_finish_groups(const BuildArgs &a, const int32_t *__res
     const int64_t warp = ((int64_t)blockIdx.x * kBuildThreads + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * kBuildThreads) >> 5;
     const float inf = __int_as_float(0x7f800000);
-    const float4 sentinel = make_float4(0.0f, inf, 0.0f, inf);
+    const float4 sentinel = make_float4(0.0f, inf, 0.0f, inf);  // inert: +inf ordinates never straddle a finite p.y
     // warp-uniform trip counts: every __ballot_sync / __shfl_sync below sees all 32 lanes
     for (int64_t base = warp * GPW; base < a.n_buckets; base += nwarps * GPW) {
         const int64_t gb = base + grp;
@@ -732,7 +627,8 @@ __device__ void ph_bucket_finish_groups(const BuildArgs &a, const int32_t *__res
         } else {
             h.flags = 0, h.bucket_base = 0;
         }
-        // parts with holes: entries ascending by edge id (grouped by ring), as ph_bucket_finish orders them
+        // parts with holes: entries sorted by ascending edge id, which groups them by ring (the bucket walk switches ring
+        // when the ring index changes).  A hole-free part keeps the order the atomic cursors gave: no consumer depends on it.
         if (have && (h.flags & 1) && sub == 0) {
             int64_t *g = a.entry_edge + e0;
             for (int32_t i = 1; i < n; ++i) {
@@ -810,7 +706,7 @@ __device__ void ph_bucket_finish_groups(const BuildArgs &a, const int32_t *__res
                 const int32_t n0 = max(c0 - (kFastListRecs - 1), 0), n1 = max(c1 - (kFastListRecs - 1), 0);
                 list0[0] = make_float4(__int_as_float(c0), __int_as_float(n0 ? ovf.x : 0), 0.0f, 0.0f);
                 list1[0] = make_float4(__int_as_float(c1), __int_as_float(n1 ? ovf.y : 0), 0.0f, 0.0f);
-                if (n0 & 1) fbase[ovf.x + n0] = sentinel;
+                if (n0 & 1) fbase[ovf.x + n0] = sentinel;  // overflow runs are padded to an even number of records
                 if (n1 & 1) fbase[ovf.y + n1] = sentinel;
             }
         }
@@ -1045,8 +941,6 @@ struct RasterSmem {
 };
 __device__ void ph_raster(const BuildArgs &a, const GridParams &g, const int32_t *__restrict__ cell_start, RasterSmem &sm) {
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int64_t warp = ((int64_t)blockIdx.x * kBuildThreads + threadIdx.x) >> 5;
-    const int64_t nwarps = ((int64_t)gridDim.x * kBuildThreads) >> 5;
     if (g.inv_fw == 0.0 || g.inv_fh == 0.0) return;  // degenerate axis: the raster was filled with 3 (fill kernel, T0)
     int32_t *cnt = sm.cnt[wid];
     uint32_t *list = sm.list[wid];
@@ -1054,8 +948,7 @@ __device__ void ph_raster(const BuildArgs &a, const GridParams &g, const int32_t
     // work item = (part, k): the chunks ra = fy0 + R (k + K j) of the part, R = 32 fine rows each (one lane per row).  A
     // part's bbox is about one coarse cell high, i.e. K = 2^rs / R chunks; they are independent (every raster write is an
     // atomicOr).  Items are claimed from a global counter: a warp that finishes early takes the next one, so the phase ends
-    // one small item after the work runs out instead of after a last, partly filled wave of a static deal.  Legacy (A/B):
-    // item it to warp it mod nwarps.
+    // one small item after the work runs out instead of after a last, partly filled wave of a static deal.
     constexpr int32_t R = 32;
     const int32_t K = max(1, (1 << g.rs) / R);
     auto claim = [&]() -> int64_t {
@@ -1064,7 +957,7 @@ __device__ void ph_raster(const BuildArgs &a, const GridParams &g, const int32_t
         return (int64_t)__shfl_sync(0xffffffffu, v, 0);
     };
     const int64_t n_items = a.P * K;
-    for (int64_t it = a.build_legacy ? warp : claim(); it < n_items; it = a.build_legacy ? it + nwarps : claim()) {
+    for (int64_t it = claim(); it < n_items; it = claim()) {
         const int64_t p = it / K;
         const int32_t kk = (int32_t)(it - p * K);
         const PartHeader h = a.hdr[p];
@@ -1291,8 +1184,7 @@ __global__ void __launch_bounds__(kBuildThreads, 3) k_pip_build_fill(const Build
     GPL_STAMP(a, 8);
     // T3: candidate lists in ascending order; every y-bucket finished by a group of lanes (sort, f64 records, FP32 lists)
     ph_sort_segments<int32_t>(a.items, cell_start, a.n_cells);
-    if (a.build_legacy) ph_bucket_finish(a, bstart);
-    else ph_bucket_finish_groups(a, bstart);
+    ph_bucket_finish_groups(a, bstart);
     ph_part_recs(a);
     for (int64_t b = tid; b < a.n_buckets; b += nth) a.bucket_range[b] = make_int2(bstart[b], bstart[b + 1]);
     grid.sync();
@@ -1900,10 +1792,9 @@ static int env_int(const char *name, int dflt) {
 }
 
 static int query_grid(int64_t n) {
-    // persistent-style: 132 SMs x resident CTAs, grid-stride over the point stream
-    static const int per_sm = env_int("GPL_PIP_CTAS_PER_SM", 8);
+    // persistent-style: 132 SMs x 8 resident CTAs, grid-stride over the point stream
     int64_t want = ceil_div(n, kQueryThreads);
-    return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * per_sm));
+    return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * 8));
 }
 // the streaming kernel on exactly the resident CTAs (persistent warps, one tile of 128 points per warp and iteration)
 template <bool LEAN>
@@ -1916,10 +1807,8 @@ static void launch_stream(const IndexView &v, const double2 *pts, const uint8_t 
     int occ = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pip_stream<LEAN>, kQueryThreads, smem) != cudaSuccess || occ < 1) occ = 1;
     (void)cudaGetLastError();
-    static const int cap = env_int("GPL_PIP_STREAM_CTAS_PER_SM", 0);
-    const int per_sm = cap > 0 ? std::min(cap, occ) : occ;
     const int64_t want = ceil_div(ceil_div(m, kTilePts), kStreamWarps);
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * per_sm));
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * occ));
     k_pip_stream<LEAN><<<grid, kQueryThreads, smem, stream>>>(v, pts, val, m, first, cnt, idx->n_deferred, idx->deferred_list,
                                                               idx->deferred_cap, hints);
 }
@@ -1982,8 +1871,7 @@ using namespace gpl;
 // when the index that set them is freed (neither call waits for running kernels: they are cache hints).
 static void l2_pin(gpl_pip_index *idx, bool on) {
     gpl_ctx *ctx = idx->ctx;
-    static const bool enabled = env_int("GPL_L2_PIN", 1) != 0;
-    if (!enabled || ctx->l2_persist_max == 0 || ctx->l2_window_max == 0) return;
+    if (ctx->l2_persist_max == 0 || ctx->l2_window_max == 0) return;
     cudaStreamAttrValue attr;
     memset(&attr, 0, sizeof(attr));
     if (on) {
@@ -2194,9 +2082,6 @@ extern "C" int gpl_pip_index_build(gpl_ctx *ctx, const gpl_array *polys, gpl_pip
     a.xy = reinterpret_cast<const double2 *>(polys->xy);
     a.geom_off = polys->geom_off, a.part_off = polys->part_off, a.ring_off = polys->ring_off, a.validity = polys->validity;
     a.slots_x100 = slots_x100, a.G = (int32_t)G, a.rs = rs, a.n_cells = n_cells;
-    // GPL_PIP_BUILD_LEGACY=1: the previous build (static deal of (part, 32-row) raster items), for A/B measurements
-    static const bool build_legacy = env_int("GPL_PIP_BUILD_LEGACY", 0) != 0;
-    a.build_legacy = build_legacy ? 1 : 0;
     // sum of n_buckets <= P + n_coords * 100 / slots_x100 + 1 without a host round trip
     a.NB_cap = Pa + (polys->n_coords * 100) / slots_x100 + 1;
     Scratch<PartHeader> hdr;
@@ -2268,11 +2153,8 @@ extern "C" int gpl_pip_index_build(gpl_ctx *ctx, const gpl_array *polys, gpl_pip
     const size_t o_defer = carve(2 * sizeof(unsigned long long));
     const size_t o_phase = carve(16 * sizeof(unsigned long long));
     const bool all_fast = idx->n_fast > 0 && !idx->multi && !idx->any_holes;
-    {
-        static const bool lean_enabled = env_int("GPL_PIP_LEAN", 1) != 0;  // GPL_PIP_LEAN=0 forces the full walk (A/B measurements)
-        // POLYGON rows without holes, every valid part has FP32 lists (cells may hold several candidates)
-        idx->lean_ok = lean_enabled && all_fast && idx->n_not_fast == 0;
-    }
+    // POLYGON rows without holes, every valid part has FP32 lists (cells may hold several candidates)
+    idx->lean_ok = all_fast && idx->n_not_fast == 0;
     const size_t hot_mark = off;
     const size_t o_entries = carve(sizeof(EdgeRec) * (idx->n_entries + 1));
     const size_t o_ring = idx->any_holes ? carve(sizeof(int32_t) * (idx->n_entries + 1)) : 0;

@@ -1,9 +1,9 @@
 """Runs every entry point of the points-in-polygons join on a fixed set of indexes and saves the outputs; a helper of
 test_gpu_pip_regimes.py, not a test module.
 
-The join's A/B switches (GPL_PIP_LEAN, GPL_PIP_LD_HINTS, GPL_PIP_RASTER_LOG2, GPL_PIP_STREAM_CTAS_PER_SM, ...) are
-read once per process, so each kernel variant needs a fresh process: the test starts this script with the variant's
-environment and compares what it wrote with the oracle.
+The join's switches (GPL_PIP_LD_HINTS, GPL_PIP_RASTER_LOG2, GPL_PIP_RASTER_MCELLS, GPL_PIP_SLOTS_X100) are read once
+per process, so each variant needs a fresh process: the test starts this script with the variant's environment and
+compares what it wrote with the oracle.
 
     python tests/pip_variant_child.py OUTDIR
 

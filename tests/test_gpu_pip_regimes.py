@@ -5,7 +5,8 @@ A. Index regimes reached by real inputs: the raster resolution rs falls from 7 t
    32 M fine cells, G = ceil(sqrt(P)) coarse cells per axis).  Below rs = 4 one raster word spans several coarse cells, so
    stage 2 of the streaming kernel takes candidate #0 from cand01; with G odd the last word of a row is only partly used;
    from 4.19 M parts G is capped at 2048 and coarse cells hold several parts.
-B. Kernel variants: the A/B switches are read once per process, so every variant runs in a child process
+B. Kernel variants and index geometries: the load-hint switch and the three seams that set the raster resolution, the
+   raster budget and the bucket sizing are read once per process, so every variant runs in a child process
    (pip_variant_child.py) that writes its outputs to a directory and exits before they are compared.
 C. Entry points: null rows in a Point column, the pipelined host path, the per-polygon histograms, more than 2^31 points.
 
@@ -216,14 +217,11 @@ def test_index_regimes_vs_oracle(ctx, og, conv, form, P, rs, G):
 # ---- B. kernel variants in child processes ----------------------------------------------------------------------------------
 VARIANTS = {
     "default": {},
-    "lean0": {"GPL_PIP_LEAN": "0"},
     **{f"ld-hints{h}": {"GPL_PIP_LD_HINTS": str(h)} for h in (0, 1, 2, 3, 4, 6, 7)},
-    "one-cta-per-sm": {"GPL_PIP_STREAM_CTAS_PER_SM": "1", "GPL_PIP_CTAS_PER_SM": "1"},
     **{f"raster-log2-{k}": {"GPL_PIP_RASTER_LOG2": str(k)} for k in (0, 1, 2, 3)},
     "raster-1mcells": {"GPL_PIP_RASTER_MCELLS": "1"},
     "slots-25": {"GPL_PIP_SLOTS_X100": "25"},
     "slots-6400": {"GPL_PIP_SLOTS_X100": "6400"},
-    "no-l2-pin": {"GPL_L2_PIN": "0"},
 }
 _SWITCHES = sorted({k for v in VARIANTS.values() for k in v})
 
@@ -257,10 +255,10 @@ def control(tmp_path_factory):
 
 @pytest.mark.parametrize("variant", list(VARIANTS))
 def test_kernel_variants_vs_oracle(variant, variant_oracle, control, tmp_path_factory):
-    """every entry point under every A/B switch.  Where the ABI shows the path taken, the test asserts it: raster_log2 and
+    """every entry point under every switch.  Where the ABI shows the path taken, the test asserts it: raster_log2 and
     fine_cells_per_axis for the raster switches, the index bytes for the bucket sizing, the launches of query_counts and
-    one kernel-timing pair per query.  Nothing in the ABI shows whether the LEAN walk, a cache-hint variant or one CTA per SM
-    ran; those variants are checked on their outputs only."""
+    one kernel-timing pair per query.  Nothing in the ABI shows which load-hint variant ran; those variants are checked on
+    their outputs only."""
     res, meta = control if variant == "default" else run_variant(tmp_path_factory, variant)
     _, cmeta = control
     for name, o in variant_oracle.items():

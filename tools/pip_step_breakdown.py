@@ -16,7 +16,7 @@ inputs and prints ONE JSON line with min and median over `--reps` steps of:
 
     python tools/pip_step_breakdown.py [--workload c2|c4] [--reps 20] [--warmup 5] [--points N] [--out FILE]
 
-The environment switches of the library (e.g. GPL_PIP_BUILD_LEGACY=1) apply as in bench.py.  Needs a CUDA device."""
+Needs a CUDA device."""
 import argparse
 import json
 import os
@@ -180,7 +180,6 @@ def main():
         "points": n,
         "polygons": n_polys,
         "reps": args.reps,
-        "build_legacy": os.environ.get("GPL_PIP_BUILD_LEGACY", "0"),
         "card": card(),
         "step_ms": stat(step_ms),
         "step_ms_back_to_back": round(step_ms_back_to_back, 4),
