@@ -47,6 +47,10 @@ pub struct GplPairs {
 pub struct GplNearestIndex {
     _p: [u8; 0],
 }
+#[repr(C)]
+pub struct GplGeoIndex {
+    _p: [u8; 0],
+}
 
 const GPL_HOST: c_int = 0;
 const GPL_ORIGIN_CENTROID: c_int = 0;
@@ -95,6 +99,17 @@ extern "C" {
     fn gpl_nearest_join_geom_pairs(ctx: *mut GplCtx, idx: *const GplNearestIndex, lhs: *const GplArray, max_distance: f64, out: *mut *mut GplPairs, distance: *mut f64, mem: c_int) -> c_int;
     fn gpl_dwithin_join_pairs(ctx: *mut GplCtx, idx: *const GplNearestIndex, lhs: *const GplArray, distance: f64, with_distance: c_int, out: *mut *mut GplPairs) -> c_int;
     fn gpl_pairs_copy_distance(ctx: *mut GplCtx, pairs: *const GplPairs, distance: *mut f64, mem: c_int) -> c_int;
+    fn gpl_haversine_distance(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, out: *mut f64, out_validity: *mut u8, mem: c_int) -> c_int;
+    fn gpl_geo_index_build(ctx: *mut GplCtx, rhs: *const GplArray, out: *mut *mut GplGeoIndex) -> c_int;
+    fn gpl_geo_index_free(idx: *mut GplGeoIndex);
+    #[allow(dead_code)] // diagnostics
+    fn gpl_geo_index_stats(ctx: *mut GplCtx, idx: *const GplGeoIndex, out8: *mut i64) -> c_int;
+    #[allow(dead_code)] // the dense forms: the pair lists below carry the same rows
+    fn gpl_geo_dwithin_count(ctx: *mut GplCtx, idx: *const GplGeoIndex, lhs: *const GplArray, distance: f64, count: *mut i32, mem: c_int) -> c_int;
+    #[allow(dead_code)]
+    fn gpl_geo_nearest_join(ctx: *mut GplCtx, idx: *const GplGeoIndex, lhs: *const GplArray, max_distance: f64, nearest_id: *mut i32, distance: *mut f64, n_tied: *mut i32, mem: c_int) -> c_int;
+    fn gpl_geo_dwithin_join_pairs(ctx: *mut GplCtx, idx: *const GplGeoIndex, lhs: *const GplArray, distance: f64, with_distance: c_int, out: *mut *mut GplPairs) -> c_int;
+    fn gpl_geo_nearest_join_pairs(ctx: *mut GplCtx, idx: *const GplGeoIndex, lhs: *const GplArray, max_distance: f64, out: *mut *mut GplPairs, distance: *mut f64, mem: c_int) -> c_int;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -400,6 +415,14 @@ pub trait GeoSeriesB200Ext {
     /// `sjoin(predicate="dwithin", distance)`): every right row at distance <= `distance` (inclusive; finite and >= 0), as
     /// (lhs_index, rhs_index, distance) sorted by (lhs, rhs); the distance is exactly what `self.distance(rhs)` computes
     fn dwithin_join_pairs(&self, rhs: &Series, distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
+    /// row-wise great-circle distance in metres of two Point columns in (lon, lat) degrees: geo's `HaversineDistance`
+    /// (mean sphere), the value `geodesic_length(Haversine)` sums over segments; null or empty points give null
+    fn haversine_distance(&self, other: &Series) -> Result<Series>;
+    /// `nearest_join_pairs` for two Point columns in (lon, lat) degrees with `haversine_distance` as the distance
+    /// (metres); rows outside |lat| <= 90, |lon| <= 360 match nothing
+    fn geo_nearest_join_pairs(&self, rhs: &Series, max_distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
+    /// `dwithin_join_pairs` for two Point columns in (lon, lat) degrees with `haversine_distance` as the distance (metres)
+    fn geo_dwithin_join_pairs(&self, rhs: &Series, distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
 }
 
 impl GeoSeriesB200Ext for Series {
@@ -469,6 +492,63 @@ impl GeoSeriesB200Ext for Series {
         let mut pairs = std::ptr::null_mut();
         let rc = unsafe { gpl_dwithin_join_pairs(ctx, idx, a.0, distance, 1, &mut pairs) };
         unsafe { gpl_nearest_index_free(idx) };
+        if rc != 0 && !pairs.is_null() {
+            unsafe { gpl_pairs_free(pairs) };
+        }
+        check(rc)?;
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r, mut d) = (vec![0u64; n], vec![0u64; n], vec![0f64; n]);
+        let mut rc = 0;
+        if n > 0 {
+            rc = unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) };
+            if rc == 0 {
+                rc = unsafe { gpl_pairs_copy_distance(ctx, pairs, d.as_mut_ptr(), GPL_HOST) };
+            }
+        }
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
+        Ok((l, r, d))
+    }
+
+    fn haversine_distance(&self, other: &Series) -> Result<Series> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, other)?);
+        let mut v = vec![0f64; self.len()];
+        let mut valid = vec![0u8; (self.len() + 7) / 8];
+        check(unsafe { gpl_haversine_distance(ctx, a.0, b.0, v.as_mut_ptr(), valid.as_mut_ptr(), GPL_HOST) })?;
+        Ok(f64_series("haversine_distance", v, valid))
+    }
+
+    fn geo_nearest_join_pairs(&self, rhs: &Series, max_distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let mut idx = std::ptr::null_mut();
+        check(unsafe { gpl_geo_index_build(ctx, b.0, &mut idx) })?;
+        let mut dist = vec![0f64; self.len()];
+        let mut pairs = std::ptr::null_mut();
+        let rc = unsafe { gpl_geo_nearest_join_pairs(ctx, idx, a.0, max_distance, &mut pairs, dist.as_mut_ptr(), GPL_HOST) };
+        unsafe { gpl_geo_index_free(idx) };
+        if rc != 0 && !pairs.is_null() {
+            unsafe { gpl_pairs_free(pairs) };
+        }
+        check(rc)?;
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r) = (vec![0u64; n], vec![0u64; n]);
+        let rc = if n > 0 { unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) } } else { 0 };
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
+        let d = l.iter().map(|&i| dist[i as usize]).collect();
+        Ok((l, r, d))
+    }
+
+    fn geo_dwithin_join_pairs(&self, rhs: &Series, distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let mut idx = std::ptr::null_mut();
+        check(unsafe { gpl_geo_index_build(ctx, b.0, &mut idx) })?;
+        let mut pairs = std::ptr::null_mut();
+        let rc = unsafe { gpl_geo_dwithin_join_pairs(ctx, idx, a.0, distance, 1, &mut pairs) };
+        unsafe { gpl_geo_index_free(idx) };
         if rc != 0 && !pairs.is_null() {
             unsafe { gpl_pairs_free(pairs) };
         }

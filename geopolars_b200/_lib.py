@@ -167,6 +167,14 @@ SIGNATURES = {
     "gpl_dwithin_count": (_INT, [_P, _P, _P, _D, _P, _INT]),
     "gpl_dwithin_join_pairs": (_INT, [_P, _P, _P, _D, _INT, C.POINTER(_P)]),
     "gpl_pairs_copy_distance": (_INT, [_P, _P, _P, _INT]),
+    "gpl_haversine_distance": (_INT, [_P, _P, _P, _P, _P, _INT]),
+    "gpl_geo_index_build": (_INT, [_P, _P, C.POINTER(_P)]),
+    "gpl_geo_index_free": (None, [_P]),
+    "gpl_geo_index_stats": (_INT, [_P, _P, _P]),
+    "gpl_geo_dwithin_count": (_INT, [_P, _P, _P, _D, _P, _INT]),
+    "gpl_geo_dwithin_join_pairs": (_INT, [_P, _P, _P, _D, _INT, C.POINTER(_P)]),
+    "gpl_geo_nearest_join": (_INT, [_P, _P, _P, _D, _P, _P, _P, _INT]),
+    "gpl_geo_nearest_join_pairs": (_INT, [_P, _P, _P, _D, C.POINTER(_P), _P, _INT]),
     "gpl_gen_uniform_points": (_INT, [_P, C.c_uint64, _I64, _I64, _D, _P]),
     "gpl_gen_walk_linestrings": (_INT, [_P, C.c_uint64, _I64, _I64, _I64, C.c_int32, _P, _P]),
     "gpl_gen_blob_polygons": (_INT, [_P, C.c_uint64, _I64, _I64, C.c_int32, _P, _P, _P]),

@@ -13,22 +13,13 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "haversine.cuh"
 
 namespace gpl {
 
-constexpr double kMeanEarthRadius = 6371008.8;  // geo MEAN_EARTH_RADIUS
 constexpr double kWgs84A = 6378137.0;
 constexpr double kWgs84B = 6356752.314245;  // geo POLAR_EARTH_RADIUS (Vincenty)
-constexpr double DEG = 0.017453292519943295769;
 constexpr double kPi = 3.14159265358979323846;
-__device__ __forceinline__ double haversine_distance(double2 p, double2 q) {
-    double theta1 = p.y * DEG, theta2 = q.y * DEG;
-    double delta_theta = (q.y - p.y) * DEG, delta_lambda = (q.x - p.x) * DEG;
-    double s1 = sin(delta_theta / 2.0), s2 = sin(delta_lambda / 2.0);
-    double a = s1 * s1 + cos(theta1) * cos(theta2) * (s2 * s2);
-    double c = 2.0 * asin(sqrt(a));
-    return kMeanEarthRadius * c;
-}
 /* Ok(distance) -> 1, Err(FailedToConvergeError) -> 0 */
 __device__ __noinline__ int vincenty_distance(double2 p, double2 q, double *out) {
     const double a = kWgs84A, b = kWgs84B, f = (kWgs84A - kWgs84B) / kWgs84A;

@@ -411,6 +411,17 @@ def distance(a: DeviceArray, b: DeviceArray) -> Tuple[np.ndarray, np.ndarray]:
     return out, _bits(bm, n)
 
 
+def haversine_distance(a: DeviceArray, b: DeviceArray) -> Tuple[np.ndarray, np.ndarray]:
+    """row-wise great-circle distance in metres of two Point columns in (lon, lat) degrees: geo's HaversineDistance on the
+    mean sphere, the value `geodesic_length(method="haversine")` sums over segments; (values, valid) — a null or empty
+    point gives an invalid row"""
+    n = len(a)
+    out = np.empty(n, dtype=np.float64)
+    bm = np.zeros((n + 7) // 8, dtype=np.uint8)
+    check(a.ctx.lib.gpl_haversine_distance(a.ctx._h, a._h, b._h, _np_ptr(out), _np_ptr(bm), GPL_HOST))
+    return out, _bits(bm, n)
+
+
 def intersects(a: DeviceArray, b: DeviceArray) -> np.ndarray:
     n = len(a)
     bm = np.zeros((n + 7) // 8, dtype=np.uint8)
@@ -718,6 +729,86 @@ class NearestIndex:
     def free(self) -> None:
         if getattr(self, "_h", None) and self.ctx._h:
             self.ctx.lib.gpl_nearest_index_free(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def _pairs_with_distance(ctx: Context, h, with_distance: bool):
+    """(lhs uint64, rhs uint64, d float64 or None) of a sorted pair list; frees it"""
+    try:
+        n = int(ctx.lib.gpl_pairs_count(h))
+        a = np.empty(n, dtype=np.uint64)
+        b = np.empty(n, dtype=np.uint64)
+        d = np.empty(n, dtype=np.float64) if with_distance else None
+        if n:
+            check(ctx.lib.gpl_pairs_copy(ctx._h, h, _np_ptr(a), _np_ptr(b), GPL_HOST))
+            if with_distance:
+                check(ctx.lib.gpl_pairs_copy_distance(ctx._h, h, _np_ptr(d), GPL_HOST))
+    finally:
+        ctx.lib.gpl_pairs_free(h)
+    return a, b, d
+
+
+class GeoIndex:
+    """Right side of the great-circle joins (DESIGN.md §4.15): a grid over the Point rows of a (lon, lat) degree column.  The
+    distance of a (left row, right row) pair is exactly what `haversine_distance` returns for it, in metres.  Rows that are
+    null, empty, non-finite or outside |lat| <= 90, |lon| <= 360 match nothing, on either side."""
+
+    STATS = ("rows", "ineligible", "grid_cells_per_axis", "grid_columns", "grid_rows", "cell_items", "bytes", "evaluations")
+
+    def __init__(self, rhs: DeviceArray):
+        self.ctx = rhs.ctx
+        h = C.c_void_p()
+        check(self.ctx.lib.gpl_geo_index_build(self.ctx._h, rhs._h, C.byref(h)))
+        self._h = h
+
+    def stats(self) -> dict:
+        """eligible and ineligible rows, grid shape and size; exact evaluations of the last query pass"""
+        out = np.zeros(8, dtype=np.int64)
+        check(self.ctx.lib.gpl_geo_index_stats(self.ctx._h, self._h, _np_ptr(out)))
+        return dict(zip(self.STATS, (int(v) for v in out)))
+
+    def count_within(self, lhs: DeviceArray, distance: float) -> np.ndarray:
+        """number of right rows within `distance` metres (inclusive, finite, >= 0) of each left point: int32 per left row"""
+        out = np.empty(len(lhs), dtype=np.int32)
+        check(self.ctx.lib.gpl_geo_dwithin_count(self.ctx._h, self._h, lhs._h, float(distance), _np_ptr(out), GPL_HOST))
+        return out
+
+    def pairs_within(self, lhs: DeviceArray, distance: float, with_distance: bool = False):
+        """every (left row, right row) pair within `distance` metres, once, sorted by (lhs, rhs): (lhs uint64, rhs uint64[, d])"""
+        h = C.c_void_p()
+        check(self.ctx.lib.gpl_geo_dwithin_join_pairs(self.ctx._h, self._h, lhs._h, float(distance), int(bool(with_distance)), C.byref(h)))
+        a, b, d = _pairs_with_distance(self.ctx, h, with_distance)
+        return (a, b, d) if with_distance else (a, b)
+
+    def query(self, lhs: DeviceArray, max_distance=None):
+        """(nearest_id int32 (-1: none), distance float64 metres (NaN: none), n_tied int32) for a Point column in HBM;
+        max_distance is inclusive (None: unbounded)"""
+        n = len(lhs)
+        nid = np.empty(n, dtype=np.int32)
+        dist = np.empty(n, dtype=np.float64)
+        tied = np.empty(n, dtype=np.int32)
+        check(self.ctx.lib.gpl_geo_nearest_join(self.ctx._h, self._h, lhs._h, NearestIndex._maxd(max_distance), _np_ptr(nid), _np_ptr(dist),
+                                                _np_ptr(tied), GPL_HOST))
+        return nid, dist, tied
+
+    def pairs(self, lhs: DeviceArray, max_distance=None, with_distance: bool = False):
+        """every tied (left row, right row) pair once, sorted by (lhs, rhs) [+ the dense distance of every left row, NaN: no match]"""
+        h = C.c_void_p()
+        dist = np.empty(len(lhs), dtype=np.float64) if with_distance else None
+        check(self.ctx.lib.gpl_geo_nearest_join_pairs(self.ctx._h, self._h, lhs._h, NearestIndex._maxd(max_distance), C.byref(h), _np_ptr(dist),
+                                                      GPL_HOST))
+        a, b, _ = _pairs_with_distance(self.ctx, h, False)
+        return (a, b, dist) if with_distance else (a, b)
+
+    def free(self) -> None:
+        if getattr(self, "_h", None) and self.ctx._h:
+            self.ctx.lib.gpl_geo_index_free(self._h)
         self._h = None
 
     def __del__(self):

@@ -265,6 +265,12 @@ class GeoRustSeries:
         out, valid = E.distance(self._d(), other.device)
         return _pa().array(valid.astype(bool) & (out <= float(distance)))
 
+    def haversine_distance(self, other: GeoSeries):
+        """row-wise great-circle distance in metres to `other`, both Point columns in (lon, lat) degrees (geo's
+        HaversineDistance, mean earth radius 6 371 008.8 m); a null or empty point gives null"""
+        out, valid = E.haversine_distance(self._d(), other.device)
+        return _f64(out, valid)
+
     def translate(self, xoff: float = 0.0, yoff: float = 0.0) -> GeoSeries:
         return self._wrap(E.translate(self._d(), xoff, yoff))
 
@@ -374,4 +380,59 @@ def dwithin_join(lhs: GeoSeries, rhs: GeoSeries, distance: float, how: str = "in
         d = np.concatenate([d, np.full(len(miss), np.nan)])
         order = np.lexsort((b, a))
         a, b, d = a[order], b[order], d[order]
+    return a, b, d
+
+
+def _left_rows(a, b, d, unmatched):
+    """how='left': the unmatched left rows once, with rhs_index -1 and distance NaN, merged in (lhs, rhs) order"""
+    a = np.concatenate([a, unmatched])
+    b = np.concatenate([b, np.full(len(unmatched), -1, dtype=np.int64)])
+    d = np.concatenate([d, np.full(len(unmatched), np.nan)])
+    order = np.lexsort((b, a))
+    return a[order], b[order], d[order]
+
+
+def geo_nearest_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", max_distance: Optional[float] = None):
+    """`nearest_join` for two Point columns in (lon, lat) degrees, by great-circle distance in metres: (lhs_index int64,
+    rhs_index int64, distance float64), sorted by (lhs, rhs).  The distance is exactly what `lhs.geo.haversine_distance`
+    computes for the pair, so the join is right across the antimeridian and at the poles, where degrees are not distances.
+    Every right row at the minimum distance is returned (ties are equal f64 values); max_distance is in metres and inclusive
+    (None: unbounded).  Rows that are null, empty, non-finite or outside |lat| <= 90, |lon| <= 360 match nothing, on either
+    side.  how='inner' -> matched left rows only; how='left' -> unmatched left rows once, with rhs_index -1 and distance NaN
+    (DESIGN.md §4.15)."""
+    if how not in ("inner", "left"):
+        raise ValueError("how must be 'inner' or 'left'")
+    idx = E.GeoIndex(rhs.device)
+    try:
+        a, b, dist = idx.pairs(lhs.device, max_distance, with_distance=True)
+    finally:
+        idx.free()
+    a = a.astype(np.int64)
+    b = b.astype(np.int64)
+    d = dist[a]
+    if how == "left":
+        a, b, d = _left_rows(a, b, d, np.nonzero(np.isnan(dist))[0])
+    return a, b, d
+
+
+def geo_dwithin_join(lhs: GeoSeries, rhs: GeoSeries, distance: float, how: str = "inner"):
+    """`dwithin_join` for two Point columns in (lon, lat) degrees, by great-circle distance: (lhs_index int64, rhs_index
+    int64, distance float64) for every right row within `distance` metres (inclusive; finite and >= 0) of the left row,
+    sorted by (lhs, rhs).  The distance is exactly what `lhs.geo.haversine_distance` computes for the pair; a NaN distance
+    never matches.  Rows that are null, empty, non-finite or outside |lat| <= 90, |lon| <= 360 match nothing, on either side.
+    how='inner' -> matched left rows only; how='left' -> unmatched left rows once, with rhs_index -1 and distance NaN
+    (DESIGN.md §4.15)."""
+    if how not in ("inner", "left"):
+        raise ValueError("how must be 'inner' or 'left'")
+    idx = E.GeoIndex(rhs.device)
+    try:
+        a, b, d = idx.pairs_within(lhs.device, distance, with_distance=True)
+    finally:
+        idx.free()
+    a = a.astype(np.int64)
+    b = b.astype(np.int64)
+    if how == "left":
+        matched = np.zeros(len(lhs), dtype=bool)
+        matched[a] = True
+        a, b, d = _left_rows(a, b, d, np.nonzero(~matched)[0])
     return a, b, d

@@ -71,6 +71,7 @@ typedef struct gpl_ctx gpl_ctx;             /* one per (host thread, device) */
 typedef struct gpl_array gpl_array;         /* GeoArrow geometry array resident in HBM */
 typedef struct gpl_pip_index gpl_pip_index;
 typedef struct gpl_nearest_index gpl_nearest_index; /* right side of a nearest join */
+typedef struct gpl_geo_index gpl_geo_index; /* right side of a great-circle join */
 typedef struct gpl_pairs gpl_pairs;         /* (lhs_index, rhs_index) pair list of a join, resident on the device */ /* polygon-side index of a contains join */
 
 /* Raw GeoArrow buffers (the zero-dependency form of an Arrow array; replaces the WKB BinaryArray the
@@ -361,6 +362,44 @@ int gpl_dwithin_join_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl
                            gpl_pairs **out);
 /* the distance of each pair of a list built with distances (any other list: GPL_ERR_INVALID_ARG); distance[n] in `mem` */
 int gpl_pairs_copy_distance(gpl_ctx *ctx, const gpl_pairs *pairs, double *distance, int mem);
+
+/* ---------------------------------------------------------------- great-circle joins ----- */
+/* Great-circle distance in metres of two POINT columns read as (lon, lat) degrees: geo 0.27 HaversineDistance on the mean
+ * sphere (6 371 008.8 m), the expression gpl_geodesic_length(method 1) sums over segments, bit for bit.  Row-wise 1:1;
+ * out[n] f64, out_validity bitmap (may be NULL).  A null or empty point gives a null row (NaN, validity 0); a non-finite
+ * coordinate gives what the expression gives (NaN).  `a` is not clamped: within about 1e-8 rad of the antipode rounding can
+ * push it above 1 and the result is NaN, as in geo.  Any other geometry type: GPL_ERR_INVALID_TYPE; unequal lengths:
+ * GPL_ERR_LENGTH_MISMATCH. */
+int gpl_haversine_distance(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, double *out, uint8_t *out_validity, int mem);
+/* Joins of two POINT columns in (lon, lat) degrees by that distance (DESIGN.md 4.15).  d(i, j) is exactly the f64 that
+ * gpl_haversine_distance returns for (lhs[i], rhs[j]).  A row of either side takes part only if it is non-null, non-empty,
+ * finite and has |lat| <= 90 and |lon| <= 360 (so both the -180..180 and the 0..360 convention are accepted, and may be
+ * mixed); no other row matches anything.  A NaN distance never matches.  Fewer than 2^31 rows on the right, and on the left
+ * per call (else GPL_ERR_UNSUPPORTED); a non-POINT column: GPL_ERR_INVALID_TYPE; both checked before any launch.  Outputs
+ * are deterministic (two calls give byte-identical results).  The index copies what it needs: `rhs` need not outlive it. */
+int gpl_geo_index_build(gpl_ctx *ctx, const gpl_array *rhs, gpl_geo_index **out);
+void gpl_geo_index_free(gpl_geo_index *idx);
+/* synchronises the context stream: out8[0] = eligible right rows, [1] = ineligible rows, [2] = grid cells per axis,
+ * [3] = columns and [4] = rows of cells in use (1 when the rows share one meridian / parallel), [5] = cell items, [6] = index
+ * bytes, [7] = exact distance evaluations of the last query pass (a pair-list call runs two passes and leaves the count of
+ * its second; concurrent queries of one index overwrite each other's count, never their results). */
+int gpl_geo_index_stats(gpl_ctx *ctx, const gpl_geo_index *idx, int64_t *out8);
+/* count[i] (int32, in `mem`) = number of right rows with d(i, j) <= distance (inclusive).  distance in metres, finite and
+ * >= 0 (NaN, negative or +-inf -> GPL_ERR_INVALID_ARG before any launch) */
+int gpl_geo_dwithin_count(gpl_ctx *ctx, const gpl_geo_index *idx, const gpl_array *lhs, double distance, int32_t *count, int mem);
+/* every such pair once, sorted by (lhs, rhs), as a device-resident gpl_pairs; with_distance != 0 also keeps d(i, j) of each
+ * pair (gpl_pairs_copy_distance) */
+int gpl_geo_dwithin_join_pairs(gpl_ctx *ctx, const gpl_geo_index *idx, const gpl_array *lhs, double distance, int with_distance,
+                               gpl_pairs **out);
+/* the right rows at the minimum d(i, j) <= max_distance (metres, inclusive; +inf = unbounded; NaN or negative ->
+ * GPL_ERR_INVALID_ARG); rows tie when their distances are equal f64 values.  nearest_id[i] = lowest tied row or -1,
+ * distance[i] (may be NULL) = its distance or NaN, n_tied[i] (may be NULL) = number of tied rows; all in `mem`. */
+int gpl_geo_nearest_join(gpl_ctx *ctx, const gpl_geo_index *idx, const gpl_array *lhs, double max_distance, int32_t *nearest_id,
+                         double *distance, int32_t *n_tied, int mem);
+/* every tied (left row, right row) pair once, sorted by (lhs, rhs); distance (may be NULL, in `mem`) receives the dense
+ * distance of every left row (NaN: no match) */
+int gpl_geo_nearest_join_pairs(gpl_ctx *ctx, const gpl_geo_index *idx, const gpl_array *lhs, double max_distance, gpl_pairs **out,
+                               double *distance, int mem);
 
 /* ---------------------------------------------------------------- synthetic data --------- */
 /* device-side generators, bit-identical to geopolars_b200/synth.py (SURVEY.md §8d RNG) */

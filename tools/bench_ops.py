@@ -4,7 +4,7 @@ fraction for the coordinate bytes read, and of the nearest join (100 M points ag
 reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
@@ -41,9 +41,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin"), default="all",
-                    help="run only the §8 rows, only the point nearest join, only the geometry nearest join or only the "
-                         "distance-within join")
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo"), default="all",
+                    help="run only the §8 rows, only the point nearest join, only the geometry nearest join, only the "
+                         "distance-within join or only the great-circle joins")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
@@ -77,7 +77,9 @@ def main():
             nearest_geom_rows(args, ctx, dev, st, res)
         if args.only in ("all", "dwithin"):
             dwithin_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom", "dwithin"):
+        if args.only in ("all", "geo"):
+            geo_rows(args, ctx, dev, st, res)
+        if args.only in ("nearest", "nearest_geom", "dwithin", "geo"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -400,6 +402,93 @@ def dwithin_rows(args, ctx, dev, st, res):
     print(json.dumps(r), flush=True)
     del lp, rp, pxy, pro, pgo, moff
     torch.cuda.empty_cache()
+
+
+def geo_rows(args, ctx, dev, st, res):
+    """great-circle joins (DESIGN.md §4.15), kernel resident: build ms, count-pass ms, pair-list ms (with distances), dense
+    nearest ms; left rows/s, pairs/s, exact haversine evaluations per left row and per second.  An evaluation is 2 sin, 1
+    sqrt, 1 asin and about 15 FP64 operations on one 32-byte record: the kernels are FP64 / transcendental bound, not HBM
+    bound (evaluations/s x 32 B is far below the HBM peak).  Plus a cKDTree CPU arm on unit vectors for workload 1."""
+    import time
+
+    import numpy as np
+
+    lib = ctx.lib
+    D = 1e4
+
+    def upload(P):
+        t = torch.from_numpy(np.ascontiguousarray(P)).to(dev)
+        return ctx.wrap_device(GeometryType.POINT, len(P), len(P), t.data_ptr(), keepalive=(t,))
+
+    def run(name, L, Rr):
+        lhs, rhs, n = upload(L), upload(Rr), len(L)
+        tb = timed(st, lambda: E.GeoIndex(rhs).free(), reps=3, warm=1)
+        idx = E.GeoIndex(rhs)
+        cnt = torch.empty(n, dtype=torch.int32, device=dev)
+        tc = timed(st, lambda: E.check(lib.gpl_geo_dwithin_count(ctx._h, idx._h, lhs._h, D, C.c_void_p(cnt.data_ptr()), E.GPL_DEVICE)), reps=3, warm=1)
+        evals = idx.stats()["evaluations"]
+        n_pairs = [0]
+
+        def pairs():
+            h = C.c_void_p()
+            E.check(lib.gpl_geo_dwithin_join_pairs(ctx._h, idx._h, lhs._h, D, 1, C.byref(h)))
+            n_pairs[0] = int(lib.gpl_pairs_count(h))
+            lib.gpl_pairs_free(h)
+
+        tp = timed(st, pairs, reps=3, warm=1)
+        nid = torch.empty(n, dtype=torch.int32, device=dev)
+        dist = torch.empty(n, dtype=torch.float64, device=dev)
+        tn = timed(st, lambda: E.check(lib.gpl_geo_nearest_join(ctx._h, idx._h, lhs._h, float("inf"), C.c_void_p(nid.data_ptr()),
+                                                                C.c_void_p(dist.data_ptr()), None, E.GPL_DEVICE)), reps=3, warm=1)
+        s = idx.stats()
+        r = {"op": f"great-circle joins: {name}, D = {D} m", "left_rows": n, "rhs_rows": len(Rr), "build_ms_min": tb[0],
+             "count_ms_min": tc[0], "count_ms_avg": tc[1], "pairs_ms_min": tp[0], "pairs_ms_avg": tp[1], "nearest_ms_min": tn[0],
+             "nearest_ms_avg": tn[1], "count_left_rows_per_s": n / (tc[1] * 1e-3), "pairs_left_rows_per_s": n / (tp[1] * 1e-3),
+             "pairs_per_s": n_pairs[0] / (tp[1] * 1e-3), "nearest_left_rows_per_s": n / (tn[1] * 1e-3), "pairs": n_pairs[0],
+             "count_evals_per_left_row": evals / n, "count_evals_per_s": evals / (tc[1] * 1e-3),
+             "count_item_GBps": evals * 32 / (tc[1] * 1e-3) / 1e9, "nearest_evals_per_left_row": s["evaluations"] / n,
+             "nearest_evals_per_s": s["evaluations"] / (tn[1] * 1e-3), "grid_cells_per_axis": s["grid_cells_per_axis"],
+             "card": res["card"], "power_limit": res["power_limit"]}
+        idx.free()
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    def sphere(rng, n):
+        return np.column_stack([rng.uniform(-180, 180, n), np.degrees(np.arcsin(rng.uniform(-1, 1, n)))])
+
+    NP, NR = int(10_000_000 * max(args.scale, 0.01)), int(1_000_000 * max(args.scale, 0.01))
+    rng = np.random.default_rng(415)
+    L, Rr = sphere(rng, NP), sphere(rng, NR)
+    run(f"{NP} x {NR} points uniform on the sphere", L, Rr)
+    # real data is skewed: both sides scattered about 100 km (1 degree sigma in latitude) around the naturalearth_cities rows
+    from geopolars_b200 import datasets
+
+    c = datasets.read_dataset("naturalearth_cities").geometry.device.to_host().xy
+
+    def around(n):
+        k = c[rng.integers(0, len(c), n)]
+        lat = np.clip(k[:, 1] + rng.normal(0, 0.9, n), -89.9, 89.9)
+        return np.column_stack([k[:, 0] + rng.normal(0, 0.9, n) / np.cos(np.radians(lat)), lat])
+
+    run(f"{NP} x {NR} points clustered around {len(c)} cities", around(NP), around(NR))
+    # CPU arm of workload 1: cKDTree on 3-D unit vectors, chord radius 2 sin(D / 2R), a prefix of the left points
+    from scipy.spatial import cKDTree
+
+    def unit(P):
+        lo, la = np.radians(P[:, 0]), np.radians(P[:, 1])
+        return np.column_stack([np.cos(la) * np.cos(lo), np.cos(la) * np.sin(lo), np.sin(la)])
+
+    k = min(NP, 2_000_000)
+    t0 = time.perf_counter()
+    tree = cKDTree(unit(Rr))
+    t1 = time.perf_counter()
+    nb = tree.query_ball_point(unit(L[:k]), 2.0 * np.sin(D / 6371008.8 / 2.0), workers=-1, return_length=True)
+    t2 = time.perf_counter()
+    r = {"op": f"great-circle dwithin CPU arm: scipy cKDTree.query_ball_point(workers=-1, return_length=True) on unit vectors, {k}-point "
+               "prefix of workload 1 (candidate counts by chord: no haversine evaluation)",
+         "left_rows": k, "nproc": os.cpu_count(), "build_s": t1 - t0, "query_s": t2 - t1, "left_rows_per_s": k / (t2 - t1), "pairs": int(nb.sum())}
+    res["rows"].append(r)
+    print(json.dumps(r), flush=True)
 
 
 if __name__ == "__main__":
