@@ -110,6 +110,8 @@ extern "C" {
     fn gpl_geo_nearest_join(ctx: *mut GplCtx, idx: *const GplGeoIndex, lhs: *const GplArray, max_distance: f64, nearest_id: *mut i32, distance: *mut f64, n_tied: *mut i32, mem: c_int) -> c_int;
     fn gpl_geo_dwithin_join_pairs(ctx: *mut GplCtx, idx: *const GplGeoIndex, lhs: *const GplArray, distance: f64, with_distance: c_int, out: *mut *mut GplPairs) -> c_int;
     fn gpl_geo_nearest_join_pairs(ctx: *mut GplCtx, idx: *const GplGeoIndex, lhs: *const GplArray, max_distance: f64, out: *mut *mut GplPairs, distance: *mut f64, mem: c_int) -> c_int;
+    fn gpl_intersection_area(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, out: *mut f64, out_validity: *mut u8, mem: c_int) -> c_int;
+    fn gpl_overlay_area_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, out: *mut *mut GplPairs) -> c_int;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -423,6 +425,14 @@ pub trait GeoSeriesB200Ext {
     fn geo_nearest_join_pairs(&self, rhs: &Series, max_distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
     /// `dwithin_join_pairs` for two Point columns in (lon, lat) degrees with `haversine_distance` as the distance (metres)
     fn geo_dwithin_join_pairs(&self, rhs: &Series, distance: f64) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
+    /// row-wise area of the intersection of two (Multi)Polygon columns (`BooleanOps::intersection(..).unsigned_area()`
+    /// without building the polygons); null or non-finite rows give null, empty rows 0.  Valid (OGC) operands only: on
+    /// invalid input the value is finite but not specified
+    fn intersection_area(&self, other: &Series) -> Result<Series>;
+    /// area-weighted overlay join of two (Multi)Polygon columns: every pair whose closed geometries intersect (touching pairs
+    /// included, with area 0), as (lhs_index, rhs_index, area) in an unspecified order; the area is bit for bit what
+    /// `intersection_area` computes for the pair
+    fn overlay_area_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
 }
 
 impl GeoSeriesB200Ext for Series {
@@ -553,6 +563,34 @@ impl GeoSeriesB200Ext for Series {
             unsafe { gpl_pairs_free(pairs) };
         }
         check(rc)?;
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r, mut d) = (vec![0u64; n], vec![0u64; n], vec![0f64; n]);
+        let mut rc = 0;
+        if n > 0 {
+            rc = unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) };
+            if rc == 0 {
+                rc = unsafe { gpl_pairs_copy_distance(ctx, pairs, d.as_mut_ptr(), GPL_HOST) };
+            }
+        }
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
+        Ok((l, r, d))
+    }
+
+    fn intersection_area(&self, other: &Series) -> Result<Series> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, other)?);
+        let mut v = vec![0f64; self.len()];
+        let mut valid = vec![0u8; (self.len() + 7) / 8];
+        check(unsafe { gpl_intersection_area(ctx, a.0, b.0, v.as_mut_ptr(), valid.as_mut_ptr(), GPL_HOST) })?;
+        Ok(f64_series("intersection_area", v, valid))
+    }
+
+    fn overlay_area_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let mut pairs = std::ptr::null_mut();
+        check(unsafe { gpl_overlay_area_join(ctx, a.0, b.0, &mut pairs) })?;
         let n = unsafe { gpl_pairs_count(pairs) } as usize;
         let (mut l, mut r, mut d) = (vec![0u64; n], vec![0u64; n], vec![0f64; n]);
         let mut rc = 0;

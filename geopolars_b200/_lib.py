@@ -167,6 +167,8 @@ SIGNATURES = {
     "gpl_dwithin_count": (_INT, [_P, _P, _P, _D, _P, _INT]),
     "gpl_dwithin_join_pairs": (_INT, [_P, _P, _P, _D, _INT, C.POINTER(_P)]),
     "gpl_pairs_copy_distance": (_INT, [_P, _P, _P, _INT]),
+    "gpl_intersection_area": (_INT, [_P, _P, _P, _P, _P, _INT]),
+    "gpl_overlay_area_join": (_INT, [_P, _P, _P, C.POINTER(_P)]),
     "gpl_haversine_distance": (_INT, [_P, _P, _P, _P, _P, _INT]),
     "gpl_geo_index_build": (_INT, [_P, _P, C.POINTER(_P)]),
     "gpl_geo_index_free": (None, [_P]),

@@ -146,12 +146,13 @@ struct gpl_array {
     int refcount = 1;
 };
 
-// result of a join (gpl_spatial_join, gpl_contains_join_pairs_array, gpl_nearest_join_pairs_array, gpl_dwithin_join_pairs):
+// result of a join (gpl_spatial_join, gpl_contains_join_pairs_array, gpl_nearest_join_pairs_array, gpl_dwithin_join_pairs,
+// gpl_overlay_area_join):
 // (lhs, rhs) row pairs
 struct gpl_pairs {
     gpl_ctx *ctx = nullptr;
     uint64_t *lhs = nullptr, *rhs = nullptr;  // device
-    double *dist = nullptr;                   // device, the distance of each pair (gpl_dwithin_join_pairs with_distance only)
+    double *dist = nullptr;                   // device, the distance of each pair (with_distance joins) or its area (gpl_overlay_area_join)
     bool with_dist = false;                   // dist was asked for (it stays NULL when the list is empty)
     int64_t n = 0;
 };
@@ -408,6 +409,8 @@ __device__ __forceinline__ int orient_sign(double2 a, double2 b, double2 c) {
     double d = orient2d(a.x, a.y, b.x, b.y, c.x, c.y);
     return (d > 0.0) - (d < 0.0);
 }
+__device__ __forceinline__ int cmpd(double a, double b) { return (a > b) - (a < b); }
+__device__ __forceinline__ int sgnd(double a) { return (a > 0.0) - (a < 0.0); }
 __device__ __forceinline__ bool value_in_between(double v, double b1, double b2) {
     return (b1 < b2) ? (v >= b1 && v <= b2) : (v >= b2 && v <= b1);
 }

@@ -240,8 +240,7 @@ struct SymQ {
     double xx, xy, vx, vy;
     int side;
 };
-__device__ __forceinline__ int cmpd(double a, double b) { return (a > b) - (a < b); }
-__device__ __forceinline__ int sgnd(double a) { return (a > 0.0) - (a < 0.0); }
+// cmpd, sgnd: common.cuh
 __device__ __forceinline__ int sym_cmp_y(const SymQ &q, double cy) {  // sign of cy - q.y
     int c = cmpd(cy, q.xy);
     if (c) return c;
@@ -599,20 +598,9 @@ __global__ void k_point_point_dist(int64_t n, const double2 *__restrict__ a, con
     if (out_valid) out_valid[i] = valid ? 1 : 0;
 }
 
-int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n);
-int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
-
 static int side_class_host(int t) { return (t == GPL_POINT || t == GPL_MULTIPOINT) ? 0 : (t == GPL_LINESTRING || t == GPL_MULTILINESTRING) ? 1 : 2; }
 
-// bool result: bytes on device -> Arrow bitmap in the caller's memory
-static int finish_bitmap(gpl_ctx *ctx, const uint8_t *bytes_dev, int64_t n, uint8_t *out_bitmap, int mem) {
-    size_t nb = (size_t)(n + 7) / 8;
-    if (mem == GPL_DEVICE) return pack_bits(ctx, bytes_dev, out_bitmap, n);
-    Scratch<uint8_t> bm;
-    GPL_TRY(bm.get(ctx, nb));
-    GPL_TRY(pack_bits(ctx, bytes_dev, bm.p, n));
-    return deliver(ctx, out_bitmap, bm.p, nb, GPL_HOST);
-}
+// finish_bitmap, polygon_view: pair_dist.cuh
 
 }  // namespace gpl
 
@@ -789,10 +777,75 @@ __global__ void k_join_compact(const uint8_t *__restrict__ hit, const int64_t *_
     if (k < n && hit[k]) ol[off[k]] = cl[k], orr[off[k]] = cr[k];
 }
 
-static Side polygon_view(const gpl_array *g) {
-    const double2 *xy = reinterpret_cast<const double2 *>(g->xy);
-    if (g->type == GPL_MULTIPOLYGON) return Side{GPL_POLYGON, xy, g->part_off, nullptr, g->ring_off};
-    return Side{g->type, xy, g->geom_off, g->part_off, g->ring_off};
+// The candidate stage of the general join: envelopes of both sides, the grid over the right side's union box, the
+// candidate list (count -> scan -> write), the exact test `test` per candidate and the compaction of the hits into res
+// (lhs / rhs, in candidate order).  res stays empty when nothing matches.
+int join_candidate_pairs(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, JoinTest test, const char *who, gpl_pairs *res) {
+    const int64_t nl = lhs->n_geoms, nr = rhs->n_geoms;
+    const int tl = lhs->type, tr = rhs->type;
+    // ---- envelopes -----------------------------------------------------------------------------------------------------
+    Scratch<double> l4, r4;
+    Scratch<uint8_t> lh, rh;
+    GPL_TRY(l4.get(ctx, (size_t)nl * 4));
+    GPL_TRY(r4.get(ctx, (size_t)nr * 4));
+    GPL_TRY(lh.get(ctx, (size_t)nl));
+    GPL_TRY(rh.get(ctx, (size_t)nr));
+    GPL_TRY(envelope_raw(ctx, lhs, l4.p, lh.p));
+    GPL_TRY(envelope_raw(ctx, rhs, r4.p, rh.p));
+    // ---- grid over the right side's union box ------------------------------------------------------------------------------
+    GridBuild grid;
+    GPL_TRY(join_grid_build(ctx, r4.p, rh.p, nr, nr, who, grid));
+    if (grid.jg.g == 0) return GPL_OK;  // no right row has an envelope
+    // ---- candidates: count -> scan -> write ----------------------------------------------------------------------------------
+    Scratch<int32_t> cand_count;
+    Scratch<int64_t> tot, cand_off;
+    GPL_TRY(tot.get(ctx, 1));
+    GPL_TRY(cand_count.get(ctx, (size_t)nl + 1));
+    GPL_TRY(cand_off.get(ctx, (size_t)nl + 2));
+    GPL_LAUNCH(ctx, k_join_candidates<0>, (int)ceil_div(nl, 128), 128, 0, l4.p, lh.p, nl, r4.p, grid.jg, grid.ux1, grid.uy1, grid.cell_start.p,
+               grid.items.p, cand_count.p, nullptr, nullptr, nullptr);
+    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cand_count.p, nl, cand_off.p, tot.p)));
+    int64_t n_cand = 0;
+    GPL_CUDA(cudaMemcpyAsync(&n_cand, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (n_cand == 0) return GPL_OK;
+    Scratch<uint64_t> cl, cr;
+    GPL_TRY(cl.get(ctx, (size_t)n_cand));
+    GPL_TRY(cr.get(ctx, (size_t)n_cand));
+    GPL_LAUNCH(ctx, k_join_candidates<1>, (int)ceil_div(nl, 128), 128, 0, l4.p, lh.p, nl, r4.p, grid.jg, grid.ux1, grid.uy1, grid.cell_start.p,
+               grid.items.p, nullptr, cand_off.p, cl.p, cr.p);
+    // ---- exact predicate per candidate ------------------------------------------------------------------------------------------
+    Scratch<uint8_t> hit;
+    GPL_TRY(hit.get(ctx, (size_t)n_cand));
+    const double2 *lxy = reinterpret_cast<const double2 *>(lhs->xy), *rxy = reinterpret_cast<const double2 *>(rhs->xy);
+    const Side sl{tl, lxy, lhs->geom_off, lhs->part_off, lhs->ring_off}, sr{tr, rxy, rhs->geom_off, rhs->part_off, rhs->ring_off};
+    const int pgrid = warp_grid(n_cand, 8);
+    switch (test) {
+    case JOIN_POINT_IN_R: GPL_LAUNCH(ctx, k_contains_point_pairs, pgrid, 256, 0, n_cand, sr, rhs->validity, lxy, lhs->validity, cr.p, cl.p, hit.p); break;
+    case JOIN_POINT_IN_L: GPL_LAUNCH(ctx, k_contains_point_pairs, pgrid, 256, 0, n_cand, sl, lhs->validity, rxy, rhs->validity, cl.p, cr.p, hit.p); break;
+    case JOIN_POLY_CONTAINS:
+        GPL_LAUNCH(ctx, k_contains_polygon, pgrid, 256, 0, n_cand, polygon_view(lhs), tl == GPL_MULTIPOLYGON ? lhs->geom_off : nullptr, lhs->validity,
+                   polygon_view(rhs), rhs->validity, cl.p, cr.p, hit.p);
+        break;
+    default: GPL_LAUNCH(ctx, k_intersects_pairs, pgrid, 256, 0, n_cand, sl, lhs->validity, sr, rhs->validity, cl.p, cr.p, hit.p); break;
+    }
+    // ---- compaction ----------------------------------------------------------------------------------------------------------------
+    Scratch<int64_t> hit_off;
+    GPL_TRY(hit_off.get(ctx, (size_t)n_cand + 2));
+    GPL_TRY((exclusive_scan<uint8_t, int64_t>(ctx, hit.p, n_cand, hit_off.p, tot.p)));
+    int64_t n_hit = 0;
+    GPL_CUDA(cudaMemcpyAsync(&n_hit, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (n_hit == 0) return GPL_OK;
+    void *pl = nullptr, *pr = nullptr;
+    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)n_hit, &pl));
+    res->lhs = (uint64_t *)pl;
+    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)n_hit, &pr));
+    res->rhs = (uint64_t *)pr;
+    res->n = n_hit;
+    GPL_LAUNCH(ctx, k_join_compact, (int)ceil_div(n_cand, 256), 256, 0, hit.p, hit_off.p, n_cand, cl.p, cr.p, res->lhs, res->rhs);
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch lists above return to the cache when this scope ends
+    return GPL_OK;
 }
 
 }  // namespace gpl
@@ -857,73 +910,11 @@ extern "C" int gpl_spatial_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_ar
     // ---- the type-pair dispatch table of spatial_index.rs:89-137 (anything else: no pair matches) ------------------------
     const int tl = lhs->type, tr = rhs->type;
     const int cl_ = side_class_host(tl), cr_ = side_class_host(tr);
-    enum { NONE, POINT_IN_R, POINT_IN_L, POLY_CONTAINS, INTERSECTS } mode = NONE;
-    if (tl == GPL_POINT && (cr_ == 2 || tr == GPL_LINESTRING || tr == GPL_MULTILINESTRING)) mode = POINT_IN_R;       // :91, :95, :130-134
-    else if (tr == GPL_POINT && (cl_ == 2 || tl == GPL_LINESTRING || tl == GPL_MULTILINESTRING)) mode = POINT_IN_L;  // :92, :96, :129-133
-    else if ((tl == GPL_POLYGON || tl == GPL_MULTIPOLYGON) && tr == GPL_POLYGON) mode = predicate == GPL_PREDICATE_CONTAINS ? POLY_CONTAINS : INTERSECTS;  // :99-115
-    else if (tl == GPL_POLYGON && tr == GPL_MULTIPOLYGON && predicate == GPL_PREDICATE_INTERSECTS) mode = INTERSECTS;  // :118-122
-    if (mode == NONE) return GPL_OK;
-    // ---- envelopes -----------------------------------------------------------------------------------------------------
-    Scratch<double> l4, r4;
-    Scratch<uint8_t> lh, rh;
-    GPL_TRY(l4.get(ctx, (size_t)nl * 4));
-    GPL_TRY(r4.get(ctx, (size_t)nr * 4));
-    GPL_TRY(lh.get(ctx, (size_t)nl));
-    GPL_TRY(rh.get(ctx, (size_t)nr));
-    GPL_TRY(envelope_raw(ctx, lhs, l4.p, lh.p));
-    GPL_TRY(envelope_raw(ctx, rhs, r4.p, rh.p));
-    // ---- grid over the right side's union box ------------------------------------------------------------------------------
-    GridBuild grid;
-    GPL_TRY(join_grid_build(ctx, r4.p, rh.p, nr, nr, "gpl_spatial_join", grid));
-    if (grid.jg.g == 0) return GPL_OK;  // no right row has an envelope
-    // ---- candidates: count -> scan -> write ----------------------------------------------------------------------------------
-    Scratch<int32_t> cand_count;
-    Scratch<int64_t> tot, cand_off;
-    GPL_TRY(tot.get(ctx, 1));
-    GPL_TRY(cand_count.get(ctx, (size_t)nl + 1));
-    GPL_TRY(cand_off.get(ctx, (size_t)nl + 2));
-    GPL_LAUNCH(ctx, k_join_candidates<0>, (int)ceil_div(nl, 128), 128, 0, l4.p, lh.p, nl, r4.p, grid.jg, grid.ux1, grid.uy1, grid.cell_start.p,
-               grid.items.p, cand_count.p, nullptr, nullptr, nullptr);
-    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cand_count.p, nl, cand_off.p, tot.p)));
-    int64_t n_cand = 0;
-    GPL_CUDA(cudaMemcpyAsync(&n_cand, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (n_cand == 0) return GPL_OK;
-    Scratch<uint64_t> cl, cr;
-    GPL_TRY(cl.get(ctx, (size_t)n_cand));
-    GPL_TRY(cr.get(ctx, (size_t)n_cand));
-    GPL_LAUNCH(ctx, k_join_candidates<1>, (int)ceil_div(nl, 128), 128, 0, l4.p, lh.p, nl, r4.p, grid.jg, grid.ux1, grid.uy1, grid.cell_start.p,
-               grid.items.p, nullptr, cand_off.p, cl.p, cr.p);
-    // ---- exact predicate per candidate ------------------------------------------------------------------------------------------
-    Scratch<uint8_t> hit;
-    GPL_TRY(hit.get(ctx, (size_t)n_cand));
-    const double2 *lxy = reinterpret_cast<const double2 *>(lhs->xy), *rxy = reinterpret_cast<const double2 *>(rhs->xy);
-    const Side sl{tl, lxy, lhs->geom_off, lhs->part_off, lhs->ring_off}, sr{tr, rxy, rhs->geom_off, rhs->part_off, rhs->ring_off};
-    const int pgrid = warp_grid(n_cand, 8);
-    switch (mode) {
-    case POINT_IN_R: GPL_LAUNCH(ctx, k_contains_point_pairs, pgrid, 256, 0, n_cand, sr, rhs->validity, lxy, lhs->validity, cr.p, cl.p, hit.p); break;
-    case POINT_IN_L: GPL_LAUNCH(ctx, k_contains_point_pairs, pgrid, 256, 0, n_cand, sl, lhs->validity, rxy, rhs->validity, cl.p, cr.p, hit.p); break;
-    case POLY_CONTAINS:
-        GPL_LAUNCH(ctx, k_contains_polygon, pgrid, 256, 0, n_cand, polygon_view(lhs), tl == GPL_MULTIPOLYGON ? lhs->geom_off : nullptr, lhs->validity,
-                   polygon_view(rhs), rhs->validity, cl.p, cr.p, hit.p);
-        break;
-    default: GPL_LAUNCH(ctx, k_intersects_pairs, pgrid, 256, 0, n_cand, sl, lhs->validity, sr, rhs->validity, cl.p, cr.p, hit.p); break;
-    }
-    // ---- compaction ----------------------------------------------------------------------------------------------------------------
-    Scratch<int64_t> hit_off;
-    GPL_TRY(hit_off.get(ctx, (size_t)n_cand + 2));
-    GPL_TRY((exclusive_scan<uint8_t, int64_t>(ctx, hit.p, n_cand, hit_off.p, tot.p)));
-    int64_t n_hit = 0;
-    GPL_CUDA(cudaMemcpyAsync(&n_hit, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (n_hit == 0) return GPL_OK;
-    void *pl = nullptr, *pr = nullptr;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)n_hit, &pl));
-    res->lhs = (uint64_t *)pl;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)n_hit, &pr));
-    res->rhs = (uint64_t *)pr;
-    res->n = n_hit;
-    GPL_LAUNCH(ctx, k_join_compact, (int)ceil_div(n_cand, 256), 256, 0, hit.p, hit_off.p, n_cand, cl.p, cr.p, res->lhs, res->rhs);
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch lists above return to the cache when this scope ends
-    return GPL_OK;
+    JoinTest test;
+    if (tl == GPL_POINT && (cr_ == 2 || tr == GPL_LINESTRING || tr == GPL_MULTILINESTRING)) test = JOIN_POINT_IN_R;       // :91, :95, :130-134
+    else if (tr == GPL_POINT && (cl_ == 2 || tl == GPL_LINESTRING || tl == GPL_MULTILINESTRING)) test = JOIN_POINT_IN_L;  // :92, :96, :129-133
+    else if ((tl == GPL_POLYGON || tl == GPL_MULTIPOLYGON) && tr == GPL_POLYGON) test = predicate == GPL_PREDICATE_CONTAINS ? JOIN_POLY_CONTAINS : JOIN_INTERSECTS;  // :99-115
+    else if (tl == GPL_POLYGON && tr == GPL_MULTIPOLYGON && predicate == GPL_PREDICATE_INTERSECTS) test = JOIN_INTERSECTS;  // :118-122
+    else return GPL_OK;
+    return join_candidate_pairs(ctx, lhs, rhs, test, "gpl_spatial_join", res);
 }

@@ -422,6 +422,28 @@ def haversine_distance(a: DeviceArray, b: DeviceArray) -> Tuple[np.ndarray, np.n
     return out, _bits(bm, n)
 
 
+def intersection_area(a: DeviceArray, b: DeviceArray) -> Tuple[np.ndarray, np.ndarray]:
+    """row-wise area of the intersection of the closed regions a[i] and b[i], both (Multi)Polygon columns (DESIGN.md §4.16);
+    (values, valid) — a null row or a non-finite coordinate gives an invalid row, an empty geometry 0.  The operands must be
+    valid (OGC); on invalid input the value is finite but not specified."""
+    n = len(a)
+    out = np.empty(n, dtype=np.float64)
+    bm = np.zeros((n + 7) // 8, dtype=np.uint8)
+    check(a.ctx.lib.gpl_intersection_area(a.ctx._h, a._h, b._h, _np_ptr(out), _np_ptr(bm), GPL_HOST))
+    return out, _bits(bm, n)
+
+
+def overlay_area_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """(lhs uint64, rhs uint64, area float64) for every pair of rows of two (Multi)Polygon columns whose closed geometries
+    intersect (touching pairs included, with area 0), sorted by (lhs, rhs); the area of a pair is bit for bit what
+    `intersection_area` returns for it"""
+    h = C.c_void_p()
+    check(lhs.ctx.lib.gpl_overlay_area_join(lhs.ctx._h, lhs._h, rhs._h, C.byref(h)))
+    a, b, d = _pairs_with_distance(lhs.ctx, h, True)
+    order = np.lexsort((b, a))
+    return a[order], b[order], d[order]
+
+
 def intersects(a: DeviceArray, b: DeviceArray) -> np.ndarray:
     n = len(a)
     bm = np.zeros((n + 7) // 8, dtype=np.uint8)

@@ -271,6 +271,14 @@ class GeoRustSeries:
         out, valid = E.haversine_distance(self._d(), other.device)
         return _f64(out, valid)
 
+    def intersection_area(self, other: GeoSeries):
+        """row-wise area of the intersection of self[i] and other[i], both (Multi)Polygon columns (GeoPandas'
+        `a.intersection(b).area`; only the area is computed, DESIGN.md §4.16).  Null when either row is null or has a
+        non-finite coordinate; 0 for an empty geometry; never negative.  Rings may have any orientation and need not be
+        closed.  The operands must be valid (OGC): on invalid input the value is finite but not specified."""
+        out, valid = E.intersection_area(self._d(), other.device)
+        return _f64(out, valid)
+
     def translate(self, xoff: float = 0.0, yoff: float = 0.0) -> GeoSeries:
         return self._wrap(E.translate(self._d(), xoff, yoff))
 
@@ -390,6 +398,26 @@ def _left_rows(a, b, d, unmatched):
     d = np.concatenate([d, np.full(len(unmatched), np.nan)])
     order = np.lexsort((b, a))
     return a[order], b[order], d[order]
+
+
+def overlay_area_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner"):
+    """Area-weighted overlay join of two (Multi)Polygon columns (GeoPandas' `overlay(a, b, how="intersection")` followed by
+    `.area`, without building the intersection polygons): (lhs_index int64, rhs_index int64, area float64) for every pair
+    whose closed geometries intersect — exactly the pairs `lhs.geo.intersects` accepts row-wise — sorted by (lhs, rhs).  The
+    area is bit for bit what `lhs.geo.intersection_area` computes for the pair.  Pairs that only touch are kept with area 0,
+    so the areas of a row over a partition sum to the row's area; keep `area > 0` to drop them.  how='inner' -> matched left
+    rows only; how='left' -> unmatched left rows once, with rhs_index -1 and area NaN.  The operands must be valid (OGC); on
+    invalid input the areas are finite but not specified (DESIGN.md §4.16)."""
+    if how not in ("inner", "left"):
+        raise ValueError("how must be 'inner' or 'left'")
+    a, b, d = E.overlay_area_join(lhs.device, rhs.device)
+    a = a.astype(np.int64)
+    b = b.astype(np.int64)
+    if how == "left":
+        matched = np.zeros(len(lhs), dtype=bool)
+        matched[a] = True
+        a, b, d = _left_rows(a, b, d, np.nonzero(~matched)[0])
+    return a, b, d
 
 
 def geo_nearest_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", max_distance: Optional[float] = None):

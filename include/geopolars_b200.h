@@ -360,8 +360,27 @@ int gpl_dwithin_count(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_arra
  * also keeps d(i, j) of each pair (gpl_pairs_copy_distance) */
 int gpl_dwithin_join_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int with_distance,
                            gpl_pairs **out);
-/* the distance of each pair of a list built with distances (any other list: GPL_ERR_INVALID_ARG); distance[n] in `mem` */
+/* the distance of each pair of a list built with distances (any other list: GPL_ERR_INVALID_ARG); distance[n] in `mem`.
+ * For a list from gpl_overlay_area_join the value of each pair is its intersection area. */
 int gpl_pairs_copy_distance(gpl_ctx *ctx, const gpl_pairs *pairs, double *distance, int mem);
+
+/* ---------------------------------------------------------------- intersection area ------ */
+/* Area of the intersection of the closed regions a[i] and b[i] (geo's BooleanOps::intersection(..).unsigned_area(); only the
+ * area is computed, never the intersection polygons), DESIGN.md §4.16.  Both columns Polygon or MultiPolygon, in any
+ * combination (else GPL_ERR_INVALID_TYPE); unequal lengths: GPL_ERR_LENGTH_MISMATCH.  Rings are used whatever their stored
+ * orientation; unclosed rings are closed as Polygon::new does; a ring with fewer than 4 coordinates after closing contributes
+ * nothing.  A null row, or a row with a non-finite coordinate, gives null (NaN, validity 0); an empty geometry gives 0.  The
+ * value is never negative, and exactly 0.0 when no edges cross and no vertex of either side lies inside the other.  The
+ * operands must be valid (OGC): on invalid input the value is finite but not specified.  out[n] f64, out_validity bitmap (may be
+ * NULL), both in `mem`.  Deterministic. */
+int gpl_intersection_area(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, double *out, uint8_t *out_validity, int mem);
+/* Area-weighted overlay join of two (Multi)Polygon columns: every pair (i, j) whose closed geometries intersect — exactly the
+ * pairs for which gpl_intersects(lhs[i], rhs[j]) is true, touching pairs included — with the area of lhs[i] ∩ rhs[j], bit for
+ * bit what gpl_intersection_area returns for that row pair (lhs as the first operand).  Touching pairs carry 0 (or rounding
+ * noise clamped at 0), so the areas of the pairs of a row over a partition sum to the row's area.  A device-resident gpl_pairs
+ * in an unspecified order; the area of each pair is read with gpl_pairs_copy_distance.  Fewer than 2^31 rows per side (else
+ * GPL_ERR_UNSUPPORTED); any other type: GPL_ERR_INVALID_TYPE. */
+int gpl_overlay_area_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **out);
 
 /* ---------------------------------------------------------------- great-circle joins ----- */
 /* Great-circle distance in metres of two POINT columns read as (lon, lat) degrees: geo 0.27 HaversineDistance on the mean

@@ -4,7 +4,7 @@ fraction for the coordinate bytes read, and of the nearest join (100 M points ag
 reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
@@ -41,9 +41,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo"), default="all",
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay"), default="all",
                     help="run only the §8 rows, only the point nearest join, only the geometry nearest join, only the "
-                         "distance-within join or only the great-circle joins")
+                         "distance-within join, only the great-circle joins or only the intersection area and overlay join")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
@@ -79,7 +79,9 @@ def main():
             dwithin_rows(args, ctx, dev, st, res)
         if args.only in ("all", "geo"):
             geo_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom", "dwithin", "geo"):
+        if args.only in ("all", "overlay"):
+            overlay_rows(args, ctx, dev, st, res)
+        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -402,6 +404,58 @@ def dwithin_rows(args, ctx, dev, st, res):
     print(json.dumps(r), flush=True)
     del lp, rp, pxy, pro, pgo, moff
     torch.cuda.empty_cache()
+
+
+def overlay_rows(args, ctx, dev, st, res):
+    """intersection area (DESIGN.md §4.16), kernel resident: row-wise on 1 M pairs of config 2's 65-coordinate stars against
+    the same stars shifted by (3, 2), and the overlay join of config 2's 10 000 stars against a 1000 x 1000 grid of unit
+    squares (candidate stage + exact intersects + area, host synchronisations included).  ms, pairs/s and edge pairs/s
+    (the (edge of A, edge of B) pairs of the evaluated row pairs, each examined once per pass): the kernel is FP64 bound."""
+    import numpy as np
+
+    from geopolars_b200 import synth
+
+    lib = ctx.lib
+
+    def rec(name, units, unit_name, edge_pairs, t):
+        r = {"op": name, "units": units, "unit": unit_name, "ms_min": t[0], "ms_avg": t[1], "units_per_s": units / (t[1] * 1e-3),
+             "edge_pairs": edge_pairs, "edge_pairs_per_s": edge_pairs / (t[1] * 1e-3), "card": res["card"], "power_limit": res["power_limit"]}
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    def upload(xy, ring_off, geom_off):
+        t = [torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in (xy, ring_off, geom_off)]
+        n = len(geom_off) - 1
+        return ctx.wrap_device(GeometryType.POLYGON, n, len(xy), t[0].data_ptr(), geom_off_ptr=t[2].data_ptr(), ring_off_ptr=t[1].data_ptr(),
+                               n_rings=len(ring_off) - 1, keepalive=tuple(t))
+
+    n = int(1_000_000 * args.scale)
+    g = int(np.ceil(np.sqrt(n)))
+    xy, ro, go = synth.star_polygons(m=n, grid=g)
+    a, b = upload(xy, ro, go), upload(xy + np.array([3.0, 2.0]), ro, go)
+    out = torch.empty(n, dtype=torch.float64, device=dev)
+    t = timed(st, lambda: E.check(lib.gpl_intersection_area(ctx._h, a._h, b._h, C.c_void_p(out.data_ptr()), None, E.GPL_DEVICE)), reps=3, warm=1)
+    rec("intersection_area (%d star pairs, 64 x 64 edges)" % n, n, "row pairs", n * 64 * 64, t)
+    del a, b
+
+    sxy, sro, sgo = synth.star_polygons()
+    stars = upload(sxy, sro, sgo)
+    k = int(1000 * np.sqrt(args.scale))
+    i, j = np.meshgrid(np.arange(k, dtype=np.float64), np.arange(k, dtype=np.float64), indexing="xy")
+    x0, y0 = i.ravel() * (1000.0 / k), j.ravel() * (1000.0 / k)
+    w = 1000.0 / k
+    gxy = np.stack([np.stack([x0, x0 + w, x0 + w, x0, x0], 1), np.stack([y0, y0, y0 + w, y0 + w, y0], 1)], 2).reshape(-1, 2)
+    cells = upload(gxy, np.arange(k * k + 1, dtype=np.int64) * 5, np.arange(k * k + 1, dtype=np.int64))
+    n_pairs = [0]
+
+    def join():
+        h = C.c_void_p()
+        E.check(lib.gpl_overlay_area_join(ctx._h, stars._h, cells._h, C.byref(h)))
+        n_pairs[0] = int(lib.gpl_pairs_count(h))
+        lib.gpl_pairs_free(h)
+
+    t = timed(st, join, reps=3, warm=1)
+    rec("overlay_area_join (10 000 stars x %d squares)" % (k * k), n_pairs[0], "pairs", n_pairs[0] * 64 * 4, t)
 
 
 def geo_rows(args, ctx, dev, st, res):
