@@ -1360,8 +1360,16 @@ __device__ __forceinline__ void ld256f(const float4 *p, float4 &a, float4 &b) { 
     asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w) : "l"(p));
     asm("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w) : "l"(p + 1));
 }
-// returns Polygon::contains for a plain part when `undecided` stays false
-__device__ __forceinline__ bool fast_walk(const float4 *__restrict__ fast, const PartLite &l, double px, double py, bool &undecided) {
+// What the FP32 walk of one (point, plain part) needs before its first load: the point relative to the part origin, the
+// filter's bounds and the list (b, side) as a record index into the fast table.  False when no listed edge can act on p.
+// fast_walk and the batched walk of k_pip_stream both take it from here, so both read the list the build wrote p's
+// bucket into.
+struct FastQuery {
+    float qx, qy, eta, B;
+    int32_t list;  // fast-table record of the list header (the table's offsets are int32: ph_fast_plan's scan)
+    bool und;
+};
+__device__ __forceinline__ bool fast_setup(const PartLite &l, double px, double py, FastQuery &q) {
     const double xlo = (double)l.xminf, xhi = (double)l.xmaxf;
     if (!(px >= xlo && px <= xhi)) return false;
     const int32_t nb = l.nb_flags & 0x00ffffff;
@@ -1373,15 +1381,24 @@ __device__ __forceinline__ bool fast_walk(const float4 *__restrict__ fast, const
     // t < 0 <=> p.y < yminf <= ymin ; t >= nb + 1 => p.y > ymax : no listed edge can act
     if (t < 0.0 || !(t < (double)(nb + 1))) return false;
     const int32_t b = min((int32_t)t, nb - 1);
-    const float qx = __double2float_rn(right ? px - xlo : xhi - px), qy = __double2float_rn(yrel);
-    const float4 *part = fast + (int64_t)l.bucket_base;
-    const float4 *rec = part + (b * 2 + (right ? 0 : 1)) * kFastListRecs;
+    q.qx = __double2float_rn(right ? px - xlo : xhi - px), q.qy = __double2float_rn(yrel);
+    q.list = l.bucket_base + (b * 2 + (right ? 0 : 1)) * kFastListRecs;
     const float R = fast_extent(l.xminf, l.xmaxf, l.inv_hf, nb);
-    const float eta = 9.5367431640625e-07f * R;                          // 2^-20 R
-    const float B = 1.01f * (8.5f * eta * R + 1.9073486328125e-06f * R * R);  // eta*8.5R + 2^-19 R^2
+    q.eta = 9.5367431640625e-07f * R;                              // 2^-20 R
+    q.B = 1.01f * (8.5f * q.eta * R + 1.9073486328125e-06f * R * R);  // eta*8.5R + 2^-19 R^2
+    q.und = !(q.B >= 1.17549435e-38f);  // defensive: the build never lists a part whose bounds leave the normal range
+    return true;
+}
+// returns Polygon::contains for a plain part when `undecided` stays false
+__device__ __forceinline__ bool fast_walk(const float4 *__restrict__ fast, const PartLite &l, double px, double py, bool &undecided) {
+    FastQuery fq;
+    if (!fast_setup(l, px, py, fq)) return false;
+    const float qx = fq.qx, qy = fq.qy, eta = fq.eta, B = fq.B;
+    const float4 *part = fast + (int64_t)l.bucket_base;
+    const float4 *rec = fast + (int64_t)fq.list;
     const float inf = __int_as_float(0x7f800000);
     int wn = 0;
-    bool und = !(B >= 1.17549435e-38f);  // defensive: the build never lists a part whose bounds leave the normal range
+    bool und = fq.und;
     // the list: header + (kFastListRecs - 1) edges, issued together; sentinels make the count irrelevant here
     float4 r[kFastListRecs];
 #pragma unroll
@@ -1548,8 +1565,9 @@ __global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_pairs(co
 //   code 1      -> the row of the coarse cell's candidate #0: the word's upper half
 //   code 2      -> the row of candidate #1 (one 8-byte load from the 80 KB cand01 table)
 //   code 3      -> appended to the warp's shared-memory queue (ballot + popc compaction).
-// Whenever the queue holds 32 points the warp walks them (walk_point) with all lanes active and overwrites their ids;
-// the rest is drained at the end.  ids are written as streaming 32-bit stores, 128 contiguous bytes per warp-wide store.
+// Whenever the queue holds 32 points the warp walks them with all lanes active (LEAN: as one batch, walk_batch; otherwise
+// one point per lane, walk_point) and overwrites their ids; the rest is drained at the end.  ids are written as streaming
+// 32-bit stores, 128 contiguous bytes per warp-wide store.
 constexpr int kTilePts = 128;
 constexpr int kQueueCap = kTilePts + 32;
 constexpr int kStreamWarps = kQueryThreads / 32;
@@ -1576,6 +1594,136 @@ __device__ __forceinline__ uint2 ldg_na(const uint2 *p) {
     asm("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p));
     return v;
 }
+
+// ---- the batched walk of k_pip_stream<LEAN> ------------------------------------------------------------------------
+// One lane per walked point would fetch every record of the walk with 32 lanes on 32 unrelated lines (one L1TEX wavefront
+// each), although the bytes one point needs are contiguous: a 32-byte cell record, a kFastListRecs-record list and a
+// contiguous overflow run.  The batch loads them as flat per-batch arrays instead, consecutive lanes on consecutive
+// 16-byte records, so one instruction touches a handful of lines, and every load of a phase is issued before any is used:
+//   1. cell records: 32 x 2 records;  the owner lane of each point sets up its FP32 query (fast_setup);
+//   2. lists: 32 x kFastListRecs records (record r belongs to point r / kFastListRecs; the header gives the overflow run);
+//   3. overflow runs: concatenated in point order (warp prefix sum of their lengths), 4 x 32 records per round.
+// Each edge's winding contribution is added into its point's slot (shared-memory atomics: an integer sum and an OR do not
+// depend on the order), so ids, counts and the deferred set are those of the per-lane walk.  A point whose cell record
+// is not a lone plain candidate with FP32 lists takes walk_point, in the same batch.
+struct __align__(16) BatchSmem {  // one warp
+    union {
+        float4 cell[64];  // phase 1: the batch's cell records, two 16-byte halves per point
+        struct {
+            float4 prm[32];  // qx, qy, eta, B of each point
+            int32_t list[32], tail_n[32], tail_off[32], wn[32], und[32];
+        } w;
+    };
+};
+__device__ __forceinline__ void batch_edge(BatchSmem &s, int q, float4 e) {
+    const float4 m = s.w.prm[q];
+    int wn = 0;
+    bool und = false;
+    fast_edge_rule(e, m.x, m.y, m.z, m.w, wn, und);
+    if (wn) atomicAdd(&s.w.wn[q], wn);
+    if (und) s.w.und[q] = 1;
+}
+// every lane of the warp calls it (full-mask shuffles); `active`: the lane holds a point
+__device__ __forceinline__ void walk_batch(const IndexView &ix, BatchSmem &s, const double2 p, const bool active, const bool want_count,
+                                           int32_t &first, int32_t &cnt, bool &undecided) {
+    constexpr int R = kFastListRecs;
+    const int lane = threadIdx.x & 31;
+    const float inf = __int_as_float(0x7f800000);
+    const float4 sentinel = make_float4(0.0f, inf, 0.0f, inf);
+    // phase 1: record 32h + l is half (l & 1) of point 16h + (l >> 1)'s cell record
+    const int64_t cc = active ? coarse_cell(ix.grid, p.x, p.y) : 0;
+    const uint32_t act = __ballot_sync(0xffffffffu, active);
+    float4 half[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int q = 16 * h + (lane >> 1);
+        const int64_t c = __shfl_sync(0xffffffffu, cc, q);
+        half[h] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if ((act >> q) & 1) half[h] = __ldg(reinterpret_cast<const float4 *>(ix.cells + c) + (lane & 1));
+    }
+    s.cell[lane] = half[0];
+    s.cell[32 + lane] = half[1];
+    __syncwarp();
+    int32_t cr[8];
+    {
+        const int4 a = *reinterpret_cast<const int4 *>(&s.cell[2 * lane]), b = *reinterpret_cast<const int4 *>(&s.cell[2 * lane + 1]);
+        cr[0] = a.x, cr[1] = a.y, cr[2] = a.z, cr[3] = a.w, cr[4] = b.x, cr[5] = b.y, cr[6] = b.z, cr[7] = b.w;
+    }
+    __syncwarp();  // the cell records are overwritten below
+    PartLite lite;
+    unpack_lite(cr + 2, lite);
+    const bool batched = active && !ix.multi && cr[0] == 1 && (lite.nb_flags & kFastBit);
+    FastQuery fq;
+    const bool walks = batched && fast_setup(lite, p.x, p.y, fq);  // otherwise p lies outside every listed edge's reach
+    s.w.wn[lane] = 0, s.w.tail_n[lane] = 0, s.w.tail_off[lane] = 0, s.w.und[lane] = walks && fq.und;
+    if (walks) s.w.prm[lane] = make_float4(fq.qx, fq.qy, fq.eta, fq.B), s.w.list[lane] = fq.list;
+    const uint32_t lists = __ballot_sync(0xffffffffu, walks);
+    __syncwarp();
+    // phase 2: the header is skipped by the edge rule; it gives the overflow run (count - (R - 1) records)
+    if (lists) {
+        float4 r[R];
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+            const int k = 32 * j + lane, q = k / R;
+            r[j] = sentinel;
+            if ((lists >> q) & 1) r[j] = __ldg(ix.fast + s.w.list[q] + (k - q * R));
+        }
+#pragma unroll
+        for (int j = 0; j < R; ++j) {
+            const int k = 32 * j + lane, q = k / R;
+            if (!((lists >> q) & 1)) continue;
+            if (k == q * R) {
+                s.w.tail_n[q] = max(__float_as_int(r[j].x) - (R - 1), 0);
+                s.w.tail_off[q] = __float_as_int(r[j].y);
+            } else {
+                batch_edge(s, q, r[j]);
+            }
+        }
+    }
+    __syncwarp();
+    // phase 3: tail record t belongs to the last point whose run starts at or before t
+    const int32_t n = s.w.tail_n[lane];
+    int32_t start = n;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int32_t v = __shfl_up_sync(0xffffffffu, start, o);
+        if (lane >= o) start += v;
+    }
+    const int32_t total = __shfl_sync(0xffffffffu, start, 31);
+    start -= n;
+    const int32_t src = lite.bucket_base + s.w.tail_off[lane] - start;  // + t = fast-table record of tail record t
+    for (int32_t t0 = 0; t0 < total; t0 += 4 * 32) {
+        float4 e[4];
+        int qs[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int32_t t = t0 + 32 * u + lane;
+            int q = 0;
+#pragma unroll
+            for (int step = 16; step > 0; step >>= 1)
+                if (__shfl_sync(0xffffffffu, start, q + step) <= t) q += step;
+            const int32_t at = __shfl_sync(0xffffffffu, src, q) + t;
+            qs[u] = q;
+            e[u] = sentinel;
+            if (t < total) e[u] = __ldg(ix.fast + at);
+        }
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+            if (t0 + 32 * u + lane < total) batch_edge(s, qs[u], e[u]);
+    }
+    __syncwarp();
+    if (walks) {
+        if (s.w.und[lane]) {
+            undecided = true;
+        } else if (s.w.wn[lane] != 0) {
+            first = cr[1];  // a lone candidate: CellRec::first is its part id, the polygon row
+            cnt = 1;
+        }
+    } else if (active && !batched) {
+        walk_point<0, true>(ix, p, want_count, first, cnt, undecided, 0, 0, nullptr, nullptr);
+    }
+}
+
 template <bool LEAN>
 __global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_stream(const IndexView ix, const double2 *__restrict__ pts,
                                                                                const uint8_t *__restrict__ pts_validity, int64_t n_pts,
@@ -1601,11 +1749,16 @@ __global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_stream(c
         double2 p = make_double2(0.0, 0.0);
         uint32_t idx = 0;
         if (active) p = q_pts[e], idx = q_idx[e];
-        __syncwarp();  // every lane holds its entry before the queue is written again
+        __syncwarp();  // every lane holds its entry before the queue (and the batch area) is written again
+        int32_t first = -1, cnt = 0;
+        bool undecided = false;
+        if constexpr (LEAN) {
+            BatchSmem &bs = reinterpret_cast<BatchSmem *>(smem_raw + sizeof(StreamSmem))[wid];
+            walk_batch(ix, bs, p, active, want_count, first, cnt, undecided);
+        } else if (active) {
+            walk_point<0, false>(ix, p, want_count, first, cnt, undecided, 0, 0, nullptr, nullptr);
+        }
         if (active) {
-            int32_t first = -1, cnt = 0;
-            bool undecided = false;
-            walk_point<0, LEAN>(ix, p, want_count, first, cnt, undecided, 0, 0, nullptr, nullptr);
             if (undecided) {
                 first = kDeferred;
                 const unsigned long long slot = atomicAdd(n_deferred, 1ULL);
@@ -1803,7 +1956,7 @@ static void launch_stream(const IndexView &v, const double2 *pts, const uint8_t 
     // bit 0: raster gather without an L1 line; bit 2: the point stream too; bit 1: the point stream too, plus an L2 evict-first
     // policy.  On config 2 (one H100) 0, 1 and 5 are within 1 % of each other.
     static const int hints = env_int("GPL_PIP_LD_HINTS", 5);
-    const size_t smem = sizeof(StreamSmem);
+    const size_t smem = sizeof(StreamSmem) + (LEAN ? sizeof(BatchSmem) * kStreamWarps : 0);
     int occ = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pip_stream<LEAN>, kQueryThreads, smem) != cudaSuccess || occ < 1) occ = 1;
     (void)cudaGetLastError();

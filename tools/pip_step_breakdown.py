@@ -14,7 +14,17 @@ inputs and prints ONE JSON line with min and median over `--reps` steps of:
   durations of the phases;
 * the card's name and power limit, read by nvidia-smi in the same run.
 
-    python tools/pip_step_breakdown.py [--workload c2|c4] [--reps 20] [--warmup 5] [--points N] [--out FILE]
+With `--split`, also `stream_split_ms`: `k_pip_stream` alone (the library's CUDA event pairs around each launch, median
+over `--reps` launches after `--warmup`) on the same index for three point columns of the same size:
+
+* `bench`: the benchmark's points (`gpl_gen_uniform_points`, stream 2);
+* `no_walk`: points that never walk: uniform within +-1/4 fine cell around the centres of random fine cells whose raster
+  code is 0, 1 or 2 (decoded from `PipIndex.dump("raster")`);
+* `outside`: points outside the union bbox: the stream-and-write floor, no raster gather;
+
+and `walk_ms` = bench - no_walk, `raster_ms` = no_walk - outside.
+
+    python tools/pip_step_breakdown.py [--workload c2|c4] [--reps 20] [--warmup 5] [--points N] [--split] [--out FILE]
 
 Needs a CUDA device."""
 import argparse
@@ -24,6 +34,8 @@ import statistics
 import subprocess
 import sys
 import time
+
+import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
@@ -49,9 +61,32 @@ def card():
         return {"name": "unknown", "error": str(e)}
 
 
-def stat(xs):
+def stat(xs, digits=2):
     xs = list(xs)
-    return {"min": round(min(xs), 2), "median": round(statistics.median(xs), 2)} if xs else None
+    return {"min": round(min(xs), digits), "median": round(statistics.median(xs), digits)} if xs else None
+
+
+def split_columns(torch, idx, poly_xy, n, dev):
+    """the `no_walk` and `outside` point columns of --split (n x 2 float64 each, on dev; seeded)"""
+    st = idx.stats()
+    fg = st["fine_cells_per_axis"]
+    x0, y0 = (float(v) for v in poly_xy.min(dim=0).values)
+    x1, y1 = (float(v) for v in poly_xy.max(dim=0).values)
+    words = idx.dump("raster").view(np.uint32).reshape(fg, -1, 2)[:, :, 0]  # (fine row, word): 16 two-bit codes
+    codes = (words[:, :, None] >> (2 * np.arange(16, dtype=np.uint32))) & 3
+    codes = codes.reshape(fg, -1)[:, :fg]
+    keep = torch.from_numpy(np.flatnonzero(codes != 3)).to(dev)
+    g = torch.Generator(device=dev)
+    g.manual_seed(7)
+    pick = keep[torch.randint(0, keep.numel(), (n,), device=dev, generator=g)]
+    fw, fh = (x1 - x0) / fg, (y1 - y0) / fg
+    jit = torch.rand((n, 2), dtype=torch.float64, device=dev, generator=g) * 0.5 + 0.25  # centre +- 1/4 cell
+    no_walk = torch.stack((x0 + ((pick % fg).double() + jit[:, 0]) * fw, y0 + ((pick // fg).double() + jit[:, 1]) * fh), dim=1)
+    del pick, jit
+    outside = torch.rand((n, 2), dtype=torch.float64, device=dev, generator=g)
+    outside[:, 0] = x1 + 1.0 + outside[:, 0] * (x1 - x0)
+    outside[:, 1] = y0 + outside[:, 1] * (y1 - y0)
+    return no_walk.contiguous(), outside
 
 
 def main():
@@ -60,6 +95,7 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--points", type=int, default=0)
+    ap.add_argument("--split", action="store_true", help="also time k_pip_stream alone on bench / no-walk / outside points")
     ap.add_argument("--out", default=None, help="also append the JSON line to this file")
     args = ap.parse_args()
 
@@ -171,6 +207,29 @@ def main():
             elif piece == "fill" and count_end is not None:
                 round_trip.append((s - count_end) * 1e-3)
                 count_end = None
+
+        # 5. --split: the stream kernel alone on one index, three point columns
+        split = None
+        if args.split:
+            idx = state["idx"]
+            no_walk, outside = split_columns(torch, idx, poly_xy, n, dev)
+            split = {}
+            for name, col in (("bench", pts), ("no_walk", no_walk), ("outside", outside)):
+                for _ in range(args.warmup):
+                    idx.query_device(col.data_ptr(), n, ids.data_ptr())
+                stream.synchronize()
+                ctx.kernel_timing(True)
+                ms = []
+                for _ in range(args.reps):
+                    idx.query_device(col.data_ptr(), n, ids.data_ptr())
+                    t, k = ctx.kernel_timing_read()
+                    ms.append(t / k)
+                ctx.kernel_timing(False)
+                split[name] = stat(ms, 3)
+            del no_walk, outside
+            med = {k: v["median"] for k, v in split.items()}
+            split["walk_ms"] = round(med["bench"] - med["no_walk"], 3)
+            split["raster_ms"] = round(med["no_walk"] - med["outside"], 3)
         state["idx"].free()
         stream.synchronize()
 
@@ -189,6 +248,8 @@ def main():
         "build_phases_us": {k: stat(v) for k, v in phases.items()},
         "count_end_to_fill_start_us": stat(count_to_fill),
     }
+    if split is not None:
+        res["stream_split_ms"] = split
     line = json.dumps(res)
     print(line)
     if args.out:
