@@ -77,6 +77,7 @@ extern "C" {
     fn gpl_envelope(ctx: *mut GplCtx, a: *const GplArray, out: *mut *mut GplArray, out4: *mut f64, mem: c_int) -> c_int;
     fn gpl_euclidean_length(ctx: *mut GplCtx, a: *const GplArray, out: *mut f64, mem: c_int) -> c_int;
     fn gpl_geodesic_length(ctx: *mut GplCtx, a: *const GplArray, method: c_int, out: *mut f64, out_validity: *mut u8, mem: c_int) -> c_int;
+    fn gpl_geodesic_area(ctx: *mut GplCtx, a: *const GplArray, sign: c_int, area: *mut f64, perimeter: *mut f64, out_validity: *mut u8, mem: c_int) -> c_int;
     fn gpl_convex_hull(ctx: *mut GplCtx, a: *const GplArray, out: *mut *mut GplArray) -> c_int;
     fn gpl_simplify(ctx: *mut GplCtx, a: *const GplArray, tolerance: f64, out: *mut *mut GplArray) -> c_int;
     fn gpl_distance(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, out: *mut f64, out_validity: *mut u8, mem: c_int) -> c_int;
@@ -233,6 +234,16 @@ fn f64_series(name: &str, v: Vec<f64>, validity_bits: Vec<u8>) -> Series {
     let len = v.len();
     let arr = PrimitiveArray::<f64>::new(polars::export::arrow::datatypes::DataType::Float64, v.into(), Some(Bitmap::from_u8_vec(validity_bits, len)));
     Float64Chunked::from_chunks(name, vec![Box::new(arr) as ArrayRef]).into_series()
+}
+/// gpl_geodesic_area for one of its two outputs: the area (`want_area`) or the perimeter
+fn geodesic_area(s: &Series, sign: c_int, want_area: bool, name: &str) -> Result<Series> {
+    let ctx = ctx()?;
+    let a = to_device(ctx, s)?;
+    let mut v = vec![0f64; s.len()];
+    let mut valid = vec![0u8; (s.len() + 7) / 8];
+    let (area, perimeter) = if want_area { (v.as_mut_ptr(), std::ptr::null_mut()) } else { (std::ptr::null_mut(), v.as_mut_ptr()) };
+    check(unsafe { gpl_geodesic_area(ctx, a.0, sign, area, perimeter, valid.as_mut_ptr(), GPL_HOST) })?;
+    Ok(f64_series(name, v, valid))
 }
 /// copy the input's null mask onto a value column (area / length / x / y of a null geometry is null)
 fn with_validity_of(input: &Series, out: Series) -> Series {
@@ -433,6 +444,15 @@ pub trait GeoSeriesB200Ext {
     /// included, with area 0), as (lhs_index, rhs_index, area) in an unspecified order; the area is bit for bit what
     /// `intersection_area` computes for the pair
     fn overlay_area_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
+    /// geo's `GeodesicArea::geodesic_area_signed` on WGS84 for a column in (lon, lat) degrees, square metres: counter-clockwise
+    /// exteriors positive, holes subtract, multipolygons sum their parts, other types 0; a null row, a non-finite coordinate
+    /// or |lat| > 90 gives null
+    fn geodesic_area_signed(&self) -> Result<Series>;
+    /// geo's `GeodesicArea::geodesic_area_unsigned`: as `geodesic_area_signed` but in [0, area of the ellipsoid), so a
+    /// clockwise exterior gives the ellipsoid's area minus the enclosed area, as in geo
+    fn geodesic_area_unsigned(&self) -> Result<Series>;
+    /// geo's `GeodesicArea::geodesic_perimeter`, metres: the closed geodesic length of every ring, holes included
+    fn geodesic_perimeter(&self) -> Result<Series>;
 }
 
 impl GeoSeriesB200Ext for Series {
@@ -584,6 +604,18 @@ impl GeoSeriesB200Ext for Series {
         let mut valid = vec![0u8; (self.len() + 7) / 8];
         check(unsafe { gpl_intersection_area(ctx, a.0, b.0, v.as_mut_ptr(), valid.as_mut_ptr(), GPL_HOST) })?;
         Ok(f64_series("intersection_area", v, valid))
+    }
+
+    fn geodesic_area_signed(&self) -> Result<Series> {
+        geodesic_area(self, 1, true, "geodesic_area_signed")
+    }
+
+    fn geodesic_area_unsigned(&self) -> Result<Series> {
+        geodesic_area(self, 0, true, "geodesic_area_unsigned")
+    }
+
+    fn geodesic_perimeter(&self) -> Result<Series> {
+        geodesic_area(self, 1, false, "geodesic_perimeter")
     }
 
     fn overlay_area_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)> {

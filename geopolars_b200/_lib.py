@@ -124,6 +124,7 @@ SIGNATURES = {
     "gpl_envelope": (_INT, [_P, _P, C.POINTER(_P), _P, _INT]),
     "gpl_euclidean_length": (_INT, [_P, _P, _P, _INT]),
     "gpl_geodesic_length": (_INT, [_P, _P, _INT, _P, _P, _INT]),
+    "gpl_geodesic_area": (_INT, [_P, _P, _INT, _P, _P, _P, _INT]),
     "gpl_convex_hull": (_INT, [_P, _P, C.POINTER(_P)]),
     "gpl_simplify": (_INT, [_P, _P, _D, C.POINTER(_P)]),
     "gpl_distance": (_INT, [_P, _P, _P, _P, _P, _INT]),

@@ -390,6 +390,19 @@ def geodesic_length(a: DeviceArray, method: str = "geodesic") -> Tuple[np.ndarra
     return out, _bits(bm, n)
 
 
+def geodesic_area(a: DeviceArray, signed: bool) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """geo's GeodesicArea on WGS84 for (lon, lat) degree columns (DESIGN.md §4.17): (area m^2, perimeter m, valid) in one pass.
+    signed=True: counter-clockwise exteriors positive, in (-area0/2, area0/2]; signed=False: in [0, area0).  Polygon holes
+    subtract by magnitude; MultiPolygon rows sum their parts; other types give 0.  A null row, a non-finite coordinate or
+    |lat| > 90 gives an invalid row (NaN)."""
+    n = len(a)
+    area = np.empty(n, dtype=np.float64)
+    perimeter = np.empty(n, dtype=np.float64)
+    bm = np.zeros((n + 7) // 8, dtype=np.uint8)
+    check(a.ctx.lib.gpl_geodesic_area(a.ctx._h, a._h, 1 if signed else 0, _np_ptr(area), _np_ptr(perimeter), _np_ptr(bm), GPL_HOST))
+    return area, perimeter, _bits(bm, n)
+
+
 def simplify(a: DeviceArray, tolerance: float) -> DeviceArray:
     """GeoSeries::simplify (geoseries.rs:108-116): geo's Ramer-Douglas-Peucker"""
     return _out_array(a.ctx, a.ctx.lib.gpl_simplify, a._h, C.c_double(float(tolerance)))

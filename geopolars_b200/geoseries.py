@@ -227,6 +227,24 @@ class GeoRustSeries:
         out, valid = E.geodesic_length(self._d(), method)
         return _f64(out, valid)
 
+    def geodesic_area_signed(self):
+        """geo's GeodesicArea::geodesic_area_signed on WGS84, square metres, for (lon, lat) degree columns (DESIGN.md §4.17):
+        counter-clockwise exteriors positive, holes subtract.  Null for a null row, a non-finite coordinate or |lat| > 90"""
+        area, _, valid = E.geodesic_area(self._d(), signed=True)
+        return _f64(area, valid)
+
+    def geodesic_area_unsigned(self):
+        """geo's GeodesicArea::geodesic_area_unsigned on WGS84, square metres, in [0, area of the ellipsoid): a clockwise
+        exterior gives the ellipsoid's area minus the enclosed area, as in geo.  Nulls as geodesic_area_signed"""
+        area, _, valid = E.geodesic_area(self._d(), signed=False)
+        return _f64(area, valid)
+
+    def geodesic_perimeter(self):
+        """geo's GeodesicArea::geodesic_perimeter on WGS84, metres: the closed geodesic length of every ring, holes included
+        (geodesic_length uses the exterior only).  Nulls as geodesic_area_signed"""
+        _, perimeter, valid = E.geodesic_area(self._d(), signed=True)
+        return _f64(perimeter, valid)
+
     @property
     def geom_type(self):
         return _pa().array(E.geom_type(self._d()))

@@ -205,6 +205,19 @@ int gpl_euclidean_length(gpl_ctx *ctx, const gpl_array *in, double *out, int mem
  * (lon, lat) degrees.  method 0 = geodesic (Karney 2013, WGS84), 1 = haversine, 2 = vincenty.  out_validity
  * (optional bitmap): a row is null when a Vincenty segment does not converge (the reference returns Err) */
 int gpl_geodesic_length(gpl_ctx *ctx, const gpl_array *in, int method, double *out, uint8_t *out_validity, int mem);
+/* geo 0.27 GeodesicArea on WGS84 (DESIGN.md 4.17), input in (lon, lat) degrees, any finite longitude.  One pass fills
+ * area[n] (m^2) and perimeter[n] (m); either may be NULL, not both.  Each ring is geographiclib's PolygonArea over its
+ * vertices, closing edge always included (a ring whose last coordinate equals its first is summed without that zero-length
+ * edge, so a closed and an unclosed copy of a ring agree bit for bit), reduced modulo the
+ * ellipsoid's area A0.  sign = 1: counter-clockwise positive, in (-A0/2, A0/2]; sign = 0: in [0, A0), so a clockwise exterior
+ * gives A0 minus the enclosed area, as in geo.  Polygon: exterior minus the summed magnitudes of the holes (holes taken
+ * clockwise positive; a negative exterior subtracts a negated sum), so with wrongly wound rings an unsigned value can leave
+ * [0, A0) as geo's does; perimeter over every ring.  MultiPolygon: the sum over its
+ * parts.  Point / LineString / MultiPoint / MultiLineString: 0.  Empty rows: 0.  A null row, a non-finite coordinate or
+ * |lat| > 90 gives a null row (NaN, validity 0 in out_validity, which may be NULL).  Results are deterministic and a row's
+ * value does not depend on the other rows of the call.  NULL ctx / in, both outputs NULL, sign not 0 or 1, or an unknown
+ * mem: GPL_ERR_INVALID_ARG before any launch. */
+int gpl_geodesic_area(gpl_ctx *ctx, const gpl_array *in, int sign, double *area, double *perimeter, uint8_t *out_validity, int mem);
 /* GeoSeries::convex_hull (geoseries.rs:23-26): POLYGON array, one closed CCW ring per geometry, in
  * geo's quick_hull vertex order */
 int gpl_convex_hull(gpl_ctx *ctx, const gpl_array *in, gpl_array **out);

@@ -4,7 +4,7 @@ fraction for the coordinate bytes read, and of the nearest join (100 M points ag
 reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
@@ -41,9 +41,11 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay"), default="all",
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic"), default="all",
                     help="run only the §8 rows, only the point nearest join, only the geometry nearest join, only the "
-                         "distance-within join, only the great-circle joins or only the intersection area and overlay join")
+                         "distance-within join, only the great-circle joins, only the intersection area and overlay join or "
+                         "only the geodesic area and perimeter (1 M stars, 10 M parcels, naturalearth_lowres to 1 M rows); "
+                         "'all' runs every arm")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
@@ -81,7 +83,9 @@ def main():
             geo_rows(args, ctx, dev, st, res)
         if args.only in ("all", "overlay"):
             overlay_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay"):
+        if args.only in ("all", "geodesic"):
+            geodesic_rows(args, ctx, dev, st, res)
+        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -456,6 +460,103 @@ def overlay_rows(args, ctx, dev, st, res):
 
     t = timed(st, join, reps=3, warm=1)
     rec("overlay_area_join (10 000 stars x %d squares)" % (k * k), n_pairs[0], "pairs", n_pairs[0] * 64 * 4, t)
+
+
+def geodesic_rows(args, ctx, dev, st, res):
+    """geodesic area and perimeter on WGS84 (DESIGN.md §4.17), kernel resident, one call filling both outputs: 1 M config-2
+    stars (65 coordinates, 65 edges each) mapped to (lon, lat) with radii near 0.01 degrees over |lat| <= 80, 10 M closed
+    5-coordinate parcels (about 20 m), and naturalearth_lowres repeated to about 1 M rows.  ms, rows/s and edges/s (an edge is
+    one inverse solve with the area term: FP64 and transcendental bound).  The CPU arm is the C oracle with every core
+    (threads=0) on the first 10 % of the rows of each input: og_geodesic_length(method="geodesic") runs the same Karney
+    inverse solve for every edge of the exterior rings, without the area term, so its edges/s bound what a CPU area pass
+    could reach from above."""
+    import time
+
+    import numpy as np
+
+    from geopolars_b200 import datasets, synth
+
+    from oracle import oracle as og
+
+    lib = ctx.lib
+    rng = np.random.default_rng(2024)
+
+    def rec(name, rows, edges, t, cpu_edges_per_s):
+        r = {"op": name, "units": rows, "unit": "rows", "ms_min": t[0], "ms_avg": t[1], "units_per_s": rows / (t[1] * 1e-3),
+             "edges": edges, "edges_per_s": edges / (t[1] * 1e-3), "cpu_oracle_threads": og.max_threads(), "cpu_oracle_edges_per_s": cpu_edges_per_s,
+             "card": res["card"], "power_limit": res["power_limit"]}
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    def upload(type_, xy, ring_off, geom_off, part_off=None):
+        vs = [xy, ring_off, geom_off] + ([part_off] if part_off is not None else [])
+        t = [torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in vs]
+        return ctx.wrap_device(type_, len(geom_off) - 1, len(xy), t[0].data_ptr(), geom_off_ptr=t[2].data_ptr(), ring_off_ptr=t[1].data_ptr(),
+                               part_off_ptr=t[3].data_ptr() if part_off is not None else None, n_rings=len(ring_off) - 1,
+                               n_parts=len(part_off) - 1 if part_off is not None else 0, keepalive=tuple(t))
+
+    def cpu_rate(type_, xy, ring_off, geom_off, part_off):
+        """C oracle (threads=0) Karney solves per second over the exterior-ring edges of the first 10 % of the rows"""
+        k = max(1, (len(geom_off) - 1) // 10)
+        go = geom_off[: k + 1]
+        if type_ == GeometryType.MULTIPOLYGON:
+            po = part_off[: go[-1] + 1]
+            ro = ring_off[: po[-1] + 1]
+            exterior = po[:-1][po[1:] > po[:-1]]
+            a = og.OGArray(og.MULTIPOLYGON, xy[: ro[-1]], geom_off=go, part_off=po, ring_off=ro)
+        else:
+            ro = ring_off[: go[-1] + 1]
+            exterior = go[:-1][go[1:] > go[:-1]]
+            a = og.OGArray(og.POLYGON, xy[: ro[-1]], geom_off=go, ring_off=ro)
+        edges = int(np.maximum(ro[exterior + 1] - ro[exterior] - 1, 0).sum())
+        og.geodesic_length(a, "geodesic", threads=0)  # warm-up: loads the library and starts the threads
+        t0 = time.perf_counter()
+        og.geodesic_length(a, "geodesic", threads=0)
+        return edges / (time.perf_counter() - t0)
+
+    def measure(name, type_, xy, ring_off, geom_off, part_off=None):
+        a = upload(type_, xy, ring_off, geom_off, part_off)
+        n = len(geom_off) - 1
+        area = torch.empty(n, dtype=torch.float64, device=dev)
+        per = torch.empty(n, dtype=torch.float64, device=dev)
+        t = timed(st, lambda: E.check(lib.gpl_geodesic_area(ctx._h, a._h, 1, C.c_void_p(area.data_ptr()), C.c_void_p(per.data_ptr()), None,
+                                                            E.GPL_DEVICE)), reps=3, warm=1)
+        rec(name, n, len(xy), t, cpu_rate(type_, xy, ring_off, geom_off, part_off))
+        del a, area, per
+        torch.cuda.empty_cache()
+
+    n = int(1_000_000 * args.scale)
+    g = int(np.ceil(np.sqrt(n)))
+    xy, ro, go = synth.star_polygons(m=n, grid=g)
+    c = (xy[ro[:-1]] + xy[ro[:-1] + 32]) / 2  # centre of each star (vertex 0 and 32 are opposite)
+    ll = np.stack([rng.uniform(-180, 180, n), rng.uniform(-80, 80, n)], 1)
+    xy = (np.repeat(ll, 65, 0) + (xy - np.repeat(c, 65, 0)) * (0.01 / 4.0))
+    measure("geodesic_area (%d stars, 65 coordinates, r ~ 0.01 deg)" % n, GeometryType.POLYGON, xy, ro, go)
+    del xy
+
+    n = int(10_000_000 * args.scale)
+    ll = np.stack([rng.uniform(-180, 180, n), rng.uniform(-80, 80, n)], 1)
+    d = 0.0002 * rng.uniform(0.5, 1.5, (n, 2))
+    q = np.empty((n, 5, 2))
+    q[:, 0] = ll
+    q[:, 1] = ll + [1, 0] * d
+    q[:, 2] = ll + d
+    q[:, 3] = ll + [0, 1] * d
+    q[:, 4] = ll
+    measure("geodesic_area (%d parcels, 5 coordinates, ~20 m)" % n, GeometryType.POLYGON, q.reshape(-1, 2), np.arange(n + 1, dtype=np.int64) * 5,
+            np.arange(n + 1, dtype=np.int64))
+    del q
+
+    h = datasets.read_dataset("naturalearth_lowres").geometry.device.to_host()
+    reps = max(1, int(round(1_000_000 * args.scale / len(h.geom_off[:-1]))))
+    h_part = h.part_off if h.type == GeometryType.MULTIPOLYGON else np.arange(len(h.geom_off), dtype=np.int64)
+    h_geom = h.geom_off if h.type == GeometryType.MULTIPOLYGON else np.arange(len(h.geom_off), dtype=np.int64)
+    nc, nr, npart = len(h.xy), len(h.ring_off) - 1, len(h_part) - 1
+    xy = np.tile(h.xy, (reps, 1))
+    ro = np.concatenate([h.ring_off[:-1] + k * nc for k in range(reps)] + [[reps * nc]]).astype(np.int64)
+    po = np.concatenate([(h_part if h.type == GeometryType.MULTIPOLYGON else h.geom_off)[:-1] + k * nr for k in range(reps)] + [[reps * nr]]).astype(np.int64)
+    go = np.concatenate([h_geom[:-1] + k * npart for k in range(reps)] + [[reps * npart]]).astype(np.int64)
+    measure("geodesic_area (naturalearth_lowres x %d, %d rows)" % (reps, len(go) - 1), GeometryType.MULTIPOLYGON, xy, ro, go, po)
 
 
 def geo_rows(args, ctx, dev, st, res):
