@@ -1565,16 +1565,39 @@ __global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_pairs(co
 //   code 1      -> the row of the coarse cell's candidate #0: the word's upper half
 //   code 2      -> the row of candidate #1 (one 8-byte load from the 80 KB cand01 table)
 //   code 3      -> appended to the warp's shared-memory queue (ballot + popc compaction).
-// Whenever the queue holds 32 points the warp walks them with all lanes active (LEAN: as one batch, walk_batch; otherwise
-// one point per lane, walk_point) and overwrites their ids; the rest is drained at the end.  ids are written as streaming
-// 32-bit stores, 128 contiguous bytes per warp-wide store.
+// Whenever the queue holds 32 points the warp walks its 32 oldest ones with all lanes active (LEAN: as one batch,
+// walk_batch; otherwise one point per lane, walk_point); the rest is drained at the end.
+// Output: the ids (and counts) of a tile go to one slot of the warp's ring of kRing tiles in shared memory, and the walk
+// writes its results there too.  A tile leaves the kernel once, as one coalesced streaming store of whole lines, when its
+// slot is taken again kRing tiles later or at the end, instead of once from stage 3 and again, one scattered 4-byte store
+// per walked point, from the walk (config 2 on one H100 80GB HBM3 at 700 W: 2.24 -> 1.94 ms, DESIGN.md 4.2).  The queue
+// is FIFO (a circular buffer), so a tile's walkers are the queue's oldest entries by the time its slot is needed; any of
+// them still waiting are walked first (a partial batch if fewer than 32 are queued).
 constexpr int kTilePts = 128;
-constexpr int kQueueCap = kTilePts + 32;
+constexpr int kQueueCap = kTilePts + 32;  // < 32 entries stay after a walk, a tile adds <= 128
 constexpr int kStreamWarps = kQueryThreads / 32;
+constexpr int kRing = 4;  // power of two: tile j of a warp uses slot j & (kRing - 1)
+static_assert((kRing & (kRing - 1)) == 0, "kRing must be a power of two");
 struct __align__(16) StreamSmem {
     double2 q_pts[kStreamWarps][kQueueCap];
-    uint32_t q_idx[kStreamWarps][kQueueCap];
+    uint32_t q_idx[kStreamWarps][kQueueCap];  // slot * kTilePts + the point's row in its tile: its place in the ring
+    int32_t ring_ids[kStreamWarps][kRing * kTilePts];
+    uint32_t ring_tile[kStreamWarps][kRing];  // the tile (chunk-relative) each slot holds
 };
+// with counts, the dynamic shared memory continues with int32_t ring_cnt[kStreamWarps][kRing * kTilePts]
+constexpr size_t kRingCntBytes = sizeof(int32_t) * kStreamWarps * kRing * kTilePts;
+// the ring slot `src` to rows [0, rows) of the column at dst: 16 bytes per lane when the whole tile is stored and dst is
+// 16-byte aligned (tiles start at multiples of 512 bytes, so that is the column's own alignment), 4 bytes per lane otherwise
+__device__ __forceinline__ void store_tile(int32_t *dst, const int32_t *src, int64_t rows) {
+    const int lane = threadIdx.x & 31;
+    if (rows >= kTilePts && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+        __stcs(reinterpret_cast<int4 *>(dst) + lane, reinterpret_cast<const int4 *>(src)[lane]);
+    } else {
+#pragma unroll
+        for (int k = 0; k < kTilePts / 32; ++k)
+            if (lane + 32 * k < rows) __stcs(dst + lane + 32 * k, src[lane + 32 * k]);
+    }
+}
 // cache-hint variants (GPL_PIP_LD_HINTS, A/B switch): the point stream without an L1 line (L2: evict first), the raster gather
 // (20 MB of random 8-byte words: no reuse an L1 could catch) without one — leaves the L1 to the cell / part / edge records.
 // `hints` stays a kernel argument: with the default fixed at compile time, ptxas allocates the registers of both
@@ -1739,17 +1762,28 @@ __global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_stream(c
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     double2 *q_pts = sm.q_pts[wid];
     uint32_t *q_idx = sm.q_idx[wid];
-    int qn = 0;  // points waiting in this warp's queue (warp-uniform)
+    int32_t *ring_ids = sm.ring_ids[wid];
+    uint32_t *ring_tile = sm.ring_tile[wid];
+    const bool want_count = count != nullptr;
+    int32_t *ring_cnt = nullptr;
+    if (want_count)
+        ring_cnt = reinterpret_cast<int32_t *>(smem_raw + sizeof(StreamSmem) + (LEAN ? sizeof(BatchSmem) * kStreamWarps : 0)) +
+                   wid * kRing * kTilePts;
+    int qh = 0, qn = 0;  // the oldest entry of this warp's queue and the number queued (warp-uniform)
     const int64_t n_tiles = (n_pts + kTilePts - 1) / kTilePts;
     const int64_t n_warps = (int64_t)gridDim.x * kStreamWarps;
     int64_t tile = (int64_t)blockIdx.x * kStreamWarps + wid;
-    const bool want_count = count != nullptr;
 
-    auto walk_queued = [&](int e, bool active) {
+    // walks the n (1 ... 32) oldest queue entries, one per lane, and writes their results into the ring
+    auto walk_oldest = [&](int n) {
+        const bool active = lane < n;
+        const int e = qh + lane < kQueueCap ? qh + lane : qh + lane - kQueueCap;
         double2 p = make_double2(0.0, 0.0);
-        uint32_t idx = 0;
-        if (active) p = q_pts[e], idx = q_idx[e];
+        uint32_t at = 0;
+        if (active) p = q_pts[e], at = q_idx[e];
         __syncwarp();  // every lane holds its entry before the queue (and the batch area) is written again
+        qh = qh + n < kQueueCap ? qh + n : qh + n - kQueueCap;
+        qn -= n;
         int32_t first = -1, cnt = 0;
         bool undecided = false;
         if constexpr (LEAN) {
@@ -1762,11 +1796,20 @@ __global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_stream(c
             if (undecided) {
                 first = kDeferred;
                 const unsigned long long slot = atomicAdd(n_deferred, 1ULL);
-                if (slot < list_cap) deferred_list[slot] = idx;  // chunk-relative index (chunks are < 2^32 points)
+                // chunk-relative index (chunks are < 2^32 points)
+                if (slot < list_cap) deferred_list[slot] = ring_tile[at / kTilePts] * kTilePts + at % kTilePts;
             }
-            first_id[idx] = first;
-            if (want_count) count[idx] = cnt;
+            ring_ids[at] = first;
+            if (want_count) ring_cnt[at] = cnt;
         }
+    };
+    // the tile in slot s leaves the kernel; its walkers must have been walked
+    auto flush = [&](int s) {
+        __syncwarp();  // the walk results other lanes wrote into the slot
+        const int64_t base = (int64_t)ring_tile[s] * kTilePts;
+        store_tile(first_id + base, ring_ids + s * kTilePts, n_pts - base);
+        if (want_count) store_tile(count + base, ring_cnt + s * kTilePts, n_pts - base);
+        __syncwarp();  // the slot is read before it is written again
     };
 
     // k-th point of a lane inside a tile: lane-contiguous, so that each warp-wide load reads 512 contiguous bytes
@@ -1784,7 +1827,9 @@ __global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_stream(c
         }
     };
     if (tile < n_tiles) load_tile(tile, nxt);
-    for (; tile < n_tiles; tile += n_warps) {
+    int j = 0;  // the warp's tiles so far
+    for (; tile < n_tiles; tile += n_warps, ++j) {
+        const int s = j & (kRing - 1);
         double2 p[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) p[k] = nxt[k];
@@ -1821,34 +1866,35 @@ __global__ void __launch_bounds__(kQueryThreads, kQueryMinBlocks) k_pip_stream(c
                 }
             }
         }
-        // stage 3: ids out (the queued ones are overwritten by the walk)
+        // stage 3: ids into the ring slot (the queued ones are overwritten by the walk)
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-            const int64_t i = base + slot_of(k);
-            if (i < n_pts) {
-                __stcs(first_id + i, id[k]);
-                if (want_count) __stcs(count + i, (int32_t)(id[k] >= 0));
-            }
+            ring_ids[s * kTilePts + slot_of(k)] = id[k];
+            if (want_count) ring_cnt[s * kTilePts + slot_of(k)] = (int32_t)(id[k] >= 0);
         }
+        if (lane == 0) ring_tile[s] = (uint32_t)tile;
         // stage 4: queue the walkers
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             const bool q = code[k] == 3u;
             const unsigned m = __ballot_sync(0xffffffffu, q);
             if (q) {
-                const int pos = qn + __popc(m & ((1u << lane) - 1u));
+                int pos = qh + qn + __popc(m & ((1u << lane) - 1u));
+                if (pos >= kQueueCap) pos -= kQueueCap;
                 q_pts[pos] = p[k];
-                q_idx[pos] = (uint32_t)(base + slot_of(k));
+                q_idx[pos] = (uint32_t)(s * kTilePts + slot_of(k));
             }
             qn += __popc(m);
         }
         __syncwarp();
-        while (qn >= 32) {
-            qn -= 32;
-            walk_queued(qn + lane, true);
-        }
+        // batches of 32; then what is left of tile j + 1 - kRing, whose slot the next tile takes (the queue's oldest
+        // entries, a partial batch if fewer than 32 are queued), and after the warp's last tile whatever is left
+        const uint32_t s_next = (j + 1) & (kRing - 1);
+        const bool last = tile + n_warps >= n_tiles;
+        while (qn >= 32 || (qn > 0 && (last || q_idx[qh] / kTilePts == s_next))) walk_oldest(min(qn, 32));
+        if (j + 1 >= kRing) flush(s_next);
     }
-    if (qn > 0) walk_queued(lane, lane < qn);
+    for (int d = 1; d < kRing && d <= j; ++d) flush((j - d) & (kRing - 1));  // the warp's last kRing - 1 tiles
 }
 
 // Exact re-evaluation of the points the walk marked kDeferred (those whose filters could not
@@ -1951,12 +1997,13 @@ static int query_grid(int64_t n) {
 }
 // the streaming kernel on exactly the resident CTAs (persistent warps, one tile of 128 points per warp and iteration)
 template <bool LEAN>
-static void launch_stream(const IndexView &v, const double2 *pts, const uint8_t *val, int64_t m, int32_t *first, int32_t *cnt,
+static int launch_stream(const IndexView &v, const double2 *pts, const uint8_t *val, int64_t m, int32_t *first, int32_t *cnt,
                           const gpl_pip_index *idx, cudaStream_t stream) {
     // bit 0: raster gather without an L1 line; bit 2: the point stream too; bit 1: the point stream too, plus an L2 evict-first
     // policy.  On config 2 (one H100) 0, 1 and 5 are within 1 % of each other.
     static const int hints = env_int("GPL_PIP_LD_HINTS", 5);
-    const size_t smem = sizeof(StreamSmem) + (LEAN ? sizeof(BatchSmem) * kStreamWarps : 0);
+    const size_t smem = sizeof(StreamSmem) + (LEAN ? sizeof(BatchSmem) * kStreamWarps : 0) + (cnt ? kRingCntBytes : 0);
+    GPL_CUDA(cudaFuncSetAttribute(k_pip_stream<LEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_pip_stream<LEAN>, kQueryThreads, smem) != cudaSuccess || occ < 1) occ = 1;
     (void)cudaGetLastError();
@@ -1964,6 +2011,7 @@ static void launch_stream(const IndexView &v, const double2 *pts, const uint8_t 
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * occ));
     k_pip_stream<LEAN><<<grid, kQueryThreads, smem, stream>>>(v, pts, val, m, first, cnt, idx->n_deferred, idx->deferred_list,
                                                               idx->deferred_cap, hints);
+    return GPL_OK;
 }
 // counts[id] += number of ids equal to id, for every id in [0, n_polys)
 static int launch_histogram(gpl_ctx *ctx, const int32_t *ids, int64_t n, unsigned long long *counts, int64_t n_polys,
@@ -2001,8 +2049,8 @@ int pip_query(gpl_ctx *ctx, const gpl_pip_index *idx, const double *pts_dev, con
         int32_t *cnt = count_dev ? count_dev + lo : nullptr;
         cudaEvent_t t0 = nullptr, t1 = nullptr;
         if (ctx->kt_on && ctx->kernel_timing_pair(&t0, &t1)) GPL_CUDA(cudaEventRecord(t0, stream));
-        if (idx->lean_ok) launch_stream<true>(v, pts + lo, val, m, first_dev + lo, cnt, idx, stream);
-        else launch_stream<false>(v, pts + lo, val, m, first_dev + lo, cnt, idx, stream);
+        if (idx->lean_ok) GPL_TRY(launch_stream<true>(v, pts + lo, val, m, first_dev + lo, cnt, idx, stream));
+        else GPL_TRY(launch_stream<false>(v, pts + lo, val, m, first_dev + lo, cnt, idx, stream));
         if (t1) GPL_CUDA(cudaEventRecord(t1, stream));
         k_pip_deferred<<<kSMs * 8, 256, 0, stream>>>(v, pts + lo, m, first_dev + lo, cnt, idx->n_deferred, idx->deferred_list, idx->deferred_cap,
                                                      idx->n_deferred + 1);
