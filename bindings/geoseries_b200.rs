@@ -113,6 +113,7 @@ extern "C" {
     fn gpl_geo_nearest_join_pairs(ctx: *mut GplCtx, idx: *const GplGeoIndex, lhs: *const GplArray, max_distance: f64, out: *mut *mut GplPairs, distance: *mut f64, mem: c_int) -> c_int;
     fn gpl_intersection_area(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, out: *mut f64, out_validity: *mut u8, mem: c_int) -> c_int;
     fn gpl_overlay_area_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, out: *mut *mut GplPairs) -> c_int;
+    fn gpl_is_valid(ctx: *mut GplCtx, a: *const GplArray, reason: *mut i8, out_validity: *mut u8, mem: c_int) -> c_int;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -244,6 +245,29 @@ fn geodesic_area(s: &Series, sign: c_int, want_area: bool, name: &str) -> Result
     let (area, perimeter) = if want_area { (v.as_mut_ptr(), std::ptr::null_mut()) } else { (std::ptr::null_mut(), v.as_mut_ptr()) };
     check(unsafe { gpl_geodesic_area(ctx, a.0, sign, area, perimeter, valid.as_mut_ptr(), GPL_HOST) })?;
     Ok(f64_series(name, v, valid))
+}
+/// gpl_is_valid: the reason code of every row and the row validity bitmap
+fn validity_reasons(s: &Series) -> Result<(Vec<i8>, Vec<u8>)> {
+    let ctx = ctx()?;
+    let a = to_device(ctx, s)?;
+    let mut reason = vec![0i8; s.len()];
+    let mut valid = vec![0u8; (s.len() + 7) / 8];
+    check(unsafe { gpl_is_valid(ctx, a.0, reason.as_mut_ptr(), valid.as_mut_ptr(), GPL_HOST) })?;
+    Ok((reason, valid))
+}
+/// gpl_is_valid's reason codes -> GEOS's TopologyValidationError messages
+fn validity_message(code: i8) -> &'static str {
+    match code {
+        0 => "Valid Geometry",
+        2 => "Hole lies outside shell",
+        3 => "Holes are nested",
+        4 => "Interior is disconnected",
+        5 => "Self-intersection",
+        6 => "Ring Self-intersection",
+        7 => "Nested shells",
+        9 => "Too few distinct points in geometry component",
+        _ => "Invalid Coordinate",
+    }
 }
 /// copy the input's null mask onto a value column (area / length / x / y of a null geometry is null)
 fn with_validity_of(input: &Series, out: Series) -> Series {
@@ -453,6 +477,11 @@ pub trait GeoSeriesB200Ext {
     fn geodesic_area_unsigned(&self) -> Result<Series>;
     /// geo's `GeodesicArea::geodesic_perimeter`, metres: the closed geodesic length of every ring, holes included
     fn geodesic_perimeter(&self) -> Result<Series>;
+    /// OGC validity of every row (exact, any geometry type); null rows stay null.  `intersection_area`,
+    /// `overlay_area_join_pairs` and Polygon `contains` need valid operands
+    fn is_valid(&self) -> Result<Series>;
+    /// GEOS's reason message of the first failing validity rule, "Valid Geometry" for a valid row; null rows stay null
+    fn is_valid_reason(&self) -> Result<Series>;
 }
 
 impl GeoSeriesB200Ext for Series {
@@ -616,6 +645,22 @@ impl GeoSeriesB200Ext for Series {
 
     fn geodesic_perimeter(&self) -> Result<Series> {
         geodesic_area(self, 1, false, "geodesic_perimeter")
+    }
+
+    fn is_valid(&self) -> Result<Series> {
+        let (reason, valid) = validity_reasons(self)?;
+        let bits = reason.iter().enumerate().fold(vec![0u8; (reason.len() + 7) / 8], |mut b, (i, &c)| {
+            b[i / 8] |= ((c == 0) as u8) << (i % 8);
+            b
+        });
+        Ok(bool_series("is_valid", bits, self.len(), Some(Bitmap::from_u8_vec(valid, self.len()))))
+    }
+
+    fn is_valid_reason(&self) -> Result<Series> {
+        let (reason, valid) = validity_reasons(self)?;
+        let valid = Bitmap::from_u8_vec(valid, self.len());
+        let v: Vec<Option<&str>> = reason.iter().enumerate().map(|(i, &c)| valid.get_bit(i).then(|| validity_message(c))).collect();
+        Ok(Utf8Chunked::from_iter_options("is_valid_reason", v.into_iter()).into_series())
     }
 
     fn overlay_area_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)> {

@@ -170,6 +170,7 @@ SIGNATURES = {
     "gpl_pairs_copy_distance": (_INT, [_P, _P, _P, _INT]),
     "gpl_intersection_area": (_INT, [_P, _P, _P, _P, _P, _INT]),
     "gpl_overlay_area_join": (_INT, [_P, _P, _P, C.POINTER(_P)]),
+    "gpl_is_valid": (_INT, [_P, _P, _P, _P, _INT]),
     "gpl_haversine_distance": (_INT, [_P, _P, _P, _P, _P, _INT]),
     "gpl_geo_index_build": (_INT, [_P, _P, C.POINTER(_P)]),
     "gpl_geo_index_free": (None, [_P]),

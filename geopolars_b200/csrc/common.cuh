@@ -418,6 +418,10 @@ __device__ __forceinline__ bool point_in_rect(double2 v, double2 b1, double2 b2)
     return value_in_between(v.x, b1.x, b2.x) && value_in_between(v.y, b1.y, b2.y);
 }
 
+// lane src's value, to every lane
+__device__ __forceinline__ double2 bcast2(double2 v, int src) {
+    return make_double2(__shfl_sync(0xffffffffu, v.x, src), __shfl_sync(0xffffffffu, v.y, src));
+}
 // warp reductions on doubles
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll

@@ -521,6 +521,30 @@ def is_ring(a: DeviceArray) -> np.ndarray:
     return _bits(bm, n)
 
 
+def is_valid(a: DeviceArray) -> Tuple[np.ndarray, np.ndarray]:
+    """OGC validity of every row (DESIGN.md §4.18): (reason int8, valid bool); reason 0 is valid, else GEOS's
+    TopologyValidationError number of the first failing rule (VALIDITY_REASONS); valid is False for a null row"""
+    n = len(a)
+    reason = np.zeros(n, dtype=np.int8)
+    bm = np.zeros((n + 7) // 8, dtype=np.uint8)
+    check(a.ctx.lib.gpl_is_valid(a.ctx._h, a._h, _np_ptr(reason), _np_ptr(bm), GPL_HOST))
+    return reason, _bits(bm, n)
+
+
+# gpl_is_valid's reason codes -> GEOS's messages (without the location suffix)
+VALIDITY_REASONS = {
+    0: "Valid Geometry",
+    2: "Hole lies outside shell",
+    3: "Holes are nested",
+    4: "Interior is disconnected",
+    5: "Self-intersection",
+    6: "Ring Self-intersection",
+    7: "Nested shells",
+    9: "Too few distinct points in geometry component",
+    10: "Invalid Coordinate",
+}
+
+
 def x(a: DeviceArray) -> np.ndarray:
     out = np.empty(len(a), dtype=np.float64)
     check(a.ctx.lib.gpl_x(a.ctx._h, a._h, _np_ptr(out), GPL_HOST))

@@ -261,6 +261,18 @@ class GeoRustSeries:
         pa = _pa()
         return pa.array(E.is_ring(d), mask=None if v is None else ~v)
 
+    def is_valid(self):
+        """OGC validity of every row (GeoPandas' `is_valid`, DESIGN.md §4.18), as exact decisions on the GPU; null rows give
+        null.  Filter with it before `intersection_area`, `overlay_area_join` or Polygon `contains`, which need valid input"""
+        reason, valid = E.is_valid(self._d())
+        return _pa().array(reason == 0, mask=~valid)
+
+    def is_valid_reason(self):
+        """why each row is invalid (shapely's `explain_validity` without the location): "Valid Geometry" or GEOS's message
+        of the first failing rule, e.g. "Self-intersection"; null rows give null"""
+        reason, valid = E.is_valid(self._d())
+        return _pa().array([E.VALIDITY_REASONS[int(c)] for c in reason], type=_pa().string(), mask=~valid)
+
     def rotate(self, angle: float, origin: TransformOrigin = "center") -> GeoSeries:
         return self._wrap(E.rotate(self._d(), angle, origin))
 
@@ -293,7 +305,7 @@ class GeoRustSeries:
         """row-wise area of the intersection of self[i] and other[i], both (Multi)Polygon columns (GeoPandas'
         `a.intersection(b).area`; only the area is computed, DESIGN.md §4.16).  Null when either row is null or has a
         non-finite coordinate; 0 for an empty geometry; never negative.  Rings may have any orientation and need not be
-        closed.  The operands must be valid (OGC): on invalid input the value is finite but not specified."""
+        closed.  The operands must be valid (OGC): on invalid input the value is finite but not specified; `is_valid()` tells."""
         out, valid = E.intersection_area(self._d(), other.device)
         return _f64(out, valid)
 
@@ -312,7 +324,8 @@ class GeoRustSeries:
 
     # -- additions: binary predicates (planned-only in the reference docs, geoseries.rst:47-64) ----------
     def contains(self, other: GeoSeries):
-        """row-wise: self[i] ((Multi)Polygon or (Multi)LineString) contains other[i] (Point), or (Multi)Polygon contains Polygon"""
+        """row-wise: self[i] ((Multi)Polygon or (Multi)LineString) contains other[i] (Point), or (Multi)Polygon contains Polygon
+        (defined for valid polygons: check with `is_valid()`)"""
         return _pa().array(E.contains(self._d(), other.device))
 
     def intersects(self, other: GeoSeries):
@@ -425,7 +438,7 @@ def overlay_area_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner"):
     area is bit for bit what `lhs.geo.intersection_area` computes for the pair.  Pairs that only touch are kept with area 0,
     so the areas of a row over a partition sum to the row's area; keep `area > 0` to drop them.  how='inner' -> matched left
     rows only; how='left' -> unmatched left rows once, with rhs_index -1 and area NaN.  The operands must be valid (OGC); on
-    invalid input the areas are finite but not specified (DESIGN.md §4.16)."""
+    invalid input the areas are finite but not specified (DESIGN.md §4.16); filter with `is_valid()` first."""
     if how not in ("inner", "left"):
         raise ValueError("how must be 'inner' or 'left'")
     a, b, d = E.overlay_area_join(lhs.device, rhs.device)

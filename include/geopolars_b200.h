@@ -395,6 +395,26 @@ int gpl_intersection_area(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, 
  * GPL_ERR_UNSUPPORTED); any other type: GPL_ERR_INVALID_TYPE. */
 int gpl_overlay_area_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **out);
 
+/* ---------------------------------------------------------------- validity ---------------- */
+/* OGC validity of every row, any geometry type, DESIGN.md §4.18: reason[n] (int8, in `mem`) is the first failing rule in the
+ * order below, numbered as GEOS's TopologyValidationError except that 0 means valid:
+ *   10 Invalid Coordinate: a NaN or infinite coordinate (a Point row that is exactly (NaN, NaN) is the empty point: valid);
+ *    9 Too few distinct points in geometry component: a non-empty (Multi)LineString member with fewer than 2 distinct
+ *      coordinates, or a non-empty ring with fewer than 3 distinct consecutive vertices;
+ *    5 Self-intersection: two edges of the row's rings cross properly or overlap over a positive length (spikes, zero-area
+ *      rings, shared edges of rings or members included);
+ *    6 Ring Self-intersection: two non-adjacent edges of one ring touch at a point;
+ *    2 Hole lies outside shell (also a non-empty hole of a polygon whose exterior ring is empty);
+ *    3 Holes are nested;
+ *    7 Nested shells: a MultiPolygon member lies in the interior of another (inside its hole is fine);
+ *    4 Interior is disconnected: the rings of one polygon and their touch points form a cycle.
+ * Points and MultiPoints fail only 10, (Multi)LineStrings only 10 and 9.  Rings are closed implicitly, consecutive repeated
+ * coordinates are ignored ("adjacent" is among the non-degenerate edges, across the closing vertex too), orientation is
+ * ignored; an empty geometry, a polygon without rings and a ring without coordinates are valid.  Every decision is an exact
+ * sign of input coordinates, and a row's code depends on that row only.  A null row gets validity 0 in out_validity (Arrow
+ * bitmap in `mem`, may be NULL) and reason 0.  NULL ctx, in or reason: GPL_ERR_INVALID_ARG before any launch. */
+int gpl_is_valid(gpl_ctx *ctx, const gpl_array *in, int8_t *reason, uint8_t *out_validity, int mem);
+
 /* ---------------------------------------------------------------- great-circle joins ----- */
 /* Great-circle distance in metres of two POINT columns read as (lon, lat) degrees: geo 0.27 HaversineDistance on the mean
  * sphere (6 371 008.8 m), the expression gpl_geodesic_length(method 1) sums over segments, bit for bit.  Row-wise 1:1;

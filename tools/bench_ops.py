@@ -4,7 +4,7 @@ fraction for the coordinate bytes read, and of the nearest join (100 M points ag
 reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic|valid] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
@@ -41,7 +41,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic"), default="all",
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid"), default="all",
                     help="run only the §8 rows, only the point nearest join, only the geometry nearest join, only the "
                          "distance-within join, only the great-circle joins, only the intersection area and overlay join or "
                          "only the geodesic area and perimeter (1 M stars, 10 M parcels, naturalearth_lowres to 1 M rows); "
@@ -85,7 +85,9 @@ def main():
             overlay_rows(args, ctx, dev, st, res)
         if args.only in ("all", "geodesic"):
             geodesic_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic"):
+        if args.only in ("all", "valid"):
+            valid_rows(args, ctx, dev, st, res)
+        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -557,6 +559,65 @@ def geodesic_rows(args, ctx, dev, st, res):
     po = np.concatenate([(h_part if h.type == GeometryType.MULTIPOLYGON else h.geom_off)[:-1] + k * nr for k in range(reps)] + [[reps * nr]]).astype(np.int64)
     go = np.concatenate([h_geom[:-1] + k * npart for k in range(reps)] + [[reps * npart]]).astype(np.int64)
     measure("geodesic_area (naturalearth_lowres x %d, %d rows)" % (reps, len(go) - 1), GeometryType.MULTIPOLYGON, xy, ro, go, po)
+
+
+def valid_rows(args, ctx, dev, st, res):
+    """OGC validity (DESIGN.md §4.18), kernel resident, reason codes to device memory: 1 M config-2 stars (65 coordinates),
+    10 M closed 5-coordinate parcels, naturalearth_lowres repeated to about 1 M rows, one 10^6-vertex regular polygon and one
+    square with 10 000 square holes.  ms, rows/s and edges/s (an edge is one ring edge of the input; the edge-pair pass tests
+    each against the edges of the candidate chunks its grid cell lists: FP64 orientation bound)."""
+    import numpy as np
+
+    from geopolars_b200 import datasets, synth
+
+    lib = ctx.lib
+
+    def measure(name, type_, xy, ring_off, geom_off, part_off=None):
+        vs = [xy, ring_off, geom_off] + ([part_off] if part_off is not None else [])
+        t = [torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in vs]
+        a = ctx.wrap_device(type_, len(geom_off) - 1, len(xy), t[0].data_ptr(), geom_off_ptr=t[2].data_ptr(), ring_off_ptr=t[1].data_ptr(),
+                            part_off_ptr=t[3].data_ptr() if part_off is not None else None, n_rings=len(ring_off) - 1,
+                            n_parts=len(part_off) - 1 if part_off is not None else 0, keepalive=tuple(t))
+        n = len(geom_off) - 1
+        out = torch.empty(n, dtype=torch.int8, device=dev)
+        tm = timed(st, lambda: E.check(lib.gpl_is_valid(ctx._h, a._h, C.c_void_p(out.data_ptr()), None, E.GPL_DEVICE)), reps=5, warm=2)
+        edges = len(xy) - (len(ring_off) - 1)  # closed rings
+        r = {"op": name, "units": n, "unit": "rows", "ms_min": tm[0], "ms_avg": tm[1], "units_per_s": n / (tm[1] * 1e-3), "edges": edges,
+             "edges_per_s": edges / (tm[1] * 1e-3), "invalid_rows": int((out != 0).sum().item()), "card": res["card"], "power_limit": res["power_limit"]}
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    m = int(1_000_000 * args.scale)
+    xy, ro, go = synth.star_polygons(m, int(np.ceil(np.sqrt(m))))
+    measure("is_valid (%d config-2 stars)" % m, GeometryType.POLYGON, xy, ro, go)
+    del xy
+    n = int(10_000_000 * args.scale)
+    k = int(np.ceil(np.sqrt(n)))
+    ll = np.stack([np.arange(n) % k, np.arange(n) // k], 1).astype(np.float64) * 2.0
+    q = np.empty((n, 5, 2))
+    q[:, 0], q[:, 1], q[:, 2], q[:, 3], q[:, 4] = ll, ll + [1, 0], ll + 1, ll + [0, 1], ll
+    measure("is_valid (%d parcels, 5 coordinates)" % n, GeometryType.POLYGON, q.reshape(-1, 2), np.arange(n + 1, dtype=np.int64) * 5,
+            np.arange(n + 1, dtype=np.int64))
+    del q, ll
+    h = datasets.read_dataset("naturalearth_lowres").geometry.device.to_host()
+    reps = max(1, int(round(1_000_000 * args.scale / len(h.geom_off[:-1]))))
+    h_part = h.part_off if h.type == GeometryType.MULTIPOLYGON else np.arange(len(h.geom_off), dtype=np.int64)
+    h_geom = h.geom_off if h.type == GeometryType.MULTIPOLYGON else np.arange(len(h.geom_off), dtype=np.int64)
+    nc, nr, npart = len(h.xy), len(h.ring_off) - 1, len(h_part) - 1
+    ro = np.concatenate([h.ring_off[:-1] + i * nc for i in range(reps)] + [[reps * nc]]).astype(np.int64)
+    po = np.concatenate([h_part[:-1] + i * nr for i in range(reps)] + [[reps * nr]]).astype(np.int64)
+    go = np.concatenate([h_geom[:-1] + i * npart for i in range(reps)] + [[reps * npart]]).astype(np.int64)
+    measure("is_valid (naturalearth_lowres x %d, %d rows)" % (reps, len(go) - 1), GeometryType.MULTIPOLYGON, np.tile(h.xy, (reps, 1)), ro, go, po)
+    nv = 1_000_000
+    t = 2 * np.pi * np.arange(nv + 1) / nv
+    ring = np.stack([np.cos(t), np.sin(t)], 1) * 1000.0
+    ring[-1] = ring[0]
+    measure("is_valid (one ring of %d vertices)" % nv, GeometryType.POLYGON, ring, np.array([0, nv + 1]), np.array([0, 1]))
+    g = 100
+    holes = [np.array([[0, 0], [301, 0], [301, 301], [0, 301], [0, 0]], float)]
+    holes += [np.array([[x, y], [x, y + 1], [x + 1, y + 1], [x + 1, y], [x, y]], float) for x in range(1, 3 * g, 3) for y in range(1, 3 * g, 3)]
+    measure("is_valid (one polygon with %d holes)" % (g * g), GeometryType.POLYGON, np.concatenate(holes), np.arange(len(holes) + 1) * 5,
+            np.array([0, len(holes)]))
 
 
 def geo_rows(args, ctx, dev, st, res):
