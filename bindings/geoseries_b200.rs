@@ -114,6 +114,8 @@ extern "C" {
     fn gpl_intersection_area(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, out: *mut f64, out_validity: *mut u8, mem: c_int) -> c_int;
     fn gpl_overlay_area_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, out: *mut *mut GplPairs) -> c_int;
     fn gpl_is_valid(ctx: *mut GplCtx, a: *const GplArray, reason: *mut i8, out_validity: *mut u8, mem: c_int) -> c_int;
+    fn gpl_boolean_op(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, op: c_int, out: *mut *mut GplArray) -> c_int;
+    fn gpl_overlay_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, pairs: *mut *mut GplPairs, out: *mut *mut GplArray) -> c_int;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -482,6 +484,17 @@ pub trait GeoSeriesB200Ext {
     fn is_valid(&self) -> Result<Series>;
     /// GEOS's reason message of the first failing validity rule, "Valid Geometry" for a valid row; null rows stay null
     fn is_valid_reason(&self) -> Result<Series>;
+    /// geo's `BooleanOps::intersection` of two (Multi)Polygon columns row by row, as a MultiPolygon column: null or non-finite
+    /// rows give null, an empty result an empty MultiPolygon.  Valid (OGC) operands give valid output; on invalid operands the
+    /// output is well formed but not specified
+    fn intersection(&self, other: &Series) -> Result<Series>;
+    /// geo's `BooleanOps::union`, as `intersection`
+    fn union(&self, other: &Series) -> Result<Series>;
+    /// geo's `BooleanOps::difference` (self - other), as `intersection`
+    fn difference(&self, other: &Series) -> Result<Series>;
+    /// geometry overlay join of two (Multi)Polygon columns (`overlay(how="intersection")`): every pair whose intersection has a
+    /// member, sorted by (lhs, rhs), with that intersection (bit for bit what `intersection` gives for the pair)
+    fn overlay_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Series)>;
 }
 
 impl GeoSeriesB200Ext for Series {
@@ -681,4 +694,46 @@ impl GeoSeriesB200Ext for Series {
         check(rc)?;
         Ok((l, r, d))
     }
+
+    fn intersection(&self, other: &Series) -> Result<Series> {
+        boolean_op(self, other, GPL_BOOLEAN_INTERSECTION)
+    }
+
+    fn union(&self, other: &Series) -> Result<Series> {
+        boolean_op(self, other, GPL_BOOLEAN_UNION)
+    }
+
+    fn difference(&self, other: &Series) -> Result<Series> {
+        boolean_op(self, other, GPL_BOOLEAN_DIFFERENCE)
+    }
+
+    fn overlay_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Series)> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let (mut pairs, mut out) = (std::ptr::null_mut(), std::ptr::null_mut());
+        check(unsafe { gpl_overlay_join(ctx, a.0, b.0, &mut pairs, &mut out) })?;
+        let geoms = Dev(out);
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r) = (vec![0u64; n], vec![0u64; n]);
+        let mut rc = 0;
+        if n > 0 {
+            rc = unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) };
+        }
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
+        Ok((l, r, from_device(ctx, geoms)?))
+    }
+}
+
+const GPL_BOOLEAN_INTERSECTION: c_int = 0;
+const GPL_BOOLEAN_UNION: c_int = 1;
+const GPL_BOOLEAN_DIFFERENCE: c_int = 2;
+
+/// gpl_boolean_op of two (Multi)Polygon columns: a MultiPolygon column
+fn boolean_op(a: &Series, b: &Series, op: c_int) -> Result<Series> {
+    let ctx = ctx()?;
+    let (da, db) = (to_device(ctx, a)?, to_device(ctx, b)?);
+    let mut out = std::ptr::null_mut();
+    check(unsafe { gpl_boolean_op(ctx, da.0, db.0, op, &mut out) })?;
+    from_device(ctx, Dev(out))
 }

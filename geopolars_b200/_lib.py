@@ -171,6 +171,8 @@ SIGNATURES = {
     "gpl_intersection_area": (_INT, [_P, _P, _P, _P, _P, _INT]),
     "gpl_overlay_area_join": (_INT, [_P, _P, _P, C.POINTER(_P)]),
     "gpl_is_valid": (_INT, [_P, _P, _P, _P, _INT]),
+    "gpl_boolean_op": (_INT, [_P, _P, _P, _INT, C.POINTER(_P)]),
+    "gpl_overlay_join": (_INT, [_P, _P, _P, C.POINTER(_P), C.POINTER(_P)]),
     "gpl_haversine_distance": (_INT, [_P, _P, _P, _P, _P, _INT]),
     "gpl_geo_index_build": (_INT, [_P, _P, C.POINTER(_P)]),
     "gpl_geo_index_free": (None, [_P]),

@@ -24,6 +24,7 @@
 
 #include "common.cuh"
 #include "join_grid.cuh"
+#include "overlay.cuh"
 #include "pair_dist.cuh"
 
 namespace gpl {
@@ -192,16 +193,6 @@ __device__ double overlap_area(const Side &a, const int8_t *__restrict__ as, con
     return v > 0.0 ? v : 0.0;
 }
 
-// every coordinate of the rings of members [m0, m1) of the POLYGON view s is finite (warp-uniform)
-__device__ __forceinline__ bool members_finite(const Side &s, int64_t m0, int64_t m1, int lane) {
-    bool ok = true;
-    for (int64_t c = s.ro[s.go[m0]] + lane; c < s.ro[s.go[m1]]; c += 32) {
-        const double2 q = s.xy[c];
-        ok = ok && isfinite(q.x) && isfinite(q.y);
-    }
-    return __all_sync(0xffffffffu, ok);
-}
-
 // One warp per row, or per pair of a join (ia / ib select the rows).  am / bm: member offsets of a MultiPolygon column
 // (NULL: one member per row).  A null row or a non-finite coordinate gives NaN and validity 0.
 __global__ void __launch_bounds__(kOverlapThreads, 3) k_overlap_area(int64_t n, Side a, const int64_t *__restrict__ am, const uint8_t *__restrict__ av,
@@ -229,14 +220,8 @@ __global__ void __launch_bounds__(kOverlapThreads, 3) k_overlap_area(int64_t n, 
     }
 }
 
-// per-ring σ and boxes of a (Multi)Polygon column
-struct RingPrep {
-    Side view;
-    const int64_t *members;  // the MultiPolygon's geom_off, NULL for a Polygon column
-    Scratch<int8_t> sigma;
-    Scratch<double4> box;
-};
-static int ring_prep(gpl_ctx *ctx, const gpl_array *g, RingPrep &out) {
+// per-ring σ and boxes of a (Multi)Polygon column (overlay.cuh)
+int ring_prep(gpl_ctx *ctx, const gpl_array *g, RingPrep &out) {
     out.view = polygon_view(g);
     out.members = g->type == GPL_MULTIPOLYGON ? g->geom_off : nullptr;
     const int64_t n_members = g->type == GPL_MULTIPOLYGON ? g->n_parts : g->n_geoms;
@@ -245,8 +230,6 @@ static int ring_prep(gpl_ctx *ctx, const gpl_array *g, RingPrep &out) {
     if (n_members > 0) GPL_LAUNCH(ctx, k_ring_prep, warp_grid(n_members, 8), 256, 0, n_members, out.view, out.sigma.p, out.box.p);
     return GPL_OK;
 }
-
-static bool is_area(int t) { return t == GPL_POLYGON || t == GPL_MULTIPOLYGON; }
 
 }  // namespace gpl
 

@@ -457,6 +457,36 @@ def overlay_area_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, n
     return a[order], b[order], d[order]
 
 
+BOOLEAN_OPS = {"intersection": 0, "union": 1, "difference": 2}
+
+
+def boolean_op(a: DeviceArray, b: DeviceArray, op: str) -> DeviceArray:
+    """row-wise intersection, union or difference (a - b) of two (Multi)Polygon columns as a MultiPolygon column
+    (DESIGN.md §4.19): geo's BooleanOps; a null or non-finite row gives a null row, an empty result an empty MultiPolygon"""
+    code = BOOLEAN_OPS.get(op)
+    if code is None:
+        raise ValueError("op must be 'intersection', 'union' or 'difference'")
+    return _out_array(a.ctx, a.ctx.lib.gpl_boolean_op, a._h, b._h, code)
+
+
+def overlay_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, np.ndarray, DeviceArray]:
+    """(lhs uint64, rhs uint64, MultiPolygon column) for every pair of rows of two (Multi)Polygon columns whose intersection
+    has a member, sorted by (lhs, rhs); row k of the column is bit for bit `boolean_op(lhs[i], rhs[j], "intersection")`"""
+    ctx = lhs.ctx
+    hp, ha = C.c_void_p(), C.c_void_p()
+    check(ctx.lib.gpl_overlay_join(ctx._h, lhs._h, rhs._h, C.byref(hp), C.byref(ha)))
+    geoms = DeviceArray(ctx, ha)
+    try:
+        n = int(ctx.lib.gpl_pairs_count(hp))
+        a = np.empty(n, dtype=np.uint64)
+        b = np.empty(n, dtype=np.uint64)
+        if n:
+            check(ctx.lib.gpl_pairs_copy(ctx._h, hp, _np_ptr(a), _np_ptr(b), GPL_HOST))
+    finally:
+        ctx.lib.gpl_pairs_free(hp)
+    return a, b, geoms
+
+
 def intersects(a: DeviceArray, b: DeviceArray) -> np.ndarray:
     n = len(a)
     bm = np.zeros((n + 7) // 8, dtype=np.uint8)

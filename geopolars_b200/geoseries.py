@@ -309,6 +309,21 @@ class GeoRustSeries:
         out, valid = E.intersection_area(self._d(), other.device)
         return _f64(out, valid)
 
+    def intersection(self, other: GeoSeries) -> GeoSeries:
+        """row-wise intersection of self[i] and other[i], both (Multi)Polygon columns (GeoPandas' `a.intersection(b)`, geo's
+        BooleanOps), as a MultiPolygon column (DESIGN.md §4.19).  Null when either row is null or has a non-finite coordinate;
+        an empty result is an empty MultiPolygon.  Valid (OGC) operands give valid output; on invalid operands the output is
+        well formed but not specified; `is_valid()` tells."""
+        return self._wrap(E.boolean_op(self._d(), other.device, "intersection"))
+
+    def union(self, other: GeoSeries) -> GeoSeries:
+        """row-wise union of self[i] and other[i] (GeoPandas' `a.union(b)`), as `intersection`"""
+        return self._wrap(E.boolean_op(self._d(), other.device, "union"))
+
+    def difference(self, other: GeoSeries) -> GeoSeries:
+        """row-wise difference self[i] - other[i] (GeoPandas' `a.difference(b)`), as `intersection`"""
+        return self._wrap(E.boolean_op(self._d(), other.device, "difference"))
+
     def translate(self, xoff: float = 0.0, yoff: float = 0.0) -> GeoSeries:
         return self._wrap(E.translate(self._d(), xoff, yoff))
 
@@ -449,6 +464,15 @@ def overlay_area_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner"):
         matched[a] = True
         a, b, d = _left_rows(a, b, d, np.nonzero(~matched)[0])
     return a, b, d
+
+
+def overlay_join(lhs: GeoSeries, rhs: GeoSeries):
+    """Geometry overlay join of two (Multi)Polygon columns (GeoPandas' `overlay(a, b, how="intersection")` with
+    keep_geom_type=True): (lhs_index int64, rhs_index int64, GeoSeries of MultiPolygons) for every pair whose intersection has
+    at least one member, sorted by (lhs, rhs); pairs that only touch are dropped.  Geometry k is bit for bit
+    `lhs.geo.intersection` of the pair (DESIGN.md §4.19).  Valid (OGC) operands only; filter with `is_valid()` first."""
+    a, b, g = E.overlay_join(lhs.device, rhs.device)
+    return a.astype(np.int64), b.astype(np.int64), GeoSeries(_device=g, name=lhs.name)
 
 
 def geo_nearest_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", max_distance: Optional[float] = None):

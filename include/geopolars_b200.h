@@ -395,6 +395,28 @@ int gpl_intersection_area(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, 
  * GPL_ERR_UNSUPPORTED); any other type: GPL_ERR_INVALID_TYPE. */
 int gpl_overlay_area_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **out);
 
+/* ---------------------------------------------------------------- boolean geometry ------- */
+enum { GPL_BOOLEAN_INTERSECTION = 0, GPL_BOOLEAN_UNION = 1, GPL_BOOLEAN_DIFFERENCE = 2 };
+/* Intersection, union or difference (a - b) of the closed regions a[i] and b[i] (geo's BooleanOps::{intersection, union,
+ * difference}), DESIGN.md §4.19: the regularised result (lower-dimensional contact is dropped) as a MultiPolygon column, always.
+ * Both columns Polygon or MultiPolygon, in any combination (else GPL_ERR_INVALID_TYPE); unequal lengths: GPL_ERR_LENGTH_MISMATCH;
+ * any other op: GPL_ERR_INVALID_ARG; all before any launch.  Input rings are read as gpl_intersection_area reads them (any
+ * orientation, closed implicitly, fewer than 4 coordinates after closing: no contribution).  A null row or a row with a
+ * non-finite coordinate gives a null row; an empty result is an empty MultiPolygon.  Output: rings closed, shells
+ * counter-clockwise and holes clockwise, each ring starting at its lexicographically smallest vertex, holes ordered by their first
+ * vertex, members by their shell's first vertex; every cut point is a vertex; consecutive equal coordinates are merged and a
+ * ring left with fewer than 3 distinct vertices is dropped (a shell with its holes).  Every combinatorial decision is an exact
+ * sign except the assignment of holes to shells; only crossing points are rounded.  For valid (OGC) operands the output is valid;
+ * on invalid operands it is a well-formed MultiPolygon column of bounded size whose geometry is not specified.  A row's output
+ * depends on that row only, bit for bit. */
+int gpl_boolean_op(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, int op, gpl_array **out);
+/* Geometry overlay join of two (Multi)Polygon columns (GeoPandas' overlay(how="intersection"), keep_geom_type=True): every pair
+ * (i, j) whose intersection has at least one member, sorted by (lhs, rhs), as a device-resident gpl_pairs; row k of *out (a
+ * MultiPolygon column) is the intersection of pair k, bit for bit what gpl_boolean_op(lhs[i], rhs[j], GPL_BOOLEAN_INTERSECTION)
+ * returns.  Candidates are the pairs gpl_intersects accepts; touching pairs are dropped.  Fewer than 2^31 rows per side (else
+ * GPL_ERR_UNSUPPORTED); any other type: GPL_ERR_INVALID_TYPE. */
+int gpl_overlay_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **pairs, gpl_array **out);
+
 /* ---------------------------------------------------------------- validity ---------------- */
 /* OGC validity of every row, any geometry type, DESIGN.md §4.18: reason[n] (int8, in `mem`) is the first failing rule in the
  * order below, numbered as GEOS's TopologyValidationError except that 0 means valid:

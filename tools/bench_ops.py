@@ -4,7 +4,7 @@ fraction for the coordinate bytes read, and of the nearest join (100 M points ag
 reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic|valid] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic|valid|boolean] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
@@ -41,10 +41,11 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid"), default="all",
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean"), default="all",
                     help="run only the §8 rows, only the point nearest join, only the geometry nearest join, only the "
                          "distance-within join, only the great-circle joins, only the intersection area and overlay join or "
-                         "only the geodesic area and perimeter (1 M stars, 10 M parcels, naturalearth_lowres to 1 M rows); "
+                         "only the geodesic area and perimeter (1 M stars, 10 M parcels, naturalearth_lowres to 1 M rows), or only "
+                         "the boolean geometry ops and the geometry overlay join; "
                          "'all' runs every arm")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
@@ -83,11 +84,13 @@ def main():
             geo_rows(args, ctx, dev, st, res)
         if args.only in ("all", "overlay"):
             overlay_rows(args, ctx, dev, st, res)
+        if args.only in ("all", "boolean"):
+            boolean_rows(args, ctx, dev, st, res)
         if args.only in ("all", "geodesic"):
             geodesic_rows(args, ctx, dev, st, res)
         if args.only in ("all", "valid"):
             valid_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid"):
+        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -462,6 +465,66 @@ def overlay_rows(args, ctx, dev, st, res):
 
     t = timed(st, join, reps=3, warm=1)
     rec("overlay_area_join (10 000 stars x %d squares)" % (k * k), n_pairs[0], "pairs", n_pairs[0] * 64 * 4, t)
+
+
+def boolean_rows(args, ctx, dev, st, res):
+    """intersection, union and difference geometry (DESIGN.md §4.19) on the workload of overlay_rows: row-wise on 1 M pairs
+    of config 2's stars against the same stars shifted by (3, 2), and the geometry overlay join of config 2's 10 000 stars
+    against a 1000 x 1000 grid of unit squares; output MultiPolygon columns built on the device, host synchronisations of
+    the count / scan / write passes included"""
+    import numpy as np
+
+    from geopolars_b200 import synth
+
+    lib = ctx.lib
+
+    def rec(name, units, unit_name, t, extra):
+        r = {"op": name, "units": units, "unit": unit_name, "ms_min": t[0], "ms_avg": t[1], "units_per_s": units / (t[1] * 1e-3),
+             "card": res["card"], "power_limit": res["power_limit"], **extra}
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    def upload(xy, ring_off, geom_off):
+        t = [torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in (xy, ring_off, geom_off)]
+        n = len(geom_off) - 1
+        return ctx.wrap_device(GeometryType.POLYGON, n, len(xy), t[0].data_ptr(), geom_off_ptr=t[2].data_ptr(), ring_off_ptr=t[1].data_ptr(),
+                               n_rings=len(ring_off) - 1, keepalive=tuple(t))
+
+    n = int(1_000_000 * args.scale)
+    g = int(np.ceil(np.sqrt(n)))
+    xy, ro, go = synth.star_polygons(m=n, grid=g)
+    a, b = upload(xy, ro, go), upload(xy + np.array([3.0, 2.0]), ro, go)
+    for name, code in (("intersection", 0), ("union", 1), ("difference", 2)):
+        size = [0]
+
+        def run():
+            h = C.c_void_p()
+            E.check(lib.gpl_boolean_op(ctx._h, a._h, b._h, code, C.byref(h)))
+            size[0] = int(E.DeviceArray(ctx, h).view().n_coords)
+
+        t = timed(st, run, reps=3, warm=1)
+        rec("boolean_op %s (%d star pairs, 64 x 64 edges)" % (name, n), n, "row pairs", t, {"out_coords": size[0]})
+    del a, b
+
+    sxy, sro, sgo = synth.star_polygons()
+    stars = upload(sxy, sro, sgo)
+    k = int(1000 * np.sqrt(args.scale))
+    i, j = np.meshgrid(np.arange(k, dtype=np.float64), np.arange(k, dtype=np.float64), indexing="xy")
+    x0, y0 = i.ravel() * (1000.0 / k), j.ravel() * (1000.0 / k)
+    w = 1000.0 / k
+    gxy = np.stack([np.stack([x0, x0 + w, x0 + w, x0, x0], 1), np.stack([y0, y0, y0 + w, y0 + w, y0], 1)], 2).reshape(-1, 2)
+    cells = upload(gxy, np.arange(k * k + 1, dtype=np.int64) * 5, np.arange(k * k + 1, dtype=np.int64))
+    n_pairs = [0]
+
+    def join():
+        hp, ha = C.c_void_p(), C.c_void_p()
+        E.check(lib.gpl_overlay_join(ctx._h, stars._h, cells._h, C.byref(hp), C.byref(ha)))
+        n_pairs[0] = int(lib.gpl_pairs_count(hp))
+        lib.gpl_pairs_free(hp)
+        E.DeviceArray(ctx, ha)
+
+    t = timed(st, join, reps=3, warm=1)
+    rec("overlay_join (10 000 stars x %d squares)" % (k * k), n_pairs[0], "pairs", t, {})
 
 
 def geodesic_rows(args, ctx, dev, st, res):
