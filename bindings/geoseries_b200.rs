@@ -58,6 +58,16 @@ const GPL_ORIGIN_CENTER: c_int = 1;
 const GPL_ORIGIN_POINT: c_int = 2;
 pub const GPL_PREDICATE_INTERSECTS: c_int = 0;
 pub const GPL_PREDICATE_CONTAINS: c_int = 1;
+pub const GPL_PREDICATE_WITHIN: c_int = 2;
+pub const GPL_PREDICATE_CONTAINS_PROPERLY: c_int = 3;
+pub const GPL_PREDICATE_COVERS: c_int = 4;
+pub const GPL_PREDICATE_COVERED_BY: c_int = 5;
+pub const GPL_PREDICATE_TOUCHES: c_int = 6;
+pub const GPL_PREDICATE_CROSSES: c_int = 7;
+pub const GPL_PREDICATE_OVERLAPS: c_int = 8;
+pub const GPL_PREDICATE_DISJOINT: c_int = 9;
+pub const GPL_PREDICATE_EQUALS: c_int = 10;
+pub const GPL_PREDICATE_PATTERN: c_int = 11;
 
 #[link(name = "geopolars_b200")]
 extern "C" {
@@ -116,6 +126,9 @@ extern "C" {
     fn gpl_is_valid(ctx: *mut GplCtx, a: *const GplArray, reason: *mut i8, out_validity: *mut u8, mem: c_int) -> c_int;
     fn gpl_boolean_op(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, op: c_int, out: *mut *mut GplArray) -> c_int;
     fn gpl_overlay_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, pairs: *mut *mut GplPairs, out: *mut *mut GplArray) -> c_int;
+    fn gpl_relate(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, matrix: *mut i8, out_validity: *mut u8, mem: c_int) -> c_int;
+    fn gpl_relate_predicate(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, predicate: c_int, pattern: *const c_char, out_bitmap: *mut u8, mem: c_int) -> c_int;
+    fn gpl_predicate_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, predicate: c_int, pattern: *const c_char, out: *mut *mut GplPairs) -> c_int;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -495,6 +508,32 @@ pub trait GeoSeriesB200Ext {
     /// geometry overlay join of two (Multi)Polygon columns (`overlay(how="intersection")`): every pair whose intersection has a
     /// member, sorted by (lhs, rhs), with that intersection (bit for bit what `intersection` gives for the pair)
     fn overlay_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Series)>;
+    /// the DE-9IM matrix of every row pair as a string such as "FF2F11212" (rows: self's Interior, Boundary, Exterior); null
+    /// for a null or non-finite row.  Any two of the six types; defined for valid (OGC) operands
+    fn relate(&self, other: &Series) -> Result<Series>;
+    /// the matrix matches `pattern` (9 characters over TF*012, either case); a null row gives false
+    fn relate_pattern(&self, other: &Series, pattern: &str) -> Result<Series>;
+    /// DE-9IM T*F**F***
+    fn within(&self, other: &Series) -> Result<Series>;
+    /// DE-9IM T*****FF*, *T****FF*, ***T**FF* or ****T*FF*
+    fn covers(&self, other: &Series) -> Result<Series>;
+    /// DE-9IM T*F**F***, *TF**F***, **FT*F*** or **F*TF***
+    fn covered_by(&self, other: &Series) -> Result<Series>;
+    /// DE-9IM FT*******, F**T***** or F***T****; false for two (Multi)Point columns
+    fn touches(&self, other: &Series) -> Result<Series>;
+    /// JTS's crosses by dimension
+    fn crosses(&self, other: &Series) -> Result<Series>;
+    /// JTS's overlaps by dimension
+    fn overlaps(&self, other: &Series) -> Result<Series>;
+    /// DE-9IM FF*FF****
+    fn disjoint(&self, other: &Series) -> Result<Series>;
+    /// topological equality: same dimension and T*F**FFF*; two empty rows are equal
+    fn geom_equals(&self, other: &Series) -> Result<Series>;
+    /// DE-9IM T**FF*FF*
+    fn contains_properly(&self, other: &Series) -> Result<Series>;
+    /// GeoPandas' sjoin(predicate=...): every pair for which the predicate (a GPL_PREDICATE_* code other than DISJOINT;
+    /// `pattern` for GPL_PREDICATE_PATTERN) holds, sorted by (lhs, rhs)
+    fn predicate_join_pairs(&self, rhs: &Series, predicate: c_int, pattern: Option<&str>) -> Result<(Vec<u64>, Vec<u64>)>;
 }
 
 impl GeoSeriesB200Ext for Series {
@@ -723,6 +762,89 @@ impl GeoSeriesB200Ext for Series {
         check(rc)?;
         Ok((l, r, from_device(ctx, geoms)?))
     }
+
+    fn relate(&self, other: &Series) -> Result<Series> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, other)?);
+        let n = self.len();
+        let mut m = vec![0i8; 9 * n];
+        let mut valid = vec![0u8; (n + 7) / 8];
+        check(unsafe { gpl_relate(ctx, a.0, b.0, m.as_mut_ptr(), valid.as_mut_ptr(), GPL_HOST) })?;
+        let valid = Bitmap::from_u8_vec(valid, n);
+        let v: Vec<Option<String>> = (0..n)
+            .map(|i| valid.get_bit(i).then(|| m[9 * i..9 * i + 9].iter().map(|&e| if e < 0 { 'F' } else { (b'0' + e as u8) as char }).collect()))
+            .collect();
+        Ok(Utf8Chunked::from_iter_options("relate", v.into_iter()).into_series())
+    }
+
+    fn relate_pattern(&self, other: &Series, pattern: &str) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_PATTERN, Some(pattern), "relate_pattern")
+    }
+
+    fn within(&self, other: &Series) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_WITHIN, None, "within")
+    }
+
+    fn covers(&self, other: &Series) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_COVERS, None, "covers")
+    }
+
+    fn covered_by(&self, other: &Series) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_COVERED_BY, None, "covered_by")
+    }
+
+    fn touches(&self, other: &Series) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_TOUCHES, None, "touches")
+    }
+
+    fn crosses(&self, other: &Series) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_CROSSES, None, "crosses")
+    }
+
+    fn overlaps(&self, other: &Series) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_OVERLAPS, None, "overlaps")
+    }
+
+    fn disjoint(&self, other: &Series) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_DISJOINT, None, "disjoint")
+    }
+
+    fn geom_equals(&self, other: &Series) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_EQUALS, None, "geom_equals")
+    }
+
+    fn contains_properly(&self, other: &Series) -> Result<Series> {
+        relate_predicate(self, other, GPL_PREDICATE_CONTAINS_PROPERLY, None, "contains_properly")
+    }
+
+    fn predicate_join_pairs(&self, rhs: &Series, predicate: c_int, pattern: Option<&str>) -> Result<(Vec<u64>, Vec<u64>)> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let pat = c_pattern(pattern);
+        let mut pairs = std::ptr::null_mut();
+        check(unsafe { gpl_predicate_join(ctx, a.0, b.0, predicate, pat.as_ptr(), &mut pairs) })?;
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r) = (vec![0u64; n], vec![0u64; n]);
+        let rc = if n > 0 { unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) } } else { 0 };
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
+        Ok((l, r))
+    }
+}
+
+/// a 9-character DE-9IM pattern as a C string (an interior NUL is left to the library's length check)
+fn c_pattern(pattern: Option<&str>) -> std::ffi::CString {
+    std::ffi::CString::new(pattern.unwrap_or("").replace('\0', "?")).unwrap_or_default()
+}
+
+/// gpl_relate_predicate of two columns: a Boolean column (null rows give false)
+fn relate_predicate(a: &Series, b: &Series, predicate: c_int, pattern: Option<&str>, name: &str) -> Result<Series> {
+    let ctx = ctx()?;
+    let (da, db) = (to_device(ctx, a)?, to_device(ctx, b)?);
+    let pat = c_pattern(pattern);
+    let mut bits = vec![0u8; (a.len() + 7) / 8];
+    check(unsafe { gpl_relate_predicate(ctx, da.0, db.0, predicate, pat.as_ptr(), bits.as_mut_ptr(), GPL_HOST) })?;
+    Ok(bool_series(name, bits, a.len(), None))
 }
 
 const GPL_BOOLEAN_INTERSECTION: c_int = 0;

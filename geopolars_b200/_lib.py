@@ -139,6 +139,9 @@ SIGNATURES = {
     "gpl_explode": (_INT, [_P, _P, C.POINTER(_P)]),
     "gpl_contains_polygon": (_INT, [_P, _P, _P, _P, _INT]),
     "gpl_spatial_join": (_INT, [_P, _P, _P, _INT, C.POINTER(_P)]),
+    "gpl_relate": (_INT, [_P, _P, _P, _P, _P, _INT]),
+    "gpl_relate_predicate": (_INT, [_P, _P, _P, _INT, C.c_char_p, _P, _INT]),
+    "gpl_predicate_join": (_INT, [_P, _P, _P, _INT, C.c_char_p, C.POINTER(_P)]),
     "gpl_pairs_count": (_I64, [_P]),
     "gpl_pairs_copy": (_INT, [_P, _P, _P, _P, _INT]),
     "gpl_pairs_free": (None, [_P]),

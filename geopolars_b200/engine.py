@@ -531,6 +531,65 @@ def spatial_join(lhs: DeviceArray, rhs: DeviceArray, predicate: str = "intersect
     return _pairs_to_host(lhs.ctx, h)
 
 
+def relate(a: DeviceArray, b: DeviceArray) -> Tuple[np.ndarray, np.ndarray]:
+    """row-wise DE-9IM matrix of a[i] and b[i], any two of the six types (DESIGN.md §4.20): (int8 [n, 9] row-major, -1 = F,
+    valid bool); a null row or a non-finite coordinate gives an invalid row.  Defined for valid (OGC) operands."""
+    n = len(a)
+    out = np.empty((n, 9), dtype=np.int8)
+    bm = np.zeros((n + 7) // 8, dtype=np.uint8)
+    check(a.ctx.lib.gpl_relate(a.ctx._h, a._h, b._h, _np_ptr(out), _np_ptr(bm), GPL_HOST))
+    return out, _bits(bm, n)
+
+
+# gpl_relate_predicate / gpl_predicate_join codes (include/geopolars_b200.h)
+RELATE_PREDICATES = {
+    "intersects": 0, "contains": 1, "within": 2, "contains_properly": 3, "covers": 4, "covered_by": 5, "touches": 6,
+    "crosses": 7, "overlaps": 8, "disjoint": 9, "geom_equals": 10, "relate_pattern": 11,
+}
+
+
+def _predicate(predicate: str, pattern: Optional[str]) -> Tuple[int, Optional[bytes]]:
+    code = RELATE_PREDICATES.get(predicate)
+    if code is None:
+        raise ValueError(f"unknown predicate {predicate!r}: expected one of {', '.join(RELATE_PREDICATES)}")
+    if code != RELATE_PREDICATES["relate_pattern"]:
+        return code, None
+    if not isinstance(pattern, str) or len(pattern) != 9 or any(c not in "TF*012" for c in pattern.upper()):
+        raise ValueError(f"a DE-9IM pattern is 9 characters of T, F, *, 0, 1 and 2 (got {pattern!r})")
+    return code, pattern.encode("ascii")
+
+
+def relate_predicate(a: DeviceArray, b: DeviceArray, predicate: str, pattern: Optional[str] = None) -> np.ndarray:
+    """row-wise named DE-9IM predicate (RELATE_PREDICATES; 'relate_pattern' with a 9-character pattern over TF*012); a null
+    or non-finite row gives False"""
+    code, pat = _predicate(predicate, pattern)
+    n = len(a)
+    bm = np.zeros((n + 7) // 8, dtype=np.uint8)
+    check(a.ctx.lib.gpl_relate_predicate(a.ctx._h, a._h, b._h, code, pat, _np_ptr(bm), GPL_HOST))
+    return _bits(bm, n)
+
+
+def predicate_join(lhs: DeviceArray, rhs: DeviceArray, predicate: str = "intersects", pattern: Optional[str] = None):
+    """(lhs uint64, rhs uint64) of every pair for which relate_predicate(lhs[i], rhs[j]) holds, sorted by (lhs, rhs).  A
+    predicate that can hold for disjoint pairs ('disjoint', or a pattern with II, IB, BI and BB all F or *) raises ValueError."""
+    code, pat = _predicate(predicate, pattern)
+    if code == RELATE_PREDICATES["disjoint"]:
+        raise ValueError("predicate_join cannot use 'disjoint': it matches pairs that share no envelope")
+    if pat is not None and all(c in "F*" for c in (pat.decode().upper()[i] for i in (0, 1, 3, 4))):
+        raise ValueError("predicate_join needs a pattern that requires contact (II, IB, BI or BB not F or *)")
+    h = C.c_void_p()
+    check(lhs.ctx.lib.gpl_predicate_join(lhs.ctx._h, lhs._h, rhs._h, code, pat, C.byref(h)))
+    try:
+        n = int(lhs.ctx.lib.gpl_pairs_count(h))
+        a = np.empty(n, dtype=np.uint64)
+        b = np.empty(n, dtype=np.uint64)
+        if n:
+            check(lhs.ctx.lib.gpl_pairs_copy(lhs.ctx._h, h, _np_ptr(a), _np_ptr(b), GPL_HOST))
+    finally:
+        lhs.ctx.lib.gpl_pairs_free(h)
+    return a, b
+
+
 def geom_type(a: DeviceArray) -> np.ndarray:
     out = np.empty(len(a), dtype=np.int8)
     check(a.ctx.lib.gpl_geom_type(a.ctx._h, a._h, _np_ptr(out), GPL_HOST))

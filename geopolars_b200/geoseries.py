@@ -347,6 +347,57 @@ class GeoRustSeries:
         """row-wise geo `Intersects` for every pair of (Multi)Point / (Multi)LineString / (Multi)Polygon columns"""
         return _pa().array(E.intersects(self._d(), other.device))
 
+    # -- DE-9IM (DESIGN.md §4.20): any two of the six types; defined for valid (OGC) operands, a null row gives False --
+    def relate(self, other: GeoSeries):
+        """row-wise DE-9IM matrix of self[i] and other[i] as a string such as "FF2F11212" (rows: self's Interior, Boundary,
+        Exterior; columns: other's); null when either row is null or has a non-finite coordinate"""
+        m, valid = E.relate(self._d(), other.device)
+        chars = np.array(list("F012"))[m.astype(np.int64) + 1]
+        return _pa().array(["".join(r) if v else None for r, v in zip(chars, valid)], type=_pa().string())
+
+    def relate_pattern(self, other: GeoSeries, pattern: str):
+        """row-wise: the DE-9IM matrix matches `pattern`, 9 characters over T, F, *, 0, 1, 2 (either case; else ValueError)"""
+        return _pa().array(E.relate_predicate(self._d(), other.device, "relate_pattern", pattern))
+
+    def _pred(self, other: GeoSeries, name: str):
+        return _pa().array(E.relate_predicate(self._d(), other.device, name))
+
+    def within(self, other: GeoSeries):
+        """row-wise DE-9IM within: T*F**F***"""
+        return self._pred(other, "within")
+
+    def covers(self, other: GeoSeries):
+        """row-wise DE-9IM covers: T*****FF*, *T****FF*, ***T**FF* or ****T*FF*"""
+        return self._pred(other, "covers")
+
+    def covered_by(self, other: GeoSeries):
+        """row-wise DE-9IM covered_by: T*F**F***, *TF**F***, **FT*F*** or **F*TF***"""
+        return self._pred(other, "covered_by")
+
+    def touches(self, other: GeoSeries):
+        """row-wise DE-9IM touches: FT*******, F**T***** or F***T****; False for two (Multi)Point rows"""
+        return self._pred(other, "touches")
+
+    def crosses(self, other: GeoSeries):
+        """row-wise DE-9IM crosses: T*T****** (lower dimension first), T*****T** (higher first), 0******** (two lines)"""
+        return self._pred(other, "crosses")
+
+    def overlaps(self, other: GeoSeries):
+        """row-wise DE-9IM overlaps: T*T***T** (two point or two polygon columns), 1*T***T** (two line columns)"""
+        return self._pred(other, "overlaps")
+
+    def disjoint(self, other: GeoSeries):
+        """row-wise DE-9IM disjoint: FF*FF****"""
+        return self._pred(other, "disjoint")
+
+    def geom_equals(self, other: GeoSeries):
+        """row-wise topological equality: same dimension and T*F**FFF*; two empty rows are equal"""
+        return self._pred(other, "geom_equals")
+
+    def contains_properly(self, other: GeoSeries):
+        """row-wise DE-9IM contains_properly: T**FF*FF*"""
+        return self._pred(other, "contains_properly")
+
 
 def spatial_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", predicate: str = "intersects"):
     """spatial_join(lhs, rhs, SpatialJoinArgs{join_type, predicate}) (geopolars/src/spatial_index.rs:37-204): the
@@ -368,6 +419,38 @@ def spatial_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", predicate: 
     if how == "left":
         n = len(lhs)
         matched = np.zeros(n, dtype=bool)
+        matched[a] = True
+        miss = np.nonzero(~matched)[0]
+        a = np.concatenate([a, miss])
+        b = np.concatenate([b, np.full(len(miss), -1, dtype=np.int64)])
+        order = np.lexsort((b, a))
+        a, b = a[order], b[order]
+    return a, b
+
+
+def predicate_join(lhs: GeoSeries, rhs: GeoSeries, predicate: str = "intersects", how: str = "inner", pattern: Optional[str] = None):
+    """Predicate join of any two geometry columns (GeoPandas' sjoin(predicate=...)): (lhs_index int64, rhs_index int64) for
+    every pair for which `lhs.geo.<predicate>(rhs)` holds row-wise, sorted by (lhs, rhs).  predicate: intersects, contains,
+    within, contains_properly, covers, covered_by, touches, crosses, overlaps, geom_equals, or relate_pattern with `pattern`;
+    disjoint (and a pattern that matches disjoint pairs) raises ValueError.  how='inner' -> matching pairs; how='left' -> each
+    unmatched lhs row once more, with rhs_index -1.  Points within (Multi)Polygons, and (Multi)Polygons containing points, run
+    on the points-in-polygons index; everything else on the DE-9IM kernel over envelope candidates (DESIGN.md §4.20)."""
+    if how not in ("inner", "left"):
+        raise ValueError("how must be 'inner' or 'left'")
+    lt, rt = lhs.device.type, rhs.device.type
+    areas = (GeometryType.POLYGON, GeometryType.MULTIPOLYGON)
+    if predicate == "within" and lt == GeometryType.POINT and rt in areas:
+        a, b = E.PipIndex(rhs.device).pairs_array(lhs.device)
+    elif predicate == "contains" and rt == GeometryType.POINT and lt in areas:
+        p, q = E.PipIndex(lhs.device).pairs_array(rhs.device)
+        order = np.lexsort((p, q))
+        a, b = q[order], p[order]
+    else:
+        a, b = E.predicate_join(lhs.device, rhs.device, predicate, pattern)
+    a = a.astype(np.int64)
+    b = b.astype(np.int64)
+    if how == "left":
+        matched = np.zeros(len(lhs), dtype=bool)
         matched[a] = True
         miss = np.nonzero(~matched)[0]
         a = np.concatenate([a, miss])

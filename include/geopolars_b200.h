@@ -314,6 +314,40 @@ int gpl_contains_polygon(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, u
 #define GPL_PREDICATE_INTERSECTS 0
 #define GPL_PREDICATE_CONTAINS 1
 int gpl_spatial_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, int predicate, gpl_pairs **out);
+
+/* ---------------------------------------------------------------- DE-9IM relate ---------- */
+/* The DE-9IM matrix of a[i] and b[i] for any pair of the six types (DESIGN.md §4.20): rows are a's Interior, Boundary and
+ * Exterior, columns b's; boundaries follow the OGC defaults (a point has none, a line's is the Mod-2 set of its chain ends, a
+ * polygon's is its rings; rings are closed implicitly).  Every decision is an exact sign of input coordinates.  Defined for
+ * valid (OGC) operands; on invalid input every entry is still F, 0, 1 or 2 but its value is not specified.  An empty operand
+ * has F in its Interior and Boundary rows / columns.  A null row, or a row with a non-finite coordinate, gives a null matrix.
+ * matrix[9 n] int8 in `mem`, row-major, -1 = F; out_validity (Arrow bitmap in `mem`, may be NULL).  Unequal lengths:
+ * GPL_ERR_LENGTH_MISMATCH; a type outside the six: GPL_ERR_INVALID_TYPE. */
+int gpl_relate(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, int8_t *matrix, uint8_t *out_validity, int mem);
+/* predicates of gpl_relate_predicate / gpl_predicate_join, JTS's definitions on the matrix (dims: the operands' type
+ * dimensions).  GPL_PREDICATE_CONTAINS here is the DE-9IM [T*****FF*] for any pair of types. */
+#define GPL_PREDICATE_WITHIN 2            /* T*F**F*** */
+#define GPL_PREDICATE_CONTAINS_PROPERLY 3 /* T**FF*FF* */
+#define GPL_PREDICATE_COVERS 4            /* T*****FF*, *T****FF*, ***T**FF* or ****T*FF* */
+#define GPL_PREDICATE_COVERED_BY 5        /* T*F**F***, *TF**F***, **FT*F*** or **F*TF*** */
+#define GPL_PREDICATE_TOUCHES 6           /* FT*******, F**T***** or F***T****; false when both dims are 0 */
+#define GPL_PREDICATE_CROSSES 7           /* dims a < b: T*T******; a > b: T*****T**; both 1: 0********; else false */
+#define GPL_PREDICATE_OVERLAPS 8          /* dims both 0 or both 2: T*T***T**; both 1: 1*T***T**; else false */
+#define GPL_PREDICATE_DISJOINT 9          /* FF*FF**** */
+#define GPL_PREDICATE_EQUALS 10           /* same dimension and T*F**FFF*; two empty rows are equal */
+#define GPL_PREDICATE_PATTERN 11          /* `pattern`: 9 characters over TF*012, either case */
+/* row-wise predicate as an Arrow bitmap in `mem`; a null or non-finite row gives false.  `pattern` is read only for
+ * GPL_PREDICATE_PATTERN.  An unknown predicate or a bad pattern: GPL_ERR_INVALID_ARG.  A row stops as soon as its answer is
+ * decided. */
+int gpl_relate_predicate(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, int predicate, const char *pattern, uint8_t *out_bitmap,
+                         int mem);
+/* Predicate join (GeoPandas' sjoin(predicate=...)): every pair (i, j) for which gpl_relate_predicate(lhs[i], rhs[j]) holds,
+ * sorted by (lhs, rhs), as a device-resident gpl_pairs.  Candidates are the pairs gpl_intersects accepts (every accepted
+ * predicate implies it); GPL_PREDICATE_INTERSECTS returns them as they are.  A predicate that can hold for disjoint pairs
+ * (GPL_PREDICATE_DISJOINT, or a pattern whose II, IB, BI and BB entries are all F or *) is GPL_ERR_INVALID_ARG.  Fewer than
+ * 2^31 rows per side (else GPL_ERR_UNSUPPORTED). */
+int gpl_predicate_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, int predicate, const char *pattern, gpl_pairs **out);
+
 int64_t gpl_pairs_count(const gpl_pairs *pairs);
 int gpl_pairs_copy(gpl_ctx *ctx, const gpl_pairs *pairs, uint64_t *lhs, uint64_t *rhs, int mem);
 void gpl_pairs_free(gpl_pairs *pairs);

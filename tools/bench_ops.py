@@ -4,7 +4,7 @@ fraction for the coordinate bytes read, and of the nearest join (100 M points ag
 reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic|valid|boolean] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic|valid|boolean|relate] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
@@ -41,11 +41,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean"), default="all",
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate"), default="all",
                     help="run only the §8 rows, only the point nearest join, only the geometry nearest join, only the "
                          "distance-within join, only the great-circle joins, only the intersection area and overlay join or "
                          "only the geodesic area and perimeter (1 M stars, 10 M parcels, naturalearth_lowres to 1 M rows), or only "
-                         "the boolean geometry ops and the geometry overlay join; "
+                         "the boolean geometry ops and the geometry overlay join, or only the DE-9IM relate, predicates and "
+                         "predicate join; "
                          "'all' runs every arm")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
@@ -86,11 +87,13 @@ def main():
             overlay_rows(args, ctx, dev, st, res)
         if args.only in ("all", "boolean"):
             boolean_rows(args, ctx, dev, st, res)
+        if args.only in ("all", "relate"):
+            relate_rows(args, ctx, dev, st, res)
         if args.only in ("all", "geodesic"):
             geodesic_rows(args, ctx, dev, st, res)
         if args.only in ("all", "valid"):
             valid_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean"):
+        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -525,6 +528,85 @@ def boolean_rows(args, ctx, dev, st, res):
 
     t = timed(st, join, reps=3, warm=1)
     rec("overlay_join (10 000 stars x %d squares)" % (k * k), n_pairs[0], "pairs", t, {})
+
+
+def relate_rows(args, ctx, dev, st, res):
+    """DE-9IM (DESIGN.md §4.20) on the workload of boolean_rows: relate and the touches / within predicates row-wise on 1 M
+    pairs of config 2's stars against the same stars shifted by (3, 2); the predicate join of config 2's 10 000 stars against
+    a 1000 x 1000 grid of unit squares for intersects, touches and within (candidates, sort and the per-pair kernel, host
+    synchronisations included); points within polygons, 10 M uniform points against the 10 000 stars, through the
+    points-in-polygons index and through the DE-9IM route"""
+    import numpy as np
+
+    from geopolars_b200 import synth
+
+    lib = ctx.lib
+
+    def rec(name, units, unit_name, t, extra):
+        r = {"op": name, "units": units, "unit": unit_name, "ms_min": t[0], "ms_avg": t[1], "units_per_s": units / (t[1] * 1e-3),
+             "card": res["card"], "power_limit": res["power_limit"], **extra}
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    def upload(xy, ring_off, geom_off):
+        t = [torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in (xy, ring_off, geom_off)]
+        n = len(geom_off) - 1
+        return ctx.wrap_device(GeometryType.POLYGON, n, len(xy), t[0].data_ptr(), geom_off_ptr=t[2].data_ptr(), ring_off_ptr=t[1].data_ptr(),
+                               n_rings=len(ring_off) - 1, keepalive=tuple(t))
+
+    n = int(1_000_000 * args.scale)
+    g = int(np.ceil(np.sqrt(n)))
+    xy, ro, go = synth.star_polygons(m=n, grid=g)
+    a, b = upload(xy, ro, go), upload(xy + np.array([3.0, 2.0]), ro, go)
+    mat = torch.empty(n * 9, dtype=torch.int8, device=dev)
+    bits = torch.empty((n + 7) // 8, dtype=torch.uint8, device=dev)
+    t = timed(st, lambda: E.check(lib.gpl_relate(ctx._h, a._h, b._h, C.c_void_p(mat.data_ptr()), None, E.GPL_DEVICE)), reps=3, warm=1)
+    rec("relate (%d star pairs, 64 x 64 edges)" % n, n, "row pairs", t, {})
+    for name in ("touches", "within"):
+        code = E.RELATE_PREDICATES[name]
+        t = timed(st, lambda: E.check(lib.gpl_relate_predicate(ctx._h, a._h, b._h, code, None, C.c_void_p(bits.data_ptr()), E.GPL_DEVICE)),
+                  reps=3, warm=1)
+        rec("relate_predicate %s (%d star pairs)" % (name, n), n, "row pairs", t, {})
+    del a, b
+
+    sxy, sro, sgo = synth.star_polygons()
+    stars = upload(sxy, sro, sgo)
+    k = int(1000 * np.sqrt(args.scale))
+    i, j = np.meshgrid(np.arange(k, dtype=np.float64), np.arange(k, dtype=np.float64), indexing="xy")
+    x0, y0 = i.ravel() * (1000.0 / k), j.ravel() * (1000.0 / k)
+    w = 1000.0 / k
+    gxy = np.stack([np.stack([x0, x0 + w, x0 + w, x0, x0], 1), np.stack([y0, y0, y0 + w, y0 + w, y0], 1)], 2).reshape(-1, 2)
+    cells = upload(gxy, np.arange(k * k + 1, dtype=np.int64) * 5, np.arange(k * k + 1, dtype=np.int64))
+
+    def join(lhs, rhs, code, out):
+        h = C.c_void_p()
+        E.check(lib.gpl_predicate_join(ctx._h, lhs._h, rhs._h, code, None, C.byref(h)))
+        out[0] = int(lib.gpl_pairs_count(h))
+        lib.gpl_pairs_free(h)
+
+    for name, lhs, rhs in (("intersects", stars, cells), ("touches", stars, cells), ("within", cells, stars)):
+        cnt = [0]
+        t = timed(st, lambda: join(lhs, rhs, E.RELATE_PREDICATES[name], cnt), reps=3, warm=1)
+        rec("predicate_join %s (%d x %d)" % (name, len(lhs), len(rhs)), cnt[0], "pairs", t, {})
+
+    m = int(10_000_000 * args.scale)
+    pts_t = torch.empty((m, 2), dtype=torch.float64, device=dev)
+    E.check(lib.gpl_gen_uniform_points(ctx._h, 9, 0, m, 1000.0, pts_t.data_ptr()))
+    pts = ctx.wrap_device(GeometryType.POINT, m, m, pts_t.data_ptr(), keepalive=(pts_t,))
+    cnt = [0]
+
+    def pip():
+        idx = E.PipIndex(stars)
+        h = C.c_void_p()
+        E.check(lib.gpl_contains_join_pairs_array(ctx._h, idx._h, pts._h, C.byref(h)))
+        cnt[0] = int(lib.gpl_pairs_count(h))
+        lib.gpl_pairs_free(h)
+        idx.free()
+
+    t = timed(st, pip, reps=3, warm=1)
+    rec("points within polygons, index route (%d points x %d stars, index build included)" % (m, len(stars)), cnt[0], "pairs", t, {})
+    t = timed(st, lambda: join(pts, stars, E.RELATE_PREDICATES["within"], cnt), reps=3, warm=1)
+    rec("points within polygons, relate route (%d points x %d stars)" % (m, len(stars)), cnt[0], "pairs", t, {})
 
 
 def geodesic_rows(args, ctx, dev, st, res):
