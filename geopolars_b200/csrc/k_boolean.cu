@@ -14,13 +14,14 @@
 //   classes   the piece after an edge start or a vertex is classified by sym_ring_pos of the symbolic point just after it
 //             (on the other boundary: the symbolic point just left of it tells the direction), the piece after a crossing is
 //             the other state of the piece before it; the keep rules of the op select the pieces;
-//   linking   a kept piece ends at the node where the next one starts; at a vertex with several kept pieces leaving, the one
-//             bounding the same interior sector follows (the first clockwise from the reversed incoming direction, an exact
-//             angular order by quadrant and orient2d of input points); every ring that visits a node twice is then split into
-//             the loops between its visits;
-//   rings     a loop's turning number (exact: quadrants of the input edge directions and the turn signs at its nodes) makes it
-//             a shell (counter-clockwise) or a hole; a hole goes to the smallest shell containing one of its vertices that is not
-//             on that shell (orient2d on the output coordinates: the one decision that reads constructed points).
+//   linking   a kept piece ends at the output point where the next one starts (nodes are points: two crossings that round
+//             to one point are one node); where several kept pieces leave a point, the one bounding the same interior sector
+//             follows (the first clockwise from the reversed incoming direction, an exact angular order by quadrant and
+//             orient2d of the point and input points); every ring that visits a point twice is then split into the loops
+//             between its visits, loops of fewer than 3 points dropped;
+//   rings     the sign of a loop's f64 shoelace makes it a shell (counter-clockwise) or a hole, a loop whose area is within
+//             the sum's rounding bound is dropped; a hole goes to the smallest shell containing one of its vertices that is not
+//             on that shell (orient2d on the output coordinates).
 // Layout: the cut-point enumeration (O(|∂A| |∂B|) per row, the hot path) is one warp per row, groups of lanes per outer edge
 // and ring-box skipping as in overlap_pass; it runs as a count pass, a scan and a write pass.  One warp per row orders and
 // classifies the records; one thread per row links and assembles them, twice (counts, then the MultiPolygon's offsets and
@@ -342,31 +343,6 @@ __global__ void __launch_bounds__(kBoolThreads) k_bool_classify(int64_t n, BOper
 }
 
 // ---- linking and ring assembly: one thread per row ----------------------------------------------------------------------
-struct NKey {
-    int kind;  // 0 vertex (x, y), 1 crossing (ar, as, br, bs)
-    double x, y;
-    int64_t ar, br;
-    int32_t as, bs;
-};
-__device__ __forceinline__ int key_cmp(const NKey &a, const NKey &b) {
-    if (a.kind != b.kind) return a.kind < b.kind ? -1 : 1;
-    if (a.kind == 0) {
-        if (a.x != b.x) return a.x < b.x ? -1 : 1;
-        if (a.y != b.y) return a.y < b.y ? -1 : 1;
-        return 0;
-    }
-    if (a.ar != b.ar) return a.ar < b.ar ? -1 : 1;
-    if (a.as != b.as) return a.as < b.as ? -1 : 1;
-    if (a.br != b.br) return a.br < b.br ? -1 : 1;
-    if (a.bs != b.bs) return a.bs < b.bs ? -1 : 1;
-    return 0;
-}
-__device__ __forceinline__ NKey node_key(const BNode &nd) {
-    if (nd.kind != K_CROSS) return NKey{0, nd.pt.x, nd.pt.y, 0, 0, 0, 0};
-    if (nd.side == 0) return NKey{1, 0.0, 0.0, nd.ring, nd.oring, nd.seg, nd.oseg};
-    return NKey{1, 0.0, 0.0, nd.oring, nd.ring, nd.oseg, nd.seg};
-}
-
 // the kept pieces of one row, in output direction (B pieces of a difference reversed)
 struct Pieces {
     const BOperands *o;
@@ -379,14 +355,6 @@ struct Pieces {
         return k + 1 < nn && nd[k + 1].side == nd[k].side && nd[k + 1].ring == nd[k].ring && nd[k + 1].seg == nd[k].seg;
     }
     // start (a = 0) or end (a = 1) of the piece along its directed input edge
-    __device__ NKey raw_key(int j, int a) const {
-        const int64_t k = kp[j];
-        if (a == 0) return node_key(nd[k]);
-        if (next_on_edge(k)) return node_key(nd[k + 1]);
-        double2 p, q;
-        dir_edge(*o, nd[k].side, nd[k].ring, nd[k].seg, p, q);
-        return NKey{0, q.x, q.y, 0, 0, 0, 0};
-    }
     __device__ double2 raw_pt(int j, int a) const {
         const int64_t k = kp[j];
         if (a == 0) return nd[k].pt;
@@ -395,8 +363,6 @@ struct Pieces {
         dir_edge(*o, nd[k].side, nd[k].ring, nd[k].seg, p, q);
         return q;
     }
-    __device__ NKey from_key(int j) const { return raw_key(j, rev(j) ? 1 : 0); }
-    __device__ NKey to_key(int j) const { return raw_key(j, rev(j) ? 0 : 1); }
     __device__ double2 from_pt(int j) const { return raw_pt(j, rev(j) ? 1 : 0); }
     __device__ double2 to_pt(int j) const { return raw_pt(j, rev(j) ? 0 : 1); }
     // the input edge of the piece, in output direction
@@ -410,31 +376,15 @@ struct Pieces {
     }
 };
 
-struct FromKeyLess {
+__device__ __forceinline__ int pt_cmp(double2 a, double2 b) { return a.x != b.x ? (a.x < b.x ? -1 : 1) : (a.y != b.y ? (a.y < b.y ? -1 : 1) : 0); }
+
+struct FromPtLess {  // pieces by the output coordinates of their start
     const Pieces *pc;
     __device__ bool operator()(int32_t a, int32_t b) const {
-        const int c = key_cmp(pc->from_key(a), pc->from_key(b));
+        const int c = pt_cmp(pc->from_pt(a), pc->from_pt(b));
         return c ? c < 0 : a < b;
     }
 };
-
-// quadrant of the direction Q - P: 0 [0, 90°), 1 [90°, 180°), 2 [180°, 270°), 3 [270°, 360°)
-__device__ __forceinline__ int quadrant(double2 P, double2 Q) {
-    const int dx = cmpd(Q.x, P.x), dy = cmpd(Q.y, P.y);
-    if (dx > 0 && dy >= 0) return 0;
-    if (dx <= 0 && dy > 0) return 1;
-    if (dx < 0 && dy <= 0) return 2;
-    return 3;
-}
-
-// sign of the turn from piece u into piece w at the node where u ends
-__device__ __forceinline__ int turn_sign(const Pieces &pc, int u, int w) {
-    double2 Pu, Qu, Pw, Qw;
-    pc.edge(u, Pu, Qu);
-    pc.edge(w, Pw, Qw);
-    if (pc.to_key(u).kind == 0) return orient_sign(Pu, pc.to_pt(u), Qw);
-    return orient_sign(Pu, Qu, Qw);  // a proper crossing: Pw and Qw lie strictly on either side of u's line
-}
 
 // 0 outside / 1 on the boundary / 2 inside of the loop through the from-points of its pieces
 __device__ int point_in_loop(const Pieces &pc, const int32_t *lp, const BLoop &L, double2 v) {
@@ -465,7 +415,6 @@ __device__ double loop_area2(const Pieces &pc, const int32_t *lp, const BLoop &L
 
 struct LoopLess {  // members by their shell's first vertex, holes after their shell by their first vertex
     const BLoop *L;
-    __device__ static int pt_cmp(double2 a, double2 b) { return a.x != b.x ? (a.x < b.x ? -1 : 1) : (a.y != b.y ? (a.y < b.y ? -1 : 1) : 0); }
     __device__ bool operator()(int32_t a, int32_t b) const {
         const int pa = L[a].type > 0 ? a : L[a].parent, pb = L[b].type > 0 ? b : L[b].parent;
         int c = pt_cmp(L[pa].first, L[pb].first);
@@ -497,32 +446,42 @@ __global__ void __launch_bounds__(128) k_bool_assemble(int64_t n, BOperands o, i
         for (int64_t k = 0; k < nn; ++k)
             if (nd[k].keep) kp[J++] = (int32_t)k;
         const Pieces pc{&o, nd, nn, kp, op == GPL_BOOLEAN_DIFFERENCE};
-        // nodes: the kept pieces sorted by their start; gs: the first position of each start node
+        // a piece whose two ends round to one point (between two crossings within half an ulp of each other) has no length
+        int Jp = 0;
+        for (int j = 0; j < J; ++j)
+            if (!same_pt(pc.raw_pt(j, 0), pc.raw_pt(j, 1))) kp[Jp++] = kp[j];
+        J = Jp;
+        // nodes are output coordinates: the kept pieces sorted by the point they start at; gs: the first position of each
+        // point.  Distinct input nodes are distinct points unless rounding puts two crossings (or a crossing and a vertex) on
+        // one point; linking at that point by the angular rule below then joins the rings that meet there as the rounded
+        // coordinates require, where linking by input node would leave a ring through the point twice or rings touching in
+        // a cycle of such points
         for (int j = 0; j < J; ++j) ord[j] = j;
-        heap_sort(ord, (int64_t)J, FromKeyLess{&pc});
+        heap_sort(ord, (int64_t)J, FromPtLess{&pc});
         for (int i = 0; i < J; ++i) {
             rank[ord[i]] = i;
-            gs[i] = (i > 0 && key_cmp(pc.from_key(ord[i]), pc.from_key(ord[i - 1])) == 0) ? gs[i - 1] : i;
+            gs[i] = (i > 0 && same_pt(pc.from_pt(ord[i]), pc.from_pt(ord[i - 1]))) ? gs[i - 1] : i;
         }
         // successor of every kept piece
         for (int j = 0; j < J; ++j) {
-            const NKey to = pc.to_key(j);
+            const double2 V = pc.to_pt(j);
             int lo = 0, hi = J;
             while (lo < hi) {
                 const int mid = (lo + hi) >> 1;
-                if (key_cmp(pc.from_key(ord[mid]), to) < 0) lo = mid + 1;
+                if (pt_cmp(pc.from_pt(ord[mid]), V) < 0) lo = mid + 1;
                 else hi = mid;
             }
             int end = lo;
-            while (end < J && key_cmp(pc.from_key(ord[end]), to) == 0) ++end;
+            while (end < J && same_pt(pc.from_pt(ord[end]), V)) ++end;
             if (end == lo) {
                 nxt[j] = -1;  // a dangling piece (invalid input)
-            } else if (end == lo + 1 || to.kind != 0) {
+            } else if (end == lo + 1) {
                 nxt[j] = ord[lo];
-            } else {  // several pieces leave this vertex: the first clockwise from the reversed incoming direction
+            } else {  // several pieces leave this point: the first clockwise from the reversed incoming direction; a piece
+                      // straight back along it comes last (it bounds the sector on the far side of a notch that rounding
+                      // folded to zero width; kept pieces of valid operands never run back along each other in exact terms)
                 double2 Pu, Qu;
                 pc.edge(j, Pu, Qu);
-                const double2 V = pc.to_pt(j);
                 int best = -1, bh = -1;
                 double2 bq = V;
                 for (int i = lo; i < end; ++i) {
@@ -532,14 +491,15 @@ __global__ void __launch_bounds__(128) k_bool_assemble(int64_t n, BOperands o, i
                     int h;
                     if (c > 0) h = 0;
                     else if (c < 0) h = 2;
-                    else h = (cmpd(Qw.x, V.x) == cmpd(Pu.x, V.x) && cmpd(Qw.y, V.y) == cmpd(Pu.y, V.y)) ? 3 : 1;
+                    else h = (cmpd(Qw.x, V.x) == cmpd(Pu.x, V.x) && cmpd(Qw.y, V.y) == cmpd(Pu.y, V.y)) ? -1 : 1;
                     if (best < 0 || h > bh || (h == bh && (h == 0 || h == 2) && orient_sign(V, bq, Qw) > 0)) best = ord[i], bh = h, bq = Qw;
                 }
                 nxt[j] = best;
             }
         }
-        // trace the rings and split each at its repeated nodes: stk holds the open path, npos[node] its position there
-        // (a visited piece has rank -1 - rank)
+        // trace the rings and split each at its repeated points: stk holds the open path, npos[point] its position there
+        // (a visited piece has rank -1 - rank).  A spike ... X Y X ... closes the loop (X, Y), dropped below with fewer than
+        // 3 coordinates
         for (int i = 0; i < J; ++i) npos[i] = -1;
         int nl = 0, nlp = 0;
         for (int j0 = 0; j0 < J; ++j0) {
@@ -569,26 +529,26 @@ __global__ void __launch_bounds__(128) k_bool_assemble(int64_t n, BOperands o, i
             }
             for (int i = 0; i < sp; ++i) npos[gs[-1 - rank[stk[i]]]] = -1;
         }
-        // shells and holes: the turning number of each loop; coordinates after merging repeats; the first (smallest) vertex
+        // shells and holes: the sign of each loop's shoelace (f64, relative to its first coordinate), a loop of fewer than 3
+        // points or whose area is within the rounding bound of that sum dropped; the first (smallest) vertex
         for (int l = 0; l < nl; ++l) {
             BLoop &lo = L[l];
-            int m = 0, nc = 0, rot = -1;
-            double2 first = make_double2(0.0, 0.0);
-            for (int i = 0; i < lo.len; ++i) {
-                const int u = lp[lo.start + i], w = lp[lo.start + (i + 1 == lo.len ? 0 : i + 1)];
-                double2 Pu, Qu, Pw, Qw;
-                pc.edge(u, Pu, Qu);
-                pc.edge(w, Pw, Qw);
-                const int d = (quadrant(Pw, Qw) - quadrant(Pu, Qu) + 4) & 3;
-                m += d == 1 ? 1 : d == 3 ? -1 : d == 2 ? (turn_sign(pc, u, w) > 0 ? 2 : -2) : 0;
-                const double2 v = pc.from_pt(w), pv = pc.from_pt(u);
-                if (!same_pt(v, pv)) {
-                    ++nc;
-                    if (rot < 0 || v.x < first.x || (v.x == first.x && v.y < first.y)) rot = i + 1 == lo.len ? 0 : i + 1, first = v;
+            int rot = 0;
+            const double2 o0 = pc.from_pt(lp[lo.start]);
+            double2 first = o0;
+            double a2 = 0.0, mag = 0.0;
+            for (int i = 1; i < lo.len; ++i) {
+                const double2 v = pc.from_pt(lp[lo.start + i]);
+                if (pt_cmp(v, first) < 0) rot = i, first = v;
+                if (i + 1 < lo.len) {
+                    const double2 e = pc.from_pt(lp[lo.start + i + 1]);
+                    const double t1 = (v.x - o0.x) * (e.y - o0.y), t2 = (e.x - o0.x) * (v.y - o0.y);
+                    a2 += t1 - t2;
+                    mag += fabs(t1) + fabs(t2);
                 }
             }
-            lo.ncoord = nc, lo.rot = rot, lo.first = first, lo.parent = -1;
-            lo.type = nc < 3 ? 0 : m > 0 ? 1 : m < 0 ? -1 : 0;
+            lo.ncoord = lo.len, lo.rot = rot, lo.first = first, lo.parent = -1;
+            lo.type = lo.len < 3 || fabs(a2) <= (double)(lo.len + 4) * 0x1p-52 * mag ? 0 : a2 > 0.0 ? 1 : -1;
         }
         // every hole to the smallest shell containing it
         for (int h = 0; h < nl; ++h) {
