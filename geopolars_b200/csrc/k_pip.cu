@@ -2029,6 +2029,9 @@ static int launch_histogram(gpl_ctx *ctx, const int32_t *ids, int64_t n, unsigne
 int pip_query(gpl_ctx *ctx, const gpl_pip_index *idx, const double *pts_dev, const uint8_t *validity_dev, int64_t n,
               int32_t *first_dev, int32_t *count_dev, cudaStream_t stream, unsigned long long *hist = nullptr) {
     if (n == 0) return GPL_OK;
+    // the stream kernel reads each point as one 16-byte load: a misaligned column would fault it
+    GPL_REQUIRE((reinterpret_cast<uintptr_t>(pts_dev) & 15) == 0, GPL_ERR_INVALID_ARG,
+                "contains join: the device point column must be 16-byte aligned (got %p)", (const void *)pts_dev);
     const double2 *pts = reinterpret_cast<const double2 *>(pts_dev);
     const IndexView v = view_of(idx);
     // the deferred list holds chunk-relative uint32 indices: process at most 2^31 points per launch pair
@@ -2070,6 +2073,12 @@ using namespace gpl;
 // line).  Best effort: failures only cost performance.  The device-wide carve-out only ever grows while
 // the context lives and is restored by gpl_ctx_destroy; the window is dropped and the persisting lines are released
 // when the index that set them is freed (neither call waits for running kernels: they are cache hints).
+// The carve-out (set-aside) is capped at kL2SetAsideMax while the window keeps covering the whole hot part with a hit ratio
+// of 1: a large set-aside starves the point stream of L2.  Config 2's index asks for 31.25 MB of the 50 MB; with all of it
+// set aside even a torch op moving the same 16 B in / 4 B out per point took 1.05 ms instead of 0.65 ms, and k_pip_stream
+// 1.95 ms; with 8 MB it took 1.78 ms, the same as with 0 or 16 MB, while config 4 (9.4 MB asked) was unchanged at 8 MB
+// (one H100 80GB HBM3 at 700 W, DESIGN.md 4.2).
+constexpr size_t kL2SetAsideMax = size_t(8) << 20;
 static void l2_pin(gpl_pip_index *idx, bool on) {
     gpl_ctx *ctx = idx->ctx;
     if (ctx->l2_persist_max == 0 || ctx->l2_window_max == 0) return;
@@ -2077,7 +2086,8 @@ static void l2_pin(gpl_pip_index *idx, bool on) {
     memset(&attr, 0, sizeof(attr));
     if (on) {
         const size_t want = idx->hot_bytes ? idx->hot_bytes : idx->slab_bytes;
-        size_t carve = std::min<size_t>(want, ctx->l2_persist_max);
+        const size_t carve = std::min<size_t>(want, ctx->l2_persist_max);
+        const size_t set_aside = std::min(carve, kL2SetAsideMax);
         if (!ctx->l2_limit_saved) {
             size_t prev = 0;
             if (cudaDeviceGetLimit(&prev, cudaLimitPersistingL2CacheSize) == cudaSuccess) {
@@ -2086,11 +2096,10 @@ static void l2_pin(gpl_pip_index *idx, bool on) {
                 ctx->l2_cur_limit = prev;
             }
         }
-        if (carve > ctx->l2_cur_limit) {
-            (void)cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve);
-            ctx->l2_cur_limit = carve;
+        if (set_aside > ctx->l2_cur_limit) {
+            (void)cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, set_aside);
+            ctx->l2_cur_limit = set_aside;
         }
-        carve = std::min(carve, ctx->l2_cur_limit);
         size_t win = std::min<size_t>(want, ctx->l2_window_max);
         attr.accessPolicyWindow.base_ptr = idx->slab;
         attr.accessPolicyWindow.num_bytes = win;

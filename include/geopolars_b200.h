@@ -278,7 +278,8 @@ int gpl_pip_index_timeline(gpl_ctx *ctx, const gpl_pip_index *idx, double *out12
 int gpl_pip_index_dump(gpl_ctx *ctx, const gpl_pip_index *idx, int which, void *dst, int64_t *nbytes);
 /* spatial_join(points, polygons, Inner) candidate+exact test (spatial_index.rs:74-143):
  * first_id[p] = lowest polygon row containing point p, or -1; count[p] (may be NULL) = number of
- * containing rows.  points: xy interleaved, n points, in `mem`. */
+ * containing rows.  points: xy interleaved, n points, in `mem`; a device column must be 16-byte aligned
+ * (GPL_ERR_INVALID_ARG otherwise). */
 int gpl_contains_join(gpl_ctx *ctx, const gpl_pip_index *idx, const double *points_xy, int64_t n_points,
                       int32_t *first_id, int32_t *count, int mem);
 /* the join and the per-polygon hit counts of config 4 in ONE pass over the points: counts[n polygon rows] (u64) +=

@@ -22,7 +22,9 @@ over `--reps` launches after `--warmup`) on the same index for three point colum
   code is 0, 1 or 2 (decoded from `PipIndex.dump("raster")`);
 * `outside`: points outside the union bbox: the stream-and-write floor, no raster gather;
 
-and `walk_ms` = bench - no_walk, `raster_ms` = no_walk - outside.
+and `walk_ms` = bench - no_walk, `raster_ms` = no_walk - outside, and beside them `traffic_floor`: a torch op on the
+benchmark's point column that reads 16 bytes and writes 4 per point, as the kernel does (see `traffic_floor`), the time
+the card takes for the same traffic without any of the kernel's work.
 
     python tools/pip_step_breakdown.py [--workload c2|c4] [--reps 20] [--warmup 5] [--points N] [--split] [--out FILE]
 
@@ -87,6 +89,25 @@ def split_columns(torch, idx, poly_xy, n, dev):
     outside[:, 0] = x1 + 1.0 + outside[:, 0] * (x1 - x0)
     outside[:, 1] = y0 + outside[:, 1] * (y1 - y0)
     return no_walk.contiguous(), outside
+
+
+def traffic_floor(torch, pts, stream, warmup, reps):
+    """ms of a torch op that moves what k_pip_stream must move per point, 16 bytes in and 4 out: an int32 column of the
+    low words of x, a strided read that still pulls every 32-byte sector of the point column.  CUDA events around the
+    op; min and median over `reps`."""
+    low = pts.view(torch.int32)[:, 0]
+    out = torch.empty(low.shape[0], dtype=torch.int32, device=pts.device)
+    for _ in range(warmup):
+        out.copy_(low)
+    ms = []
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(stream)
+        out.copy_(low)
+        e1.record(stream)
+        e1.synchronize()
+        ms.append(e0.elapsed_time(e1))
+    return stat(ms, 3)
 
 
 def main():
@@ -230,6 +251,7 @@ def main():
             med = {k: v["median"] for k, v in split.items()}
             split["walk_ms"] = round(med["bench"] - med["no_walk"], 3)
             split["raster_ms"] = round(med["no_walk"] - med["outside"], 3)
+            split["traffic_floor"] = traffic_floor(torch, pts, stream, args.warmup, args.reps)
         state["idx"].free()
         stream.synchronize()
 
