@@ -126,6 +126,7 @@ extern "C" {
     fn gpl_is_valid(ctx: *mut GplCtx, a: *const GplArray, reason: *mut i8, out_validity: *mut u8, mem: c_int) -> c_int;
     fn gpl_boolean_op(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, op: c_int, out: *mut *mut GplArray) -> c_int;
     fn gpl_overlay_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, pairs: *mut *mut GplPairs, out: *mut *mut GplArray) -> c_int;
+    fn gpl_dissolve(ctx: *mut GplCtx, input: *const GplArray, group: *const i64, mem: c_int, n_groups: i64, out: *mut *mut GplArray) -> c_int;
     fn gpl_relate(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, matrix: *mut i8, out_validity: *mut u8, mem: c_int) -> c_int;
     fn gpl_relate_predicate(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, predicate: c_int, pattern: *const c_char, out_bitmap: *mut u8, mem: c_int) -> c_int;
     fn gpl_predicate_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, predicate: c_int, pattern: *const c_char, out: *mut *mut GplPairs) -> c_int;
@@ -508,6 +509,12 @@ pub trait GeoSeriesB200Ext {
     /// geometry overlay join of two (Multi)Polygon columns (`overlay(how="intersection")`): every pair whose intersection has a
     /// member, sorted by (lhs, rhs), with that intersection (bit for bit what `intersection` gives for the pair)
     fn overlay_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Series)>;
+    /// the union of the rows of each group (GeoPandas' `dissolve(by=...)`, geo's `unary_union` per group): `group[i]` in
+    /// [-1, n_groups) names row i's group (-1 skips it); row g of the MultiPolygon result is the union of its group's rows.
+    /// Null rows are skipped, a non-finite row nulls its group, a group with no row is an empty MultiPolygon
+    fn dissolve(&self, group: &[i64], n_groups: i64) -> Result<Series>;
+    /// the union of every row as a one-row MultiPolygon column (`dissolve` with one group)
+    fn union_all(&self) -> Result<Series>;
     /// the DE-9IM matrix of every row pair as a string such as "FF2F11212" (rows: self's Interior, Boundary, Exterior); null
     /// for a null or non-finite row.  Any two of the six types; defined for valid (OGC) operands
     fn relate(&self, other: &Series) -> Result<Series>;
@@ -744,6 +751,21 @@ impl GeoSeriesB200Ext for Series {
 
     fn difference(&self, other: &Series) -> Result<Series> {
         boolean_op(self, other, GPL_BOOLEAN_DIFFERENCE)
+    }
+
+    fn dissolve(&self, group: &[i64], n_groups: i64) -> Result<Series> {
+        if group.len() != self.len() {
+            return Err(PolarsError::ShapeMismatch(format!("dissolve: {} group codes for {} rows", group.len(), self.len()).into()).into());
+        }
+        let ctx = ctx()?;
+        let a = to_device(ctx, self)?;
+        let mut out = std::ptr::null_mut();
+        check(unsafe { gpl_dissolve(ctx, a.0, group.as_ptr(), GPL_HOST, n_groups, &mut out) })?; // code range -> error
+        from_device(ctx, Dev(out))
+    }
+
+    fn union_all(&self) -> Result<Series> {
+        self.dissolve(&vec![0i64; self.len()], 1)
     }
 
     fn overlay_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Series)> {

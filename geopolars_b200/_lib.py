@@ -176,6 +176,7 @@ SIGNATURES = {
     "gpl_is_valid": (_INT, [_P, _P, _P, _P, _INT]),
     "gpl_boolean_op": (_INT, [_P, _P, _P, _INT, C.POINTER(_P)]),
     "gpl_overlay_join": (_INT, [_P, _P, _P, C.POINTER(_P), C.POINTER(_P)]),
+    "gpl_dissolve": (_INT, [_P, _P, _P, _INT, C.c_int64, C.POINTER(_P)]),
     "gpl_haversine_distance": (_INT, [_P, _P, _P, _P, _P, _INT]),
     "gpl_geo_index_build": (_INT, [_P, _P, C.POINTER(_P)]),
     "gpl_geo_index_free": (None, [_P]),

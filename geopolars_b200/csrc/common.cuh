@@ -344,6 +344,22 @@ __device__ __forceinline__ int fast_expansion_sum_zeroelim(int elen, const doubl
     if ((Q != 0.0) || (hi == 0)) h[hi++] = Q;
     return hi;
 }
+// h = b * e exactly (at most 2 elen terms, zeros eliminated, at least one term)
+__device__ __forceinline__ int scale_expansion_zeroelim(int elen, const double *e, double b, double *h) {
+    double Q, sum, hh, p1, p0;
+    int hi = 0;
+    two_product(e[0], b, Q, hh);
+    if (hh != 0.0) h[hi++] = hh;
+    for (int ei = 1; ei < elen; ++ei) {
+        two_product(e[ei], b, p1, p0);
+        two_sum(Q, p0, sum, hh);
+        if (hh != 0.0) h[hi++] = hh;
+        fast_two_sum(p1, sum, Q, hh);
+        if (hh != 0.0) h[hi++] = hh;
+    }
+    if ((Q != 0.0) || (hi == 0)) h[hi++] = Q;
+    return hi;
+}
 
 // stages B, C, D of the adaptive predicate: exact sign whenever the filter cannot decide
 static __device__ __noinline__ double orient2d_adapt(double ax, double ay, double bx, double by, double cx, double cy,

@@ -32,6 +32,7 @@
 #include <algorithm>
 #include <memory>
 
+#include "boolean.cuh"
 #include "common.cuh"
 #include "join_grid.cuh"
 #include "join_host.cuh"
@@ -41,118 +42,6 @@
 #include "sym_point.cuh"
 
 namespace gpl {
-
-constexpr int kBoolThreads = 128;
-
-// one node on a directed input edge: its start, a vertex of the other side inside it, or a proper crossing
-struct BNode {
-    double2 pt;
-    double t;              // f64 parameter along the directed edge (a tie-break for invalid input only)
-    int64_t ring, oring;   // the edge's ring; a crossing: the other edge's ring (else -1)
-    int32_t seg, oseg;     // segment index in the ring (stored orientation)
-    int8_t side, kind, state, keep;
-};
-enum { K_START = 0, K_VERTEX = 1, K_CROSS = 2 };
-enum { S_OUT = 0, S_IN = 2, S_ON_SAME = 3, S_ON_OPP = 4 };
-
-// one closed loop of kept pieces
-struct BLoop {
-    int32_t start, len, ncoord, rot, type, parent;  // type: 1 shell, -1 hole, 0 dropped
-    double2 first;                                  // the lexicographically smallest vertex
-};
-
-struct BOperands {
-    Side v[2];
-    const int64_t *mem[2];   // member offsets of a MultiPolygon column, NULL for Polygon
-    const uint8_t *valid[2];
-    const int8_t *sg[2];
-    const double4 *box[2];
-};
-
-__device__ __forceinline__ void row_members(const BOperands &o, int s, int64_t r, int64_t &m0, int64_t &m1) {
-    m0 = o.mem[s] ? o.mem[s][r] : r, m1 = o.mem[s] ? o.mem[s][r + 1] : r + 1;
-}
-
-// the directed edge (interior on the left) of segment `seg` of ring `ring`
-__device__ __forceinline__ void dir_edge(const BOperands &o, int side, int64_t ring, int32_t seg, double2 &p, double2 &q) {
-    const Chain c = part_ring(o.v[side], ring);
-    const double2 u = c[seg], w = c[seg + 1];
-    if (o.sg[side][ring] > 0) p = u, q = w;
-    else p = w, q = u;
-}
-__device__ __forceinline__ void stored_edge(const BOperands &o, int side, int64_t ring, int32_t seg, double2 &p, double2 &q) {
-    const Chain c = part_ring(o.v[side], ring);
-    p = c[seg], q = c[seg + 1];
-}
-__device__ __forceinline__ bool same_pt(double2 a, double2 b) { return a.x == b.x && a.y == b.y; }
-
-// the crossing point of the stored A edge (a0, a1) and B edge (b0, b1): the same bits from either side's records
-__device__ __forceinline__ double2 crossing_point(double2 a0, double2 a1, double2 b0, double2 b1) {
-    const double o0 = orient2d(b0.x, b0.y, b1.x, b1.y, a0.x, a0.y), o1 = orient2d(b0.x, b0.y, b1.x, b1.y, a1.x, a1.y);
-    const double t = o0 / (o0 - o1);
-    return make_double2(a0.x + t * (a1.x - a0.x), a0.y + t * (a1.y - a0.y));
-}
-
-// One enumeration pass: the nodes of the directed edges of rings [xr0, xr1) of side X against the rings [yr0, yr1) of the
-// other side.  Returns this lane's number of nodes; WRITE: also stores them at base + atomicAdd(slot).
-template <bool WRITE>
-__device__ int64_t node_pass(const BOperands &o, int X, int64_t xr0, int64_t xr1, int64_t yr0, int64_t yr1, int lane, BNode *base,
-                             int *slot) {
-    const int Y = 1 - X;
-    const Side &xv = o.v[X], &yv = o.v[Y];
-    int64_t cnt = 0;
-    for (int64_t rx = xr0; rx < xr1; ++rx) {
-        const int sx = o.sg[X][rx];
-        if (sx == 0) continue;
-        const Chain cx = part_ring(xv, rx);
-        const int64_t nseg = cx.coords() - 1;
-        int groups = 32;
-        while (groups > 1 && groups / 2 >= nseg) groups >>= 1;
-        const int G = 32 / groups, grp = lane / G, sub = lane - grp * G;
-        for (int64_t b0 = 0; b0 < nseg; b0 += groups) {
-            const int64_t i = b0 + grp;
-            if (i >= nseg) continue;
-            const double2 u = cx[i], w = cx[i + 1];
-            if (same_pt(u, w)) continue;
-            const double2 p = sx > 0 ? u : w, q = sx > 0 ? w : u;
-            if (sub == 0) {
-                ++cnt;
-                if (WRITE) base[atomicAdd(slot, 1)] = BNode{p, 0.0, rx, -1, (int32_t)i, -1, (int8_t)X, K_START, 0, 0};
-            }
-            const double ex0 = fmin(p.x, q.x), ex1 = fmax(p.x, q.x), ey0 = fmin(p.y, q.y), ey1 = fmax(p.y, q.y);
-            const double dx = q.x - p.x, dy = q.y - p.y, dd = dx * dx + dy * dy;
-            for (int64_t ry = yr0; ry < yr1; ++ry) {
-                if (o.sg[Y][ry] == 0) continue;
-                const double4 rb = o.box[Y][ry];
-                if (ex1 < rb.x || rb.z < ex0 || ey1 < rb.y || rb.w < ey0) continue;
-                const Chain cy = part_ring(yv, ry);
-                const int64_t ny = cy.coords() - 1;
-                for (int64_t j = sub; j < ny; j += G) {
-                    const double2 s = cy[j], g = cy[j + 1];
-                    if (same_pt(s, g)) continue;
-                    if (ex1 < fmin(s.x, g.x) || fmax(s.x, g.x) < ex0 || ey1 < fmin(s.y, g.y) || fmax(s.y, g.y) < ey0) continue;
-                    const int os = orient_sign(p, q, s), og = orient_sign(p, q, g);
-                    if (os == 0 && point_in_rect(s, p, q) && !same_pt(s, p) && !same_pt(s, q)) {  // s: a vertex inside (p, q)
-                        ++cnt;
-                        if (WRITE) {
-                            const double t = ((s.x - p.x) * dx + (s.y - p.y) * dy) / dd;
-                            base[atomicAdd(slot, 1)] = BNode{s, t, rx, -1, (int32_t)i, -1, (int8_t)X, K_VERTEX, 0, 0};
-                        }
-                    }
-                    if (os * og < 0 && orient_sign(s, g, p) * orient_sign(s, g, q) < 0) {  // a proper crossing
-                        ++cnt;
-                        if (WRITE) {
-                            const double2 pt = X == 0 ? crossing_point(u, w, s, g) : crossing_point(s, g, u, w);
-                            const double op = orient2d(s.x, s.y, g.x, g.y, p.x, p.y), oq = orient2d(s.x, s.y, g.x, g.y, q.x, q.y);
-                            base[atomicAdd(slot, 1)] = BNode{pt, op / (op - oq), rx, ry, (int32_t)i, (int32_t)j, (int8_t)X, K_CROSS, 0, 0};
-                        }
-                    }
-                }
-            }
-        }
-    }
-    return cnt;
-}
 
 // the row's validity (both rows present and finite) and, when valid, its node count; the rows are ia[r] / ib[r] (or r)
 __device__ __forceinline__ bool row_ok(const BOperands &o, int64_t ra, int64_t rb, int lane) {
@@ -194,73 +83,6 @@ __global__ void __launch_bounds__(kBoolThreads) k_bool_nodes(int64_t n, BOperand
             row_valid[r] = ok ? 1 : 0;
             if (c >= (1LL << 30)) atomicExch(too_big, 1);
         }
-    }
-}
-
-// ---- ordering of the nodes of one row: by edge, the start first, then along the edge by exact signs ---------------------
-struct NodeLess {
-    const BOperands *o;
-    // -1: a before b along the directed edge (p, q); 0: undecided
-    __device__ int along(const BNode &a, const BNode &b, double2 p, double2 q) const {
-        if (a.kind == K_VERTEX && b.kind == K_VERTEX) {
-            const int d = cmpd(q.x, p.x);
-            return d ? cmpd(a.pt.x, b.pt.x) * d : cmpd(a.pt.y, b.pt.y) * cmpd(q.y, p.y);
-        }
-        if (a.kind == K_VERTEX || b.kind == K_VERTEX) {
-            const BNode &v = a.kind == K_VERTEX ? a : b, &x = a.kind == K_VERTEX ? b : a;
-            double2 s, g;
-            stored_edge(*o, 1 - x.side, x.oring, x.oseg, s, g);
-            const int sv = orient_sign(s, g, v.pt);
-            if (sv == 0) return 0;
-            const int vb = sv == orient_sign(s, g, p) ? -1 : 1;  // v before the crossing
-            return a.kind == K_VERTEX ? vb : -vb;
-        }
-        double2 s1, g1, s2, g2;
-        stored_edge(*o, 1 - a.side, a.oring, a.oseg, s1, g1);
-        stored_edge(*o, 1 - b.side, b.oring, b.oseg, s2, g2);
-        int c1 = orient_sign(s1, g1, s2), c2 = orient_sign(s1, g1, g2);
-        if (c1 * c2 >= 0 && (c1 | c2)) return (c1 ? c1 : c2) == orient_sign(s1, g1, p) ? 1 : -1;  // b's edge on one side of a's line
-        c1 = orient_sign(s2, g2, s1), c2 = orient_sign(s2, g2, g1);
-        if (c1 * c2 >= 0 && (c1 | c2)) return (c1 ? c1 : c2) == orient_sign(s2, g2, p) ? -1 : 1;
-        return cmpd(a.t, b.t);
-    }
-    __device__ bool operator()(const BNode &a, const BNode &b) const {
-        if (a.side != b.side) return a.side < b.side;
-        if (a.ring != b.ring) return a.ring < b.ring;
-        if (a.seg != b.seg) return a.seg < b.seg;
-        if ((a.kind == K_START) != (b.kind == K_START)) return a.kind == K_START;
-        if (a.kind != K_START) {
-            double2 p, q;
-            dir_edge(*o, a.side, a.ring, a.seg, p, q);
-            const int c = along(a, b, p, q);
-            if (c) return c < 0;
-        }
-        if (a.kind != b.kind) return a.kind < b.kind;
-        if (a.oring != b.oring) return a.oring < b.oring;
-        if (a.oseg != b.oseg) return a.oseg < b.oseg;
-        if (a.pt.x != b.pt.x) return a.pt.x < b.pt.x;
-        return a.pt.y < b.pt.y;
-    }
-};
-
-template <class T, class Less>
-__device__ void heap_sort(T *a, int64_t n, const Less &less) {
-    auto sift = [&](int64_t i, int64_t m) {
-        for (;;) {
-            int64_t c = 2 * i + 1;
-            if (c >= m) return;
-            if (c + 1 < m && less(a[c], a[c + 1])) ++c;
-            if (!less(a[i], a[c])) return;
-            const T t = a[i];
-            a[i] = a[c], a[c] = t;
-            i = c;
-        }
-    };
-    for (int64_t i = n / 2 - 1; i >= 0; --i) sift(i, n);
-    for (int64_t m = n - 1; m > 0; --m) {
-        const T t = a[0];
-        a[0] = a[m], a[m] = t;
-        sift(0, m);
     }
 }
 
@@ -342,90 +164,6 @@ __global__ void __launch_bounds__(kBoolThreads) k_bool_classify(int64_t n, BOper
     }
 }
 
-// ---- linking and ring assembly: one thread per row ----------------------------------------------------------------------
-// the kept pieces of one row, in output direction (B pieces of a difference reversed)
-struct Pieces {
-    const BOperands *o;
-    const BNode *nd;  // the row's nodes
-    int64_t nn;
-    const int32_t *kp;  // kept piece -> node index
-    bool rev_b;
-    __device__ bool rev(int j) const { return rev_b && nd[kp[j]].side == 1; }
-    __device__ bool next_on_edge(int64_t k) const {
-        return k + 1 < nn && nd[k + 1].side == nd[k].side && nd[k + 1].ring == nd[k].ring && nd[k + 1].seg == nd[k].seg;
-    }
-    // start (a = 0) or end (a = 1) of the piece along its directed input edge
-    __device__ double2 raw_pt(int j, int a) const {
-        const int64_t k = kp[j];
-        if (a == 0) return nd[k].pt;
-        if (next_on_edge(k)) return nd[k + 1].pt;
-        double2 p, q;
-        dir_edge(*o, nd[k].side, nd[k].ring, nd[k].seg, p, q);
-        return q;
-    }
-    __device__ double2 from_pt(int j) const { return raw_pt(j, rev(j) ? 1 : 0); }
-    __device__ double2 to_pt(int j) const { return raw_pt(j, rev(j) ? 0 : 1); }
-    // the input edge of the piece, in output direction
-    __device__ void edge(int j, double2 &P, double2 &Q) const {
-        const BNode &n = nd[kp[j]];
-        dir_edge(*o, n.side, n.ring, n.seg, P, Q);
-        if (rev(j)) {
-            const double2 t = P;
-            P = Q, Q = t;
-        }
-    }
-};
-
-__device__ __forceinline__ int pt_cmp(double2 a, double2 b) { return a.x != b.x ? (a.x < b.x ? -1 : 1) : (a.y != b.y ? (a.y < b.y ? -1 : 1) : 0); }
-
-struct FromPtLess {  // pieces by the output coordinates of their start
-    const Pieces *pc;
-    __device__ bool operator()(int32_t a, int32_t b) const {
-        const int c = pt_cmp(pc->from_pt(a), pc->from_pt(b));
-        return c ? c < 0 : a < b;
-    }
-};
-
-// 0 outside / 1 on the boundary / 2 inside of the loop through the from-points of its pieces
-__device__ int point_in_loop(const Pieces &pc, const int32_t *lp, const BLoop &L, double2 v) {
-    int wn = 0;
-    for (int i = 0; i < L.len; ++i) {
-        const double2 s = pc.from_pt(lp[L.start + i]), e = pc.from_pt(lp[L.start + (i + 1 == L.len ? 0 : i + 1)]);
-        if (same_pt(s, e)) continue;
-        const int o = orient_sign(s, e, v);
-        if (o == 0 && point_in_rect(v, s, e)) return 1;
-        if (s.y <= v.y) {
-            if (e.y > v.y && o > 0) ++wn;
-        } else if (e.y <= v.y && o < 0) {
-            --wn;
-        }
-    }
-    return wn ? 2 : 0;
-}
-
-__device__ double loop_area2(const Pieces &pc, const int32_t *lp, const BLoop &L) {
-    double a = 0.0;
-    const double2 o = pc.from_pt(lp[L.start]);
-    for (int i = 1; i + 1 < L.len; ++i) {
-        const double2 s = pc.from_pt(lp[L.start + i]), e = pc.from_pt(lp[L.start + i + 1]);
-        a += (s.x - o.x) * (e.y - o.y) - (e.x - o.x) * (s.y - o.y);
-    }
-    return a;
-}
-
-struct LoopLess {  // members by their shell's first vertex, holes after their shell by their first vertex
-    const BLoop *L;
-    __device__ bool operator()(int32_t a, int32_t b) const {
-        const int pa = L[a].type > 0 ? a : L[a].parent, pb = L[b].type > 0 ? b : L[b].parent;
-        int c = pt_cmp(L[pa].first, L[pb].first);
-        if (c) return c < 0;
-        if (pa != pb) return pa < pb;
-        if ((L[a].type > 0) != (L[b].type > 0)) return L[a].type > 0;
-        c = pt_cmp(L[a].first, L[b].first);
-        return c ? c < 0 : a < b;
-    }
-};
-
 // One thread per row.  Scratch (8 int32 per node, one BLoop per node) is indexed by the row's node offset.  Counting pass:
 // members, rings and coordinates of the row; WRITE: the MultiPolygon's part / ring offsets and coordinates at the row's bases.
 template <bool WRITE>
@@ -438,161 +176,10 @@ __global__ void __launch_bounds__(128) k_bool_assemble(int64_t n, BOperands o, i
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += stride) {
         const int64_t o0 = off[r], nn = off[r + 1] - o0;
-        int32_t *kp = ws + o0, *ord = kp + ws_stride, *rank = ord + ws_stride, *gs = rank + ws_stride, *nxt = gs + ws_stride,
-                *npos = nxt + ws_stride, *stk = npos + ws_stride, *lp = stk + ws_stride;
-        BLoop *L = loops + o0;
-        const BNode *nd = nodes + o0;
-        int J = 0;
-        for (int64_t k = 0; k < nn; ++k)
-            if (nd[k].keep) kp[J++] = (int32_t)k;
-        const Pieces pc{&o, nd, nn, kp, op == GPL_BOOLEAN_DIFFERENCE};
-        // a piece whose two ends round to one point (between two crossings within half an ulp of each other) has no length
-        int Jp = 0;
-        for (int j = 0; j < J; ++j)
-            if (!same_pt(pc.raw_pt(j, 0), pc.raw_pt(j, 1))) kp[Jp++] = kp[j];
-        J = Jp;
-        // nodes are output coordinates: the kept pieces sorted by the point they start at; gs: the first position of each
-        // point.  Distinct input nodes are distinct points unless rounding puts two crossings (or a crossing and a vertex) on
-        // one point; linking at that point by the angular rule below then joins the rings that meet there as the rounded
-        // coordinates require, where linking by input node would leave a ring through the point twice or rings touching in
-        // a cycle of such points
-        for (int j = 0; j < J; ++j) ord[j] = j;
-        heap_sort(ord, (int64_t)J, FromPtLess{&pc});
-        for (int i = 0; i < J; ++i) {
-            rank[ord[i]] = i;
-            gs[i] = (i > 0 && same_pt(pc.from_pt(ord[i]), pc.from_pt(ord[i - 1]))) ? gs[i - 1] : i;
-        }
-        // successor of every kept piece
-        for (int j = 0; j < J; ++j) {
-            const double2 V = pc.to_pt(j);
-            int lo = 0, hi = J;
-            while (lo < hi) {
-                const int mid = (lo + hi) >> 1;
-                if (pt_cmp(pc.from_pt(ord[mid]), V) < 0) lo = mid + 1;
-                else hi = mid;
-            }
-            int end = lo;
-            while (end < J && same_pt(pc.from_pt(ord[end]), V)) ++end;
-            if (end == lo) {
-                nxt[j] = -1;  // a dangling piece (invalid input)
-            } else if (end == lo + 1) {
-                nxt[j] = ord[lo];
-            } else {  // several pieces leave this point: the first clockwise from the reversed incoming direction; a piece
-                      // straight back along it comes last (it bounds the sector on the far side of a notch that rounding
-                      // folded to zero width; kept pieces of valid operands never run back along each other in exact terms)
-                double2 Pu, Qu;
-                pc.edge(j, Pu, Qu);
-                int best = -1, bh = -1;
-                double2 bq = V;
-                for (int i = lo; i < end; ++i) {
-                    double2 Pw, Qw;
-                    pc.edge(ord[i], Pw, Qw);
-                    const int c = orient_sign(V, Pu, Qw);
-                    int h;
-                    if (c > 0) h = 0;
-                    else if (c < 0) h = 2;
-                    else h = (cmpd(Qw.x, V.x) == cmpd(Pu.x, V.x) && cmpd(Qw.y, V.y) == cmpd(Pu.y, V.y)) ? -1 : 1;
-                    if (best < 0 || h > bh || (h == bh && (h == 0 || h == 2) && orient_sign(V, bq, Qw) > 0)) best = ord[i], bh = h, bq = Qw;
-                }
-                nxt[j] = best;
-            }
-        }
-        // trace the rings and split each at its repeated points: stk holds the open path, npos[point] its position there
-        // (a visited piece has rank -1 - rank).  A spike ... X Y X ... closes the loop (X, Y), dropped below with fewer than
-        // 3 coordinates
-        for (int i = 0; i < J; ++i) npos[i] = -1;
-        int nl = 0, nlp = 0;
-        for (int j0 = 0; j0 < J; ++j0) {
-            if (rank[j0] < 0) continue;  // visited
-            int sp = 0, cur = j0;
-            while (cur >= 0 && rank[cur] >= 0) {
-                const int node = gs[rank[cur]];
-                rank[cur] = -1 - rank[cur];
-                if (npos[node] >= 0) {  // a loop closes here: stk[npos[node] .. sp)
-                    const int i0 = npos[node];
-                    L[nl].start = nlp, L[nl].len = sp - i0;
-                    for (int i = i0; i < sp; ++i) {
-                        lp[nlp++] = stk[i];
-                        npos[gs[-1 - rank[stk[i]]]] = -1;
-                    }
-                    ++nl;
-                    sp = i0;
-                }
-                npos[node] = sp;
-                stk[sp++] = cur;
-                cur = nxt[cur];
-            }
-            if (cur == j0 && sp > 0) {
-                L[nl].start = nlp, L[nl].len = sp;
-                for (int i = 0; i < sp; ++i) lp[nlp++] = stk[i];
-                ++nl;
-            }
-            for (int i = 0; i < sp; ++i) npos[gs[-1 - rank[stk[i]]]] = -1;
-        }
-        // shells and holes: the sign of each loop's shoelace (f64, relative to its first coordinate), a loop of fewer than 3
-        // points or whose area is within the rounding bound of that sum dropped; the first (smallest) vertex
-        for (int l = 0; l < nl; ++l) {
-            BLoop &lo = L[l];
-            int rot = 0;
-            const double2 o0 = pc.from_pt(lp[lo.start]);
-            double2 first = o0;
-            double a2 = 0.0, mag = 0.0;
-            for (int i = 1; i < lo.len; ++i) {
-                const double2 v = pc.from_pt(lp[lo.start + i]);
-                if (pt_cmp(v, first) < 0) rot = i, first = v;
-                if (i + 1 < lo.len) {
-                    const double2 e = pc.from_pt(lp[lo.start + i + 1]);
-                    const double t1 = (v.x - o0.x) * (e.y - o0.y), t2 = (e.x - o0.x) * (v.y - o0.y);
-                    a2 += t1 - t2;
-                    mag += fabs(t1) + fabs(t2);
-                }
-            }
-            lo.ncoord = lo.len, lo.rot = rot, lo.first = first, lo.parent = -1;
-            lo.type = lo.len < 3 || fabs(a2) <= (double)(lo.len + 4) * 0x1p-52 * mag ? 0 : a2 > 0.0 ? 1 : -1;
-        }
-        // every hole to the smallest shell containing it
-        for (int h = 0; h < nl; ++h) {
-            if (L[h].type >= 0) continue;
-            int best = -1;
-            double barea = 0.0;
-            for (int s = 0; s < nl; ++s) {
-                if (L[s].type <= 0) continue;
-                // the hole's smallest vertex first: for intersection and difference it is an input vertex
-                int pos = point_in_loop(pc, lp, L[s], L[h].first);
-                for (int i = 0; i < L[h].len && pos == 1; ++i) pos = point_in_loop(pc, lp, L[s], pc.from_pt(lp[L[h].start + i]));
-                if (pos != 2) continue;
-                const double a = loop_area2(pc, lp, L[s]);
-                if (best < 0 || a < barea) best = s, barea = a;
-            }
-            if (best < 0) L[h].type = 0;
-            else L[h].parent = best;
-        }
-        // output order
-        int nout = 0, nm = 0;
-        int64_t ncoords = 0;
-        for (int l = 0; l < nl; ++l)
-            if (L[l].type != 0) {
-                stk[nout++] = l;
-                nm += L[l].type > 0;
-                ncoords += L[l].ncoord + 1;
-            }
-        if (!WRITE) {
-            cm[r] = nm, cr[r] = nout, cc[r] = ncoords;
-            continue;
-        }
-        heap_sort(stk, (int64_t)nout, LoopLess{L});
-        int64_t mb = mbase[r], rb = rbase[r], cb = cbase[r];
-        for (int k = 0; k < nout; ++k) {
-            const BLoop &lo = L[stk[k]];
-            if (lo.type > 0) part_off[mb++] = rb;
-            ring_off[rb++] = cb;
-            for (int i = 0; i < lo.len; ++i) {
-                const int idx = lo.rot + i < lo.len ? lo.rot + i : lo.rot + i - lo.len;
-                const double2 v = pc.from_pt(lp[lo.start + idx]), pv = pc.from_pt(lp[lo.start + (idx == 0 ? lo.len - 1 : idx - 1)]);
-                if (i == 0 || !same_pt(v, pv)) oxy[cb++] = v;
-            }
-            oxy[cb++] = lo.first;
-        }
+        int64_t nm, nr, nc;
+        assemble_pieces<WRITE>(o, op == GPL_BOOLEAN_DIFFERENCE, nodes + o0, nn, ws + o0, ws_stride, loops + o0, nullptr, nm, nr, nc,
+                               WRITE ? mbase[r] : 0, WRITE ? rbase[r] : 0, WRITE ? cbase[r] : 0, part_off, ring_off, oxy);
+        if (!WRITE) cm[r] = nm, cr[r] = nr, cc[r] = nc;
     }
 }
 

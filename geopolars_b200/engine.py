@@ -487,6 +487,27 @@ def overlay_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, np.nda
     return a, b, geoms
 
 
+def dissolve(d: DeviceArray, codes, n_groups: int) -> DeviceArray:
+    """the union of the rows of each group of a (Multi)Polygon column (DESIGN.md §4.21): row g of the MultiPolygon result is
+    the union of the rows whose code is g, for g in [0, n_groups); code -1 and null rows are skipped, a row with a non-finite
+    coordinate makes its group null, a group with no present row is an empty MultiPolygon.  A group of two rows i < j is bit
+    for bit `boolean_op(d[i], d[j], "union")`"""
+    codes = np.ascontiguousarray(codes, dtype=np.int64)
+    n_groups = int(n_groups)
+    if codes.shape != (len(d),):
+        raise ValueError("dissolve: one group code per row (%d rows, %d codes)" % (len(d), codes.size))
+    if n_groups < 0:
+        raise ValueError("dissolve: n_groups must be >= 0")
+    if codes.size and (codes.min() < -1 or codes.max() >= n_groups):
+        raise ValueError("dissolve: group codes must lie in [-1, n_groups)")
+    return _out_array(d.ctx, d.ctx.lib.gpl_dissolve, d._h, _np_ptr(codes), GPL_HOST, n_groups)
+
+
+def union_all(d: DeviceArray) -> DeviceArray:
+    """the union of every row of a (Multi)Polygon column as a MultiPolygon column of one row (`dissolve` with one group)"""
+    return dissolve(d, np.zeros(len(d), dtype=np.int64), 1)
+
+
 def intersects(a: DeviceArray, b: DeviceArray) -> np.ndarray:
     n = len(a)
     bm = np.zeros((n + 7) // 8, dtype=np.uint8)

@@ -148,6 +148,15 @@ class GeoDataFrame:
     def __repr__(self) -> str:
         return f"GeoDataFrame(shape={self.shape}, columns={self.columns})"
 
+    def dissolve(self, by: str) -> "GeoDataFrame":
+        """GeoPandas' `dissolve(by=by)` with sort=True, dropna=True: one row per distinct non-null value of column `by`, in
+        ascending order, with the union of the geometries of its rows (see `dissolve` below).  Only the `by` column and the
+        geometry are returned: aggregating other columns (GeoPandas' `aggfunc`) is not done here; pyarrow's `Table.group_by`
+        does it on the same keys."""
+        pa = _pa()
+        keys, geoms = dissolve(self.geometry, self._table.column(by))
+        return GeoDataFrame(pa.table({by: keys, self._geometry_name: geoms.to_arrow()}), geometry=self._geometry_name)
+
 
 def from_arrow(data):
     """geopolars.from_arrow (py-geopolars/python/geopolars/convert.py:33-56): a Table becomes a GeoDataFrame, an Array or
@@ -323,6 +332,12 @@ class GeoRustSeries:
     def difference(self, other: GeoSeries) -> GeoSeries:
         """row-wise difference self[i] - other[i] (GeoPandas' `a.difference(b)`), as `intersection`"""
         return self._wrap(E.boolean_op(self._d(), other.device, "difference"))
+
+    def union_all(self) -> GeoSeries:
+        """the union of every row, a (Multi)Polygon column, as a GeoSeries of one MultiPolygon row (GeoPandas'
+        `union_all()`, formerly `unary_union`; DESIGN.md §4.21).  Null rows are skipped; a row with a non-finite coordinate
+        makes the result null; no present row gives an empty MultiPolygon.  Valid (OGC) rows give valid output."""
+        return self._wrap(E.union_all(self._d()))
 
     def translate(self, xoff: float = 0.0, yoff: float = 0.0) -> GeoSeries:
         return self._wrap(E.translate(self._d(), xoff, yoff))
@@ -602,3 +617,30 @@ def geo_dwithin_join(lhs: GeoSeries, rhs: GeoSeries, distance: float, how: str =
         matched[a] = True
         a, b, d = _left_rows(a, b, d, np.nonzero(~matched)[0])
     return a, b, d
+
+
+def _factorize(by, n: int):
+    """(sorted distinct non-null keys as a pyarrow Array, int64 code per row with -1 for a null key)"""
+    pa = _pa()
+    arr = by.combine_chunks() if isinstance(by, pa.ChunkedArray) else by if isinstance(by, pa.Array) else pa.array(list(by) if not isinstance(by, np.ndarray) else by, from_pandas=True)
+    if len(arr) != n:
+        raise ValueError("dissolve: `by` has %d values for %d rows" % (len(arr), n))
+    valid = ~np.asarray(arr.is_null(nan_is_null=True).to_numpy(zero_copy_only=False), dtype=bool)
+    keys = pa.compute.unique(arr.filter(pa.array(valid))) if valid.any() else arr.slice(0, 0)
+    keys = keys.take(pa.compute.sort_indices(keys))
+    codes = np.asarray(pa.compute.index_in(arr, value_set=keys).fill_null(-1).to_numpy(zero_copy_only=False), dtype=np.int64)
+    codes[~valid] = -1
+    return keys, codes
+
+
+def dissolve(series: GeoSeries, by):
+    """GeoPandas' `GeoSeries.groupby(by).union_all()` / `dissolve(by=...)` with sort=True, dropna=True: (keys, GeoSeries) with
+    one MultiPolygon row per distinct non-null key of `by` (array-like of one key per row: integers, strings or anything
+    pyarrow can sort), keys ascending, row k the union of the rows whose key is keys[k] (DESIGN.md §4.21).  Rows with a null
+    key and null rows are skipped; a row with a non-finite coordinate makes its group's row null.  Aggregating other columns
+    (GeoPandas' `aggfunc`) is not done here; pyarrow's `Table.group_by` does it on the same keys."""
+    import pyarrow.compute  # noqa: F401 (pa.compute)
+
+    d = series.device
+    keys, codes = _factorize(by, len(d))
+    return keys, GeoSeries(_device=E.dissolve(d, codes, len(keys)), name=series.name)

@@ -451,6 +451,18 @@ int gpl_boolean_op(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, int op,
  * returns.  Candidates are the pairs gpl_intersects accepts; touching pairs are dropped.  Fewer than 2^31 rows per side (else
  * GPL_ERR_UNSUPPORTED); any other type: GPL_ERR_INVALID_TYPE. */
 int gpl_overlay_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **pairs, gpl_array **out);
+/* Dissolve (GeoPandas' dissolve(by=...), union_all(); geo's unary_union), DESIGN.md §4.21: row g of *out (a MultiPolygon
+ * column of n_groups rows) is the regularised union of the closed rows whose group code is g.  group has in->n_geoms
+ * entries in [-1, n_groups), in `mem` (gpl_mem); code -1 skips a row, as does a null row.  Rows are read as gpl_boolean_op
+ * reads them; the output has its form (closed rings, counter-clockwise shells and clockwise holes starting at their smallest
+ * vertex, holes and members in the same order, every cut point a vertex).  A row with a non-finite coordinate makes its group's
+ * row null; a group with no present row is an empty MultiPolygon.  Every combinatorial decision is an exact sign for valid
+ * (OGC) rows, only crossing points are rounded, and a group of exactly two present rows i < j is bit for bit
+ * gpl_boolean_op(in[i], in[j], GPL_BOOLEAN_UNION) (one row: its union with an empty row).  Invalid rows give a well-formed
+ * MultiPolygon column of bounded size whose geometry is not specified.  Deterministic.  Any other type: GPL_ERR_INVALID_TYPE;
+ * a code outside [-1, n_groups) or n_groups < 0: GPL_ERR_INVALID_ARG; 2^31 or more rows or groups, or a group with 2^30 or more
+ * boundary nodes: GPL_ERR_UNSUPPORTED. */
+int gpl_dissolve(gpl_ctx *ctx, const gpl_array *in, const int64_t *group, int mem, int64_t n_groups, gpl_array **out);
 
 /* ---------------------------------------------------------------- validity ---------------- */
 /* OGC validity of every row, any geometry type, DESIGN.md §4.18: reason[n] (int8, in `mem`) is the first failing rule in the

@@ -41,12 +41,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate"), default="all",
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve"), default="all",
                     help="run only the §8 rows, only the point nearest join, only the geometry nearest join, only the "
                          "distance-within join, only the great-circle joins, only the intersection area and overlay join or "
                          "only the geodesic area and perimeter (1 M stars, 10 M parcels, naturalearth_lowres to 1 M rows), or only "
                          "the boolean geometry ops and the geometry overlay join, or only the DE-9IM relate, predicates and "
-                         "predicate join; "
+                         "predicate join, or only dissolve / union_all; "
                          "'all' runs every arm")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
@@ -89,11 +89,13 @@ def main():
             boolean_rows(args, ctx, dev, st, res)
         if args.only in ("all", "relate"):
             relate_rows(args, ctx, dev, st, res)
+        if args.only in ("all", "dissolve"):
+            dissolve_rows(args, ctx, dev, st, res)
         if args.only in ("all", "geodesic"):
             geodesic_rows(args, ctx, dev, st, res)
         if args.only in ("all", "valid"):
             valid_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate"):
+        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -528,6 +530,106 @@ def boolean_rows(args, ctx, dev, st, res):
 
     t = timed(st, join, reps=3, warm=1)
     rec("overlay_join (10 000 stars x %d squares)" % (k * k), n_pairs[0], "pairs", t, {})
+
+
+def dissolve_rows(args, ctx, dev, st, res):
+    """dissolve / union_all (DESIGN.md §4.21): 1 M two-row groups (config 2's stars and the same stars shifted by (3, 2)) beside
+    the row-wise union of the same rows; the overlay round trip of the 10 000 stars (overlay_join with the 200 x 200 grid of
+    5-unit squares, then dissolve of the pieces by star); union_all of the 10 000 stars plus the shifted stars (20 000 rows);
+    union_all of naturalearth_lowres.  Each row also carries the per-kernel GPU time of one call (torch.profiler), so the
+    phases (candidate join, nodes, classify, assembly) can be told apart."""
+    import numpy as np
+
+    from geopolars_b200 import datasets, synth
+
+    lib = ctx.lib
+
+    def phases(fn):
+        from torch.profiler import ProfilerActivity, profile
+
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        out = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", None)
+            if t is None:
+                t = getattr(e, "cuda_time_total", 0.0)
+            if t > 0:
+                key = e.key.split("<")[0].split("(")[0].replace("void ", "").replace("gpl::", "")
+                out[key] = round(out.get(key, 0.0) + t / 1e3, 3)
+        return dict(sorted(out.items(), key=lambda kv: -kv[1])[:12])
+
+    def rec(name, units, unit_name, t, extra):
+        r = {"op": name, "units": units, "unit": unit_name, "ms_min": t[0], "ms_avg": t[1], "units_per_s": units / (t[1] * 1e-3),
+             "card": res["card"], "power_limit": res["power_limit"], **extra}
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    def upload(xy, ring_off, geom_off):
+        t = [torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in (xy, ring_off, geom_off)]
+        n = len(geom_off) - 1
+        return ctx.wrap_device(GeometryType.POLYGON, n, len(xy), t[0].data_ptr(), geom_off_ptr=t[2].data_ptr(), ring_off_ptr=t[1].data_ptr(),
+                               n_rings=len(ring_off) - 1, keepalive=tuple(t))
+
+    def pair_column(xy, ro):
+        n = len(ro) - 1
+        return upload(np.concatenate([xy, xy + np.array([3.0, 2.0])]), np.concatenate([ro, ro[1:] + ro[-1]]), np.arange(2 * n + 1, dtype=np.int64))
+
+    def dissolve_call(col, codes, ng, size):
+        def run():
+            h = C.c_void_p()
+            E.check(lib.gpl_dissolve(ctx._h, col._h, codes.ctypes.data, E.GPL_HOST, ng, C.byref(h)))
+            size[0] = int(E.DeviceArray(ctx, h).view().n_coords)
+        return run
+
+    n = int(1_000_000 * args.scale)
+    g = int(np.ceil(np.sqrt(n)))
+    xy, ro, go = synth.star_polygons(m=n, grid=g)
+    a, b = upload(xy, ro, go), upload(xy + np.array([3.0, 2.0]), ro, go)
+    size = [0]
+
+    def union():
+        h = C.c_void_p()
+        E.check(lib.gpl_boolean_op(ctx._h, a._h, b._h, 1, C.byref(h)))
+        size[0] = int(E.DeviceArray(ctx, h).view().n_coords)
+
+    t = timed(st, union, reps=3, warm=1)
+    rec("boolean_op union (%d star pairs, 64 x 64 edges)" % n, n, "row pairs", t, {"out_coords": size[0]})
+    del a, b
+    both = pair_column(xy, ro)
+    codes = np.concatenate([np.arange(n), np.arange(n)]).astype(np.int64)
+    run = dissolve_call(both, codes, n, size)
+    t = timed(st, run, reps=3, warm=1)
+    rec("dissolve (%d two-row star groups)" % n, n, "groups", t, {"out_coords": size[0], "phases_ms": phases(run)})
+    del both
+
+    sxy, sro, sgo = synth.star_polygons()
+    stars = upload(sxy, sro, sgo)
+    k = 200
+    i, j = np.meshgrid(np.arange(k, dtype=np.float64), np.arange(k, dtype=np.float64), indexing="xy")
+    x0, y0 = i.ravel() * 5.0, j.ravel() * 5.0
+    gxy = np.stack([np.stack([x0, x0 + 5.0, x0 + 5.0, x0, x0], 1), np.stack([y0, y0, y0 + 5.0, y0 + 5.0, y0], 1)], 2).reshape(-1, 2)
+    cells = upload(gxy, np.arange(k * k + 1, dtype=np.int64) * 5, np.arange(k * k + 1, dtype=np.int64))
+    li, _, pieces = E.overlay_join(stars, cells)
+    lcodes = li.astype(np.int64)
+    run = dissolve_call(pieces, lcodes, len(sgo) - 1, size)
+    t = timed(st, run, reps=3, warm=1)
+    rec("dissolve (overlay round trip: %d pieces of 10 000 stars)" % len(li), len(li), "rows", t, {"out_coords": size[0], "phases_ms": phases(run)})
+
+    for m, grid in ((300, 20), (1000, 40)):  # one group is assembled by one thread: its cost grows faster than its size
+        mxy, mro, _ = synth.star_polygons(m=m, grid=grid)
+        both = pair_column(mxy, mro)
+        zeros = np.zeros(len(both), dtype=np.int64)
+        run = dissolve_call(both, zeros, 1, size)
+        t = timed(st, run, reps=1, warm=0)
+        rec("union_all (%d stars + the same shifted by (3, 2))" % m, len(both), "rows", t, {"out_coords": size[0], "phases_ms": phases(run)})
+
+    ne = datasets.read_dataset("naturalearth_lowres").geometry.device
+    zeros = np.zeros(len(ne), dtype=np.int64)
+    run = dissolve_call(ne, zeros, 1, size)
+    t = timed(st, run, reps=3, warm=1)
+    rec("union_all (naturalearth_lowres, %d rows)" % len(ne), len(ne), "rows", t, {"out_coords": size[0], "phases_ms": phases(run)})
 
 
 def relate_rows(args, ctx, dev, st, res):
