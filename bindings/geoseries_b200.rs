@@ -457,7 +457,7 @@ pub trait GeoSeriesB200Ext {
     /// `spatial_join` dispatches (geopolars/src/spatial_index.rs:89-135)
     fn contains(&self, other: &Series) -> Result<Series>;
     /// the (lhs_index, rhs_index) pair list of `spatial_join(lhs, rhs, SpatialJoinArgs { predicate, .. })`
-    /// (spatial_index.rs:139-157) for any two geometry columns; feed it to the DataFrame joins at :159-203
+    /// (spatial_index.rs:139-157) for any two geometry columns, sorted by (lhs, rhs); feed it to the DataFrame joins at :159-203
     fn spatial_join_pairs(&self, rhs: &Series, predicate: c_int) -> Result<(Vec<u64>, Vec<u64>)>;
     /// nearest-geometry join of this geometry column (any type) against any geometry column (GeoPandas'
     /// `sjoin_nearest`): every right row at the minimum distance <= `max_distance` (inclusive, `f64::INFINITY` =
@@ -481,7 +481,7 @@ pub trait GeoSeriesB200Ext {
     /// invalid input the value is finite but not specified
     fn intersection_area(&self, other: &Series) -> Result<Series>;
     /// area-weighted overlay join of two (Multi)Polygon columns: every pair whose closed geometries intersect (touching pairs
-    /// included, with area 0), as (lhs_index, rhs_index, area) in an unspecified order; the area is bit for bit what
+    /// included, with area 0), as (lhs_index, rhs_index, area) sorted by (lhs, rhs); the area is bit for bit what
     /// `intersection_area` computes for the pair
     fn overlay_area_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
     /// geo's `GeodesicArea::geodesic_area_signed` on WGS84 for a column in (lon, lat) degrees, square metres: counter-clockwise

@@ -9,6 +9,7 @@
 
 #include <algorithm>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -52,6 +53,8 @@ static int warp_grid(int64_t rows, int warps_per_cta) {
     int64_t want = ceil_div(rows, warps_per_cta);
     return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * 16));
 }
+// CTAs of 256 threads for one thread per item, at most 16 per SM (the threads stride over the remaining items)
+static int flat_grid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)kSMs * 16)); }
 
 static const char *type_name(int t) {
     switch (t) {
@@ -146,9 +149,9 @@ struct gpl_array {
     int refcount = 1;
 };
 
-// result of a join (gpl_spatial_join, gpl_contains_join_pairs_array, gpl_nearest_join_pairs_array, gpl_dwithin_join_pairs,
-// gpl_overlay_area_join):
-// (lhs, rhs) row pairs
+// result of a join (gpl_spatial_join, gpl_overlay_area_join, gpl_overlay_join, gpl_predicate_join,
+// gpl_contains_join_pairs_array, the nearest, distance-within and great-circle pair joins):
+// (lhs, rhs) row pairs, sorted by (lhs, rhs), no pair twice
 struct gpl_pairs {
     gpl_ctx *ctx = nullptr;
     uint64_t *lhs = nullptr, *rhs = nullptr;  // device
@@ -158,6 +161,27 @@ struct gpl_pairs {
 };
 
 namespace gpl {
+
+// An owned pair list: freed when it goes out of scope unless it is released to the caller.
+using Pairs = std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)>;
+// A list of n pairs of ctx with lhs / rhs (and, with_dist, dist) allocated but not written.
+static int pairs_new(gpl_ctx *ctx, int64_t n, bool with_dist, Pairs &out) {
+    out.reset(new gpl_pairs());
+    out->ctx = ctx;
+    out->with_dist = with_dist;
+    if (n == 0) return GPL_OK;
+    out->n = n;
+    void *p = nullptr;
+    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)n, &p));
+    out->lhs = (uint64_t *)p;
+    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)n, &p));
+    out->rhs = (uint64_t *)p;
+    if (with_dist) {
+        GPL_TRY(ctx->alloc(sizeof(double) * (size_t)n, &p));
+        out->dist = (double *)p;
+    }
+    return GPL_OK;
+}
 
 gpl_array *array_new(gpl_ctx *ctx, int32_t type);
 void array_retain(gpl_array *a);

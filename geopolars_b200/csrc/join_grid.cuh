@@ -108,15 +108,15 @@ static int join_grid_build(gpl_ctx *ctx, const double *b4, const uint8_t *has, i
     return GPL_OK;
 }
 
-// The candidate stage of gpl_spatial_join (k_pairs.cu), shared with gpl_overlay_area_join (k_overlay.cu): every pair whose
-// envelopes intersect (closed intervals) that passes `test`, appended to res->lhs / res->rhs in candidate order (an order
-// that depends on the grid's cell lists; callers that need a fixed order sort).  Both sides: fewer than 2^31 rows.
+// The candidate stage of gpl_spatial_join (k_pairs.cu), shared with gpl_overlay_area_join, gpl_overlay_join,
+// gpl_predicate_join and gpl_dissolve: every pair whose envelopes intersect (closed intervals) that passes `test`, as a list
+// sorted by (lhs, rhs) in out (with_dist: its dist allocated, not written).  Both sides: fewer than 2^31 rows.
 enum JoinTest {
     JOIN_POINT_IN_R,     // the Point row of lhs lies in the (Multi)Polygon / (Multi)LineString row of rhs (contains(point))
     JOIN_POINT_IN_L,     // the same with the roles swapped
     JOIN_POLY_CONTAINS,  // (Multi)Polygon lhs row contains the Polygon rhs row
     JOIN_INTERSECTS      // geo Intersects of the two rows, as gpl_intersects decides it
 };
-int join_candidate_pairs(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, JoinTest test, const char *who, gpl_pairs *res);
+int join_candidate_pairs(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, JoinTest test, const char *who, bool with_dist, Pairs &out);
 
 }  // namespace gpl

@@ -1,6 +1,6 @@
-// join_host.cuh — the host pipeline shared by the nearest and distance-within joins (k_nearest.cu) and their great-circle
-// counterparts (k_geo_join.cu): dense outputs delivered to host or device memory, and the pair list (count, scan, write,
-// per-row sort by rhs).
+// join_host.cuh — the host pipeline of the joins: the dense outputs of the nearest joins (k_nearest.cu, k_geo_join.cu)
+// delivered to host or device memory, and the pair list every join returns, sorted by (lhs, rhs): sorted_pairs (allocation
+// and per-row sort by rhs), pair_list (count, scan, write, sorted_pairs) and keep_pairs (order-preserving compaction).
 #pragma once
 
 #include <algorithm>
@@ -132,58 +132,65 @@ static __global__ void __launch_bounds__(kSortRadixThreads) k_sort_rows_large(co
     }
 }
 
-// A pair list of n left rows: count(cnt) writes each left row's number of pairs, a scan turns the counts into int64 offsets,
-// write(off, raw, raw_d) writes each row's right rows (and, when raw_d != NULL, their distances) at its offsets in any order,
-// and k_sort_rows_* order each row's pairs by rhs.  The right rows of one left row are distinct, so the sorted list does not
-// depend on the order of the write pass.
-template <class Count, class Write>
-static int pair_list(gpl_ctx *ctx, int64_t n, bool with_dist, gpl_pairs **out, Count &&count, Write &&write) {
-    gpl_pairs *res = new gpl_pairs();
-    res->ctx = ctx;
-    res->with_dist = with_dist;
-    *out = res;
-    if (n == 0) return GPL_OK;
-    Scratch<double> raw_d, tmp_d;
-    Scratch<int32_t> cnt, raw, tmp, big;
-    Scratch<int64_t> off;
-    Scratch<unsigned long long> n_big;
-    GPL_TRY(cnt.get(ctx, (size_t)n));
-    GPL_TRY(off.get(ctx, (size_t)n + 2));
-    GPL_TRY(count(cnt.p));
-    GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n, off.p, off.p + n + 1)));
-    int64_t total = 0;
-    GPL_CUDA(cudaMemcpyAsync(&total, off.p + n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+// The pair list of n left rows from each row's right rows raw[off[i] .. off[i + 1]) (distinct, in any order; with raw_d,
+// their distances), total of them: lhs / rhs (/ dist) allocated and each row's pairs sorted by rhs (k_sort_rows_*), so the
+// list is sorted by (lhs, rhs) whatever the order of raw.  raw and raw_d are overwritten.  with_dist and no raw_d: dist is
+// allocated for the caller to fill.
+static int sorted_pairs(gpl_ctx *ctx, int64_t n, const int64_t *off, int32_t *raw, double *raw_d, int64_t total, bool with_dist, Pairs &out) {
+    GPL_TRY(pairs_new(ctx, total, with_dist, out));
     if (total == 0) return GPL_OK;
-    GPL_TRY(raw.get(ctx, (size_t)total));
-    if (with_dist) GPL_TRY(raw_d.get(ctx, (size_t)total));
-    GPL_TRY(write(off.p, raw.p, raw_d.p));
-    void *pl = nullptr, *pr = nullptr, *pd = nullptr;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pl));
-    res->lhs = (uint64_t *)pl;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &pr));
-    res->rhs = (uint64_t *)pr;
-    if (with_dist) {
-        GPL_TRY(ctx->alloc(sizeof(double) * (size_t)total, &pd));
-        res->dist = (double *)pd;
-    }
-    res->n = total;
+    double *dist = raw_d ? out->dist : nullptr;
+    Scratch<double> tmp_d;
+    Scratch<int32_t> tmp, big;
+    Scratch<unsigned long long> n_big;
     // segments of more than kSortSmall pairs: at most total / (kSortSmall + 1) of them
     GPL_TRY(big.get(ctx, (size_t)(total / (kSortSmall + 1) + 1)));
     GPL_TRY(n_big.get(ctx, 1));
     GPL_CUDA(cudaMemsetAsync(n_big.p, 0, sizeof(unsigned long long), ctx->stream));
-    GPL_LAUNCH(ctx, k_sort_rows_small, warp_grid(n, 8), 256, 0, n, off.p, raw.p, raw_d.p, res->lhs, res->rhs, res->dist, big.p, n_big.p);
+    GPL_LAUNCH(ctx, k_sort_rows_small, warp_grid(n, 8), 256, 0, n, off, raw, raw_d, out->lhs, out->rhs, dist, big.p, n_big.p);
     unsigned long long h_big = 0;
     GPL_CUDA(cudaMemcpyAsync(&h_big, n_big.p, sizeof(h_big), cudaMemcpyDeviceToHost, ctx->stream));
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));
     if (h_big > 0) {
         GPL_TRY(tmp.get(ctx, (size_t)total));
-        if (with_dist) GPL_TRY(tmp_d.get(ctx, (size_t)total));
+        if (raw_d) GPL_TRY(tmp_d.get(ctx, (size_t)total));
         GPL_LAUNCH(ctx, k_sort_rows_large, (int)std::min<int64_t>((int64_t)h_big, (int64_t)kSMs * 8), kSortRadixThreads, 0, big.p,
-                   (int64_t)h_big, off.p, raw.p, raw_d.p, tmp.p, tmp_d.p, res->lhs, res->rhs, res->dist);
+                   (int64_t)h_big, off, raw, raw_d, tmp.p, tmp_d.p, out->lhs, out->rhs, dist);
     }
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
     return GPL_OK;
 }
+
+// A pair list of n left rows: count(cnt) writes each left row's number of pairs, a scan turns the counts into int64 offsets,
+// write(off, raw, raw_d) writes each row's right rows (and, when raw_d != NULL, their distances) at its offsets in any order,
+// and sorted_pairs orders them.  *out is set only on success.
+template <class Count, class Write>
+static int pair_list(gpl_ctx *ctx, int64_t n, bool with_dist, gpl_pairs **out, Count &&count, Write &&write) {
+    Scratch<double> raw_d;
+    Scratch<int32_t> cnt, raw;
+    Scratch<int64_t> off;
+    int64_t total = 0;
+    if (n > 0) {
+        GPL_TRY(cnt.get(ctx, (size_t)n));
+        GPL_TRY(off.get(ctx, (size_t)n + 2));
+        GPL_TRY(count(cnt.p));
+        GPL_TRY((exclusive_scan<int32_t, int64_t>(ctx, cnt.p, n, off.p, off.p + n + 1)));
+        GPL_CUDA(cudaMemcpyAsync(&total, off.p + n + 1, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+        GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    if (total > 0) {
+        GPL_TRY(raw.get(ctx, (size_t)total));
+        if (with_dist) GPL_TRY(raw_d.get(ctx, (size_t)total));
+        GPL_TRY(write(off.p, raw.p, raw_d.p));
+    }
+    Pairs res(nullptr, gpl_pairs_free);
+    GPL_TRY(sorted_pairs(ctx, n, off.p, raw.p, raw_d.p, total, with_dist, res));
+    *out = res.release();
+    return GPL_OK;
+}
+
+// in's pairs with keep[k] set, in their order (so still sorted), into out.  With goff (n + 1 geometry offsets of in's rows),
+// ogoff receives the kept rows' offsets and goff[n] after them.  k_pairs.cu.
+int keep_pairs(gpl_ctx *ctx, const gpl_pairs *in, const uint8_t *keep, Pairs &out, const int64_t *goff = nullptr, Scratch<int64_t> *ogoff = nullptr);
 
 }  // namespace gpl

@@ -266,38 +266,11 @@ static BOperands operands(const gpl_array *a, const RingPrep &pa, const gpl_arra
     return o;
 }
 
-// the candidate pairs grouped by left row for pair_list (join_host.cuh), which sorts each row's right rows
-__global__ void __launch_bounds__(256) k_cand_count(int64_t n, const uint64_t *__restrict__ l, int32_t *__restrict__ cnt) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) atomicAdd(&cnt[l[i]], 1);
-}
-__global__ void __launch_bounds__(256) k_cand_write(int64_t n, const uint64_t *__restrict__ l, const uint64_t *__restrict__ r,
-                                                    const int64_t *__restrict__ off, int32_t *__restrict__ cursor, int32_t *__restrict__ raw) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride)
-        raw[off[l[i]] + atomicAdd(&cursor[l[i]], 1)] = (int32_t)r[i];
-}
-
 // keep[k] = 1 when row k of the join's output has a member
 __global__ void __launch_bounds__(256) k_nonempty(int64_t n, const int64_t *__restrict__ members, uint8_t *__restrict__ keep) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) keep[i] = members[i] > 0;
 }
-// the kept pairs and the geometry offsets of their rows (the parts, rings and coordinates of the empty rows are empty)
-__global__ void __launch_bounds__(256) k_compact_pairs(int64_t n, const uint8_t *__restrict__ keep, const int64_t *__restrict__ pos,
-                                                       const uint64_t *__restrict__ l, const uint64_t *__restrict__ r,
-                                                       const int64_t *__restrict__ goff, uint64_t *__restrict__ ol, uint64_t *__restrict__ orr,
-                                                       int64_t *__restrict__ ogoff) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= n; i += stride) {
-        if (i == n) {
-            ogoff[pos[n]] = goff[n];
-        } else if (keep[i]) {
-            ol[pos[i]] = l[i], orr[pos[i]] = r[i], ogoff[pos[i]] = goff[i];
-        }
-    }
-}
-
 }  // namespace gpl
 
 using namespace gpl;
@@ -319,66 +292,30 @@ extern "C" int gpl_boolean_op(gpl_ctx *ctx, const gpl_array *a, const gpl_array 
 
 extern "C" int gpl_overlay_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **pairs, gpl_array **out) {
     GPL_REQUIRE(ctx && lhs && rhs && pairs && out, GPL_ERR_INVALID_ARG, "gpl_overlay_join: NULL argument");
+    *pairs = nullptr, *out = nullptr;
     GPL_REQUIRE(is_area(lhs->type) && is_area(rhs->type), GPL_ERR_INVALID_TYPE, "Expected (Multi)Polygon x (Multi)Polygon (found %s x %s)",
                 type_name(lhs->type), type_name(rhs->type));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t nl = lhs->n_geoms, nr = rhs->n_geoms;
     GPL_REQUIRE(nl < (1LL << 31) && nr < (1LL << 31), GPL_ERR_UNSUPPORTED, "gpl_overlay_join: at most 2^31 rows per side");
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> cand(new gpl_pairs(), gpl_pairs_free);
-    cand->ctx = ctx;
-    if (nl > 0 && nr > 0) GPL_TRY(join_candidate_pairs(ctx, lhs, rhs, JOIN_INTERSECTS, "gpl_overlay_join", cand.get()));
-    // the candidates in (lhs, rhs) order (their order from the candidate stage is unspecified)
-    gpl_pairs *sorted_raw = nullptr;
-    const int64_t nc = cand->n;
-    const int cg = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(nc, 256), (int64_t)kSMs * 16));
-    Scratch<int32_t> cursor;
-    GPL_TRY(cursor.get(ctx, (size_t)nl));
-    GPL_TRY(pair_list(
-        ctx, nl, false, &sorted_raw,
-        [&](int32_t *cnt) -> int {
-            GPL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (size_t)nl, ctx->stream));
-            if (nc > 0) GPL_LAUNCH(ctx, k_cand_count, cg, 256, 0, nc, cand->lhs, cnt);
-            return GPL_OK;
-        },
-        [&](const int64_t *off, int32_t *raw, double *) -> int {
-            GPL_CUDA(cudaMemsetAsync(cursor.p, 0, sizeof(int32_t) * (size_t)nl, ctx->stream));
-            GPL_LAUNCH(ctx, k_cand_write, cg, 256, 0, nc, cand->lhs, cand->rhs, off, cursor.p, raw);
-            return GPL_OK;
-        }));
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> sorted(sorted_raw, gpl_pairs_free);
-    const int64_t n = sorted->n;
-    const uint64_t *sl = sorted->lhs, *sr = sorted->rhs;
-    cand.reset();
+    Pairs cand(nullptr, gpl_pairs_free);
+    GPL_TRY(join_candidate_pairs(ctx, lhs, rhs, JOIN_INTERSECTS, "gpl_overlay_join", false, cand));
+    const int64_t n = cand->n;
     RingPrep pl, pr;
     GPL_TRY(ring_prep(ctx, lhs, pl));
     GPL_TRY(ring_prep(ctx, rhs, pr));
     gpl_array *all = nullptr;
     Scratch<int64_t> members;
-    GPL_TRY(boolean_rows(ctx, operands(lhs, pl, rhs, pr), n, sl, sr, GPL_BOOLEAN_INTERSECTION, &all, &members));
+    GPL_TRY(boolean_rows(ctx, operands(lhs, pl, rhs, pr), n, cand->lhs, cand->rhs, GPL_BOOLEAN_INTERSECTION, &all, &members));
     std::unique_ptr<gpl_array, void (*)(gpl_array *)> geo(all, gpl_array_free);
     // drop the pairs whose intersection has no member (touching pairs)
     Scratch<uint8_t> keep;
-    Scratch<int64_t> pos, goff;
+    Scratch<int64_t> goff;
     GPL_TRY(keep.get(ctx, (size_t)n));
-    GPL_TRY(pos.get(ctx, (size_t)n + 1));
-    const int g = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n + 1, 256), (int64_t)kSMs * 16));
-    if (n > 0) GPL_LAUNCH(ctx, k_nonempty, g, 256, 0, n, members.p, keep.p);
-    GPL_TRY((exclusive_scan<uint8_t, int64_t>(ctx, keep.p, n, pos.p, nullptr)));
-    int64_t m = 0;
-    GPL_CUDA(cudaMemcpyAsync(&m, pos.p + n, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> res(new gpl_pairs(), gpl_pairs_free);
-    res->ctx = ctx;
-    res->n = m;
-    GPL_TRY(goff.get(ctx, (size_t)m + 1));
-    if (m > 0) {
-        void *pl_ = nullptr, *pr_ = nullptr;
-        GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)m, &pl_));
-        res->lhs = (uint64_t *)pl_;
-        GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)m, &pr_));
-        res->rhs = (uint64_t *)pr_;
-    }
-    GPL_LAUNCH(ctx, k_compact_pairs, g, 256, 0, n, keep.p, pos.p, sl, sr, all->geom_off, res->lhs, res->rhs, goff.p);
+    if (n > 0) GPL_LAUNCH(ctx, k_nonempty, flat_grid(n), 256, 0, n, members.p, keep.p);
+    Pairs res(nullptr, gpl_pairs_free);
+    GPL_TRY(keep_pairs(ctx, cand.get(), keep.p, res, all->geom_off, &goff));
+    const int64_t m = res->n;
     // every output row is valid: a null or non-finite pair has no member and is dropped
     Scratch<uint8_t> bm;
     GPL_TRY(bm.get(ctx, (size_t)(m + 7) / 8));

@@ -23,7 +23,6 @@
 #include <math.h>
 
 #include <algorithm>
-#include <memory>
 
 #include "boolean.cuh"
 #include "common.cuh"
@@ -425,8 +424,6 @@ __global__ void __launch_bounds__(256) k_dis_valid(int64_t ng, const uint8_t *__
     for (int64_t g = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; g < ng; g += stride) rv[g] = gnull[g] ? 0 : 1;
 }
 
-static int flat_grid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)kSMs * 16)); }
-
 }  // namespace gpl
 
 using namespace gpl;
@@ -476,9 +473,8 @@ extern "C" int gpl_dissolve(gpl_ctx *ctx, const gpl_array *in, const int64_t *gr
     GPL_CUDA(cudaMemsetAsync(gnull.p, 0, (size_t)ng, ctx->stream));
     if (n > 0) GPL_LAUNCH(ctx, k_dis_rows, warp_grid(n, 4), 128, 0, n, pr.view, pr.members, in->validity, grp, status.p, gnull.p, ring_row.p);
     // partners: the intersecting pairs of present rows of one group, per row, sorted
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> cand(new gpl_pairs(), gpl_pairs_free);
-    cand->ctx = ctx;
-    if (n > 1) GPL_TRY(join_candidate_pairs(ctx, in, in, JOIN_INTERSECTS, "gpl_dissolve", cand.get()));
+    Pairs cand(nullptr, gpl_pairs_free);
+    GPL_TRY(join_candidate_pairs(ctx, in, in, JOIN_INTERSECTS, "gpl_dissolve", false, cand));
     const int64_t nc = cand->n;
     Scratch<int32_t> cursor;
     GPL_TRY(cursor.get(ctx, (size_t)std::max(n, ng)));
@@ -495,7 +491,7 @@ extern "C" int gpl_dissolve(gpl_ctx *ctx, const gpl_array *in, const int64_t *gr
             GPL_LAUNCH(ctx, k_dis_pair_write, flat_grid(nc), 256, 0, nc, cand->lhs, cand->rhs, status.p, grp, off, cursor.p, raw);
             return GPL_OK;
         }));
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> plist(plist_raw, gpl_pairs_free);
+    Pairs plist(plist_raw, gpl_pairs_free);
     cand.reset();
     Scratch<int64_t> poff;
     GPL_TRY(poff.get(ctx, (size_t)n + 1));
@@ -514,7 +510,7 @@ extern "C" int gpl_dissolve(gpl_ctx *ctx, const gpl_array *in, const int64_t *gr
             GPL_LAUNCH(ctx, k_dis_group_write, flat_grid(n), 256, 0, n, status.p, grp, off, cursor.p, raw);
             return GPL_OK;
         }));
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> glist(glist_raw, gpl_pairs_free);
+    Pairs glist(glist_raw, gpl_pairs_free);
     const int64_t m = glist->n;
     const uint64_t *prow = glist->rhs;
     Scratch<int64_t> gpos, icnt, ib, tot;

@@ -475,6 +475,7 @@ extern "C" int gpl_geo_dwithin_count(gpl_ctx *ctx, const gpl_geo_index *idx, con
 extern "C" int gpl_geo_dwithin_join_pairs(gpl_ctx *ctx, const gpl_geo_index *idx, const gpl_array *lhs, double distance, int with_distance,
                                           gpl_pairs **out) {
     GPL_REQUIRE(ctx && idx && lhs && out, GPL_ERR_INVALID_ARG, "gpl_geo_dwithin_join_pairs: NULL argument");
+    *out = nullptr;
     GPL_TRY(check_geo_left(lhs, "great-circle dwithin join"));
     GPL_TRY(check_geo_distance(distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
@@ -499,6 +500,7 @@ extern "C" int gpl_geo_nearest_join(gpl_ctx *ctx, const gpl_geo_index *idx, cons
 extern "C" int gpl_geo_nearest_join_pairs(gpl_ctx *ctx, const gpl_geo_index *idx, const gpl_array *lhs, double max_distance, gpl_pairs **out,
                                           double *distance, int mem) {
     GPL_REQUIRE(ctx && idx && lhs && out, GPL_ERR_INVALID_ARG, "gpl_geo_nearest_join_pairs: NULL argument");
+    *out = nullptr;
     GPL_TRY(check_geo_left(lhs, "great-circle nearest join"));
     GPL_TRY(check_geo_max_distance(max_distance));
     GPL_CUDA(cudaSetDevice(ctx->device));

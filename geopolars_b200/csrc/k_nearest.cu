@@ -1117,6 +1117,7 @@ extern "C" int gpl_nearest_join_array(gpl_ctx *ctx, const gpl_nearest_index *idx
 extern "C" int gpl_nearest_join_pairs_array(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *points, double max_distance,
                                             gpl_pairs **out, double *distance, int mem) {
     GPL_REQUIRE(ctx && idx && points && out, GPL_ERR_INVALID_ARG, "gpl_nearest_join_pairs_array: NULL argument");
+    *out = nullptr;
     GPL_REQUIRE(points->type == GPL_POINT, GPL_ERR_INVALID_TYPE, "nearest join: the left side must be Point (found %s)",
                 type_name(points->type));
     GPL_TRY(check_query(points->n_geoms, max_distance));
@@ -1155,6 +1156,7 @@ extern "C" int gpl_nearest_join_geom(gpl_ctx *ctx, const gpl_nearest_index *idx,
 extern "C" int gpl_nearest_join_geom_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double max_distance,
                                            gpl_pairs **out, double *distance, int mem) {
     GPL_REQUIRE(ctx && idx && lhs && out, GPL_ERR_INVALID_ARG, "gpl_nearest_join_geom_pairs: NULL argument");
+    *out = nullptr;
     GPL_TRY(check_geom_left(lhs, max_distance));
     if (lhs->type == GPL_POINT) return gpl_nearest_join_pairs_array(ctx, idx, lhs, max_distance, out, distance, mem);
     GPL_CUDA(cudaSetDevice(ctx->device));
@@ -1197,6 +1199,7 @@ extern "C" int gpl_dwithin_count(gpl_ctx *ctx, const gpl_nearest_index *idx, con
 extern "C" int gpl_dwithin_join_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int with_distance,
                                       gpl_pairs **out) {
     GPL_REQUIRE(ctx && idx && lhs && out, GPL_ERR_INVALID_ARG, "gpl_dwithin_join_pairs: NULL argument");
+    *out = nullptr;
     GPL_TRY(check_dwithin(lhs, distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
     RowClasses lc;

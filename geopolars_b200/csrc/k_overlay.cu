@@ -20,8 +20,6 @@
 // row-wise value bit for bit.  Per-ring σ and boxes come from a pre-pass (k_ring_prep) over each column.
 #include <math.h>
 
-#include <memory>
-
 #include "common.cuh"
 #include "join_grid.cuh"
 #include "overlay.cuh"
@@ -267,19 +265,15 @@ extern "C" int gpl_intersection_area(gpl_ctx *ctx, const gpl_array *a, const gpl
 
 extern "C" int gpl_overlay_area_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **out) {
     GPL_REQUIRE(ctx && lhs && rhs && out, GPL_ERR_INVALID_ARG, "gpl_overlay_area_join: NULL argument");
+    *out = nullptr;
     GPL_REQUIRE(is_area(lhs->type) && is_area(rhs->type), GPL_ERR_INVALID_TYPE, "Expected (Multi)Polygon x (Multi)Polygon (found %s x %s)",
                 type_name(lhs->type), type_name(rhs->type));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t nl = lhs->n_geoms, nr = rhs->n_geoms;
     GPL_REQUIRE(nl < (1LL << 31) && nr < (1LL << 31), GPL_ERR_UNSUPPORTED, "gpl_overlay_area_join: at most 2^31 rows per side");
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> res(new gpl_pairs(), gpl_pairs_free);
-    res->ctx = ctx;
-    res->with_dist = true;
-    if (nl > 0 && nr > 0) GPL_TRY(join_candidate_pairs(ctx, lhs, rhs, JOIN_INTERSECTS, "gpl_overlay_area_join", res.get()));
+    Pairs res(nullptr, gpl_pairs_free);
+    GPL_TRY(join_candidate_pairs(ctx, lhs, rhs, JOIN_INTERSECTS, "gpl_overlay_area_join", true, res));
     if (res->n > 0) {
-        void *pd = nullptr;
-        GPL_TRY(ctx->alloc(sizeof(double) * (size_t)res->n, &pd));
-        res->dist = (double *)pd;
         RingPrep pl, pr;
         GPL_TRY(ring_prep(ctx, lhs, pl));
         GPL_TRY(ring_prep(ctx, rhs, pr));

@@ -29,6 +29,7 @@
 
 #include "common.cuh"
 #include "join_grid.cuh"
+#include "join_host.cuh"
 #include "pair_dist.cuh"
 #include "point_dist.cuh"
 #include "scan.cuh"
@@ -650,8 +651,10 @@ extern "C" int gpl_distance(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b
 // the rows whose envelope overlaps it; one thread per LEFT row walks the cells its envelope overlaps and keeps the
 // candidates whose envelope intersects (each pair is reported from the single cell that holds the lower-left corner of
 // the intersection box); count -> scan -> write gives the candidate list, a warp per candidate evaluates the
-// dispatched predicate, and a second scan compacts the hits.  Points x (Multi)Polygons with millions of points should
-// use gpl_pip_index_build + gpl_contains_join (the north-star path); this entry point is the general one.
+// dispatched predicate, and a second scan compacts the hits.  The compaction keeps them grouped by left row, so a sort of
+// each row's right rows (sorted_pairs, join_host.cuh) puts the list in (lhs, rhs) order.  Points x (Multi)Polygons with
+// millions of points should use gpl_pip_index_build + gpl_contains_join (the north-star path); this entry point is the
+// general one.
 // JoinGrid, jg_cell and the grid build (join_grid_build): join_grid.cuh; struct gpl_pairs: common.cuh
 namespace gpl {
 
@@ -689,18 +692,25 @@ __global__ void k_join_candidates(const double *__restrict__ l4, const uint8_t *
     }
     if (PASS == 0) counts[i] = cnt;
 }
-__global__ void k_join_compact(const uint8_t *__restrict__ hit, const int64_t *__restrict__ off, int64_t n, const uint64_t *__restrict__ cl,
-                               const uint64_t *__restrict__ cr, uint64_t *__restrict__ ol, uint64_t *__restrict__ orr) {
-    const int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (k < n && hit[k]) ol[off[k]] = cl[k], orr[off[k]] = cr[k];
+// the right rows of the hits, in candidate order, and the first hit of each left row: row i's candidates are
+// [cand_off[i], cand_off[i + 1]) and the compaction keeps their order, so its hits are [row_off[i], row_off[i + 1])
+__global__ void __launch_bounds__(256) k_join_hits(int64_t n_cand, const uint8_t *__restrict__ hit, const int64_t *__restrict__ hit_off,
+                                                   const uint64_t *__restrict__ cr, int32_t *__restrict__ raw, int64_t nl,
+                                                   const int64_t *__restrict__ cand_off, int64_t *__restrict__ row_off) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n_cand || k <= nl; k += stride) {
+        if (k < n_cand && hit[k]) raw[hit_off[k]] = (int32_t)cr[k];
+        if (k <= nl) row_off[k] = hit_off[cand_off[k]];
+    }
 }
 
 // The candidate stage of the general join: envelopes of both sides, the grid over the right side's union box, the
-// candidate list (count -> scan -> write), the exact test `test` per candidate and the compaction of the hits into res
-// (lhs / rhs, in candidate order).  res stays empty when nothing matches.
-int join_candidate_pairs(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, JoinTest test, const char *who, gpl_pairs *res) {
+// candidate list (count -> scan -> write), the exact test `test` per candidate, the compaction of the hits and their sort
+// by (lhs, rhs) (sorted_pairs, join_host.cuh) into out.
+int join_candidate_pairs(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, JoinTest test, const char *who, bool with_dist, Pairs &out) {
     const int64_t nl = lhs->n_geoms, nr = rhs->n_geoms;
     const int tl = lhs->type, tr = rhs->type;
+    if (nl == 0 || nr == 0) return pairs_new(ctx, 0, with_dist, out);
     // ---- envelopes -----------------------------------------------------------------------------------------------------
     Scratch<double> l4, r4;
     Scratch<uint8_t> lh, rh;
@@ -713,7 +723,7 @@ int join_candidate_pairs(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rh
     // ---- grid over the right side's union box ------------------------------------------------------------------------------
     GridBuild grid;
     GPL_TRY(join_grid_build(ctx, r4.p, rh.p, nr, nr, who, grid));
-    if (grid.jg.g == 0) return GPL_OK;  // no right row has an envelope
+    if (grid.jg.g == 0) return pairs_new(ctx, 0, with_dist, out);  // no right row has an envelope
     // ---- candidates: count -> scan -> write ----------------------------------------------------------------------------------
     Scratch<int32_t> cand_count;
     Scratch<int64_t> tot, cand_off;
@@ -726,7 +736,7 @@ int join_candidate_pairs(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rh
     int64_t n_cand = 0;
     GPL_CUDA(cudaMemcpyAsync(&n_cand, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (n_cand == 0) return GPL_OK;
+    if (n_cand == 0) return pairs_new(ctx, 0, with_dist, out);
     Scratch<uint64_t> cl, cr;
     GPL_TRY(cl.get(ctx, (size_t)n_cand));
     GPL_TRY(cr.get(ctx, (size_t)n_cand));
@@ -747,22 +757,47 @@ int join_candidate_pairs(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rh
         break;
     default: GPL_LAUNCH(ctx, k_intersects_pairs, pgrid, 256, 0, n_cand, sl, lhs->validity, sr, rhs->validity, cl.p, cr.p, hit.p); break;
     }
-    // ---- compaction ----------------------------------------------------------------------------------------------------------------
-    Scratch<int64_t> hit_off;
+    // ---- compaction and per-row sort ---------------------------------------------------------------------------------------------
+    Scratch<int64_t> hit_off, row_off;
     GPL_TRY(hit_off.get(ctx, (size_t)n_cand + 2));
     GPL_TRY((exclusive_scan<uint8_t, int64_t>(ctx, hit.p, n_cand, hit_off.p, tot.p)));
     int64_t n_hit = 0;
     GPL_CUDA(cudaMemcpyAsync(&n_hit, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (n_hit == 0) return GPL_OK;
-    void *pl = nullptr, *pr = nullptr;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)n_hit, &pl));
-    res->lhs = (uint64_t *)pl;
-    GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)n_hit, &pr));
-    res->rhs = (uint64_t *)pr;
-    res->n = n_hit;
-    GPL_LAUNCH(ctx, k_join_compact, (int)ceil_div(n_cand, 256), 256, 0, hit.p, hit_off.p, n_cand, cl.p, cr.p, res->lhs, res->rhs);
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch lists above return to the cache when this scope ends
+    if (n_hit == 0) return pairs_new(ctx, 0, with_dist, out);
+    Scratch<int32_t> raw;
+    GPL_TRY(raw.get(ctx, (size_t)n_hit));
+    GPL_TRY(row_off.get(ctx, (size_t)nl + 1));
+    GPL_LAUNCH(ctx, k_join_hits, flat_grid(std::max(n_cand, nl + 1)), 256, 0, n_cand, hit.p, hit_off.p, cr.p, raw.p, nl, cand_off.p, row_off.p);
+    return sorted_pairs(ctx, nl, row_off.p, raw.p, nullptr, n_hit, with_dist, out);
+}
+
+// the order-preserving compaction of keep_pairs (join_host.cuh): pair i (with goff, also its row's offset) to pos[i]
+__global__ void __launch_bounds__(256) k_keep_pairs(int64_t n, const uint8_t *__restrict__ keep, const int64_t *__restrict__ pos,
+                                                    const uint64_t *__restrict__ l, const uint64_t *__restrict__ r, uint64_t *__restrict__ ol,
+                                                    uint64_t *__restrict__ orr, const int64_t *__restrict__ goff, int64_t *__restrict__ ogoff) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i <= n; i += stride) {
+        if (i == n) {
+            if (goff) ogoff[pos[n]] = goff[n];
+        } else if (keep[i]) {
+            ol[pos[i]] = l[i], orr[pos[i]] = r[i];
+            if (goff) ogoff[pos[i]] = goff[i];
+        }
+    }
+}
+int keep_pairs(gpl_ctx *ctx, const gpl_pairs *in, const uint8_t *keep, Pairs &out, const int64_t *goff, Scratch<int64_t> *ogoff) {
+    const int64_t n = in->n;
+    Scratch<int64_t> pos;
+    GPL_TRY(pos.get(ctx, (size_t)n + 1));
+    GPL_TRY((exclusive_scan<uint8_t, int64_t>(ctx, keep, n, pos.p, nullptr)));
+    int64_t m = 0;
+    GPL_CUDA(cudaMemcpyAsync(&m, pos.p + n, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    GPL_TRY(pairs_new(ctx, m, false, out));
+    if (goff) GPL_TRY(ogoff->get(ctx, (size_t)m + 1));
+    GPL_LAUNCH(ctx, k_keep_pairs, flat_grid(n + 1), 256, 0, n, keep, pos.p, in->lhs, in->rhs, out->lhs, out->rhs, goff, goff ? ogoff->p : nullptr);
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // pos returns to the cache when this scope ends
     return GPL_OK;
 }
 
@@ -816,23 +851,22 @@ extern "C" int gpl_contains_polygon(gpl_ctx *ctx, const gpl_array *a, const gpl_
 
 extern "C" int gpl_spatial_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, int predicate, gpl_pairs **out) {
     GPL_REQUIRE(ctx && lhs && rhs && out, GPL_ERR_INVALID_ARG, "gpl_spatial_join: NULL argument");
+    *out = nullptr;
     GPL_REQUIRE(predicate == GPL_PREDICATE_INTERSECTS || predicate == GPL_PREDICATE_CONTAINS, GPL_ERR_INVALID_ARG,
                 "gpl_spatial_join: predicate must be GPL_PREDICATE_INTERSECTS or GPL_PREDICATE_CONTAINS");
     GPL_CUDA(cudaSetDevice(ctx->device));
-    gpl_pairs *res = new gpl_pairs();
-    res->ctx = ctx;
-    *out = res;
     const int64_t nl = lhs->n_geoms, nr = rhs->n_geoms;
-    if (nl == 0 || nr == 0) return GPL_OK;
-    GPL_REQUIRE(nl < (1LL << 31) && nr < (1LL << 31), GPL_ERR_UNSUPPORTED, "gpl_spatial_join: at most 2^31 rows per side");
+    GPL_REQUIRE(nl == 0 || nr == 0 || (nl < (1LL << 31) && nr < (1LL << 31)), GPL_ERR_UNSUPPORTED, "gpl_spatial_join: at most 2^31 rows per side");
     // ---- the type-pair dispatch table of spatial_index.rs:89-137 (anything else: no pair matches) ------------------------
     const int tl = lhs->type, tr = rhs->type;
     const int cl_ = side_class_host(tl), cr_ = side_class_host(tr);
-    JoinTest test;
+    int test = -1;
     if (tl == GPL_POINT && (cr_ == 2 || tr == GPL_LINESTRING || tr == GPL_MULTILINESTRING)) test = JOIN_POINT_IN_R;       // :91, :95, :130-134
     else if (tr == GPL_POINT && (cl_ == 2 || tl == GPL_LINESTRING || tl == GPL_MULTILINESTRING)) test = JOIN_POINT_IN_L;  // :92, :96, :129-133
     else if ((tl == GPL_POLYGON || tl == GPL_MULTIPOLYGON) && tr == GPL_POLYGON) test = predicate == GPL_PREDICATE_CONTAINS ? JOIN_POLY_CONTAINS : JOIN_INTERSECTS;  // :99-115
     else if (tl == GPL_POLYGON && tr == GPL_MULTIPOLYGON && predicate == GPL_PREDICATE_INTERSECTS) test = JOIN_INTERSECTS;  // :118-122
-    else return GPL_OK;
-    return join_candidate_pairs(ctx, lhs, rhs, test, "gpl_spatial_join", res);
+    Pairs res(nullptr, gpl_pairs_free);
+    GPL_TRY(test < 0 ? pairs_new(ctx, 0, false, res) : join_candidate_pairs(ctx, lhs, rhs, (JoinTest)test, "gpl_spatial_join", false, res));
+    *out = res.release();
+    return GPL_OK;
 }

@@ -2545,24 +2545,20 @@ extern "C" int gpl_contains_join_pairs(gpl_ctx *ctx, const gpl_pip_index *idx, c
 // result of a join (struct gpl_pairs, common.cuh): the points-in-polygons join returns the same object as gpl_spatial_join
 extern "C" int gpl_contains_join_pairs_array(gpl_ctx *ctx, const gpl_pip_index *idx, const gpl_array *points, gpl_pairs **out) {
     GPL_REQUIRE(ctx && idx && points && out, GPL_ERR_INVALID_ARG, "gpl_contains_join_pairs_array: NULL argument");
+    *out = nullptr;
     GPL_REQUIRE(points->type == GPL_POINT, GPL_ERR_INVALID_TYPE, "Expected Point (found geometry type %d)", points->type);
     GPL_CUDA(cudaSetDevice(ctx->device));
-    gpl_pairs *res = new gpl_pairs();
-    res->ctx = ctx;
-    *out = res;
+    Pairs res(nullptr, gpl_pairs_free);
+    GPL_TRY(pairs_new(ctx, 0, false, res));
     const int64_t n = points->n_geoms;
-    if (n == 0) return GPL_OK;
-    GPL_TRY(pip_pairs(ctx, idx, points->xy, points->validity, n, [&](int64_t total, uint64_t **pl, uint64_t **pr) -> int {
-        if (total == 0) return GPL_OK;
-        void *q = nullptr;
-        GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &q));
-        res->lhs = *pl = (uint64_t *)q;
-        GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)total, &q));
-        res->rhs = *pr = (uint64_t *)q;
-        res->n = total;
-        return GPL_OK;
-    }));
+    if (n > 0)
+        GPL_TRY(pip_pairs(ctx, idx, points->xy, points->validity, n, [&](int64_t total, uint64_t **pl, uint64_t **pr) -> int {
+            GPL_TRY(pairs_new(ctx, total, false, res));
+            *pl = res->lhs, *pr = res->rhs;
+            return GPL_OK;
+        }));
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    *out = res.release();
     return GPL_OK;
 }
 

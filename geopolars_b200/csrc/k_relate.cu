@@ -18,8 +18,6 @@
 #include <math.h>
 #include <string.h>
 
-#include <memory>
-
 #include "common.cuh"
 #include "join_grid.cuh"
 #include "join_host.cuh"
@@ -29,11 +27,6 @@
 #include "sym_point.cuh"
 
 namespace gpl {
-
-// k_cand_count / k_cand_write: k_boolean.cu
-__global__ void k_cand_count(int64_t n, const uint64_t *__restrict__ l, int32_t *__restrict__ cnt);
-__global__ void k_cand_write(int64_t n, const uint64_t *__restrict__ l, const uint64_t *__restrict__ r, const int64_t *__restrict__ off,
-                             int32_t *__restrict__ cursor, int32_t *__restrict__ raw);
 
 // k_relate: 4 warps per CTA and 3 CTAs per SM cap it at 170 registers; at the default cap of 128 it spills (as k_overlap_area)
 constexpr int kRelateThreads = 128;
@@ -384,13 +377,6 @@ __global__ void __launch_bounds__(kRelateThreads, 3) k_relate(int64_t n, ROp a, 
         }
     }
 }
-__global__ void __launch_bounds__(256) k_pair_compact(int64_t n, const uint8_t *__restrict__ hit, const int64_t *__restrict__ pos,
-                                                      const uint64_t *__restrict__ l, const uint64_t *__restrict__ r, uint64_t *__restrict__ ol,
-                                                      uint64_t *__restrict__ orr) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride)
-        if (hit[i]) ol[pos[i]] = l[i], orr[pos[i]] = r[i];
-}
 
 // ---- host side --------------------------------------------------------------------------------------------------------
 static int cls_of(int t) {
@@ -525,6 +511,7 @@ extern "C" int gpl_relate_predicate(gpl_ctx *ctx, const gpl_array *a, const gpl_
 
 extern "C" int gpl_predicate_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, int predicate, const char *pattern, gpl_pairs **out) {
     GPL_REQUIRE(ctx && lhs && rhs && out, GPL_ERR_INVALID_ARG, "gpl_predicate_join: NULL argument");
+    *out = nullptr;
     GPL_TRY(check_pair(lhs, rhs, "predicate_join"));
     RelSpec spec;
     GPL_REQUIRE(make_spec(predicate, pattern, cls_of(lhs->type), cls_of(rhs->type), spec), GPL_ERR_INVALID_ARG,
@@ -540,33 +527,12 @@ extern "C" int gpl_predicate_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t nl = lhs->n_geoms, nr = rhs->n_geoms;
     GPL_REQUIRE(nl < (1LL << 31) && nr < (1LL << 31), GPL_ERR_UNSUPPORTED, "gpl_predicate_join: at most 2^31 rows per side");
-    *out = nullptr;
     // every accepted predicate implies intersects: the candidates are the pairs gpl_intersects accepts, in (lhs, rhs) order
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> cand(new gpl_pairs(), gpl_pairs_free);
-    cand->ctx = ctx;
-    if (nl > 0 && nr > 0 && !spec.never) GPL_TRY(join_candidate_pairs(ctx, lhs, rhs, JOIN_INTERSECTS, "gpl_predicate_join", cand.get()));
-    gpl_pairs *sorted_raw = nullptr;
-    const int64_t nc = cand->n;
-    const int cg = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(nc, 256), (int64_t)kSMs * 16));
-    Scratch<int32_t> cursor;
-    GPL_TRY(cursor.get(ctx, (size_t)nl));
-    GPL_TRY(pair_list(
-        ctx, nl, false, &sorted_raw,
-        [&](int32_t *cnt) -> int {
-            GPL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (size_t)nl, ctx->stream));
-            if (nc > 0) GPL_LAUNCH(ctx, k_cand_count, cg, 256, 0, nc, cand->lhs, cnt);
-            return GPL_OK;
-        },
-        [&](const int64_t *off, int32_t *raw, double *) -> int {
-            GPL_CUDA(cudaMemsetAsync(cursor.p, 0, sizeof(int32_t) * (size_t)nl, ctx->stream));
-            GPL_LAUNCH(ctx, k_cand_write, cg, 256, 0, nc, cand->lhs, cand->rhs, off, cursor.p, raw);
-            return GPL_OK;
-        }));
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> sorted(sorted_raw, gpl_pairs_free);
-    cand.reset();
-    const int64_t n = sorted->n;
+    Pairs cand(nullptr, gpl_pairs_free);
+    GPL_TRY(spec.never ? pairs_new(ctx, 0, false, cand) : join_candidate_pairs(ctx, lhs, rhs, JOIN_INTERSECTS, "gpl_predicate_join", false, cand));
+    const int64_t n = cand->n;
     if (predicate == GPL_PREDICATE_INTERSECTS || n == 0) {
-        *out = sorted.release();
+        *out = cand.release();
         return GPL_OK;
     }
     RingPrep pl, pr;
@@ -574,26 +540,10 @@ extern "C" int gpl_predicate_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_
     GPL_TRY(make_op(ctx, lhs, pl, ol));
     GPL_TRY(make_op(ctx, rhs, pr, orr));
     Scratch<uint8_t> hit;
-    Scratch<int64_t> pos;
     GPL_TRY(hit.get(ctx, (size_t)n));
-    GPL_TRY(pos.get(ctx, (size_t)n + 1));
-    GPL_LAUNCH(ctx, k_relate, warp_grid(n, kRelateThreads / 32), kRelateThreads, 0, n, ol, orr, sorted->lhs, sorted->rhs, spec, nullptr, nullptr, hit.p);
-    GPL_TRY((exclusive_scan<uint8_t, int64_t>(ctx, hit.p, n, pos.p, nullptr)));
-    int64_t m = 0;
-    GPL_CUDA(cudaMemcpyAsync(&m, pos.p + n, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    std::unique_ptr<gpl_pairs, void (*)(gpl_pairs *)> res(new gpl_pairs(), gpl_pairs_free);
-    res->ctx = ctx;
-    res->n = m;
-    if (m > 0) {
-        void *a_ = nullptr, *b_ = nullptr;
-        GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)m, &a_));
-        res->lhs = (uint64_t *)a_;
-        GPL_TRY(ctx->alloc(sizeof(uint64_t) * (size_t)m, &b_));
-        res->rhs = (uint64_t *)b_;
-        GPL_LAUNCH(ctx, k_pair_compact, cg, 256, 0, n, hit.p, pos.p, sorted->lhs, sorted->rhs, res->lhs, res->rhs);
-    }
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
+    GPL_LAUNCH(ctx, k_relate, warp_grid(n, kRelateThreads / 32), kRelateThreads, 0, n, ol, orr, cand->lhs, cand->rhs, spec, nullptr, nullptr, hit.p);
+    Pairs res(nullptr, gpl_pairs_free);
+    GPL_TRY(keep_pairs(ctx, cand.get(), hit.p, res));
     *out = res.release();
     return GPL_OK;
 }

@@ -452,9 +452,7 @@ def overlay_area_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, n
     `intersection_area` returns for it"""
     h = C.c_void_p()
     check(lhs.ctx.lib.gpl_overlay_area_join(lhs.ctx._h, lhs._h, rhs._h, C.byref(h)))
-    a, b, d = _pairs_with_distance(lhs.ctx, h, True)
-    order = np.lexsort((b, a))
-    return a[order], b[order], d[order]
+    return _take_pairs(lhs.ctx, h, True)
 
 
 BOOLEAN_OPS = {"intersection": 0, "union": 1, "difference": 2}
@@ -476,14 +474,7 @@ def overlay_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, np.nda
     hp, ha = C.c_void_p(), C.c_void_p()
     check(ctx.lib.gpl_overlay_join(ctx._h, lhs._h, rhs._h, C.byref(hp), C.byref(ha)))
     geoms = DeviceArray(ctx, ha)
-    try:
-        n = int(ctx.lib.gpl_pairs_count(hp))
-        a = np.empty(n, dtype=np.uint64)
-        b = np.empty(n, dtype=np.uint64)
-        if n:
-            check(ctx.lib.gpl_pairs_copy(ctx._h, hp, _np_ptr(a), _np_ptr(b), GPL_HOST))
-    finally:
-        ctx.lib.gpl_pairs_free(hp)
+    a, b = _take_pairs(ctx, hp)
     return a, b, geoms
 
 
@@ -528,17 +519,20 @@ def contains(a: DeviceArray, b: DeviceArray) -> np.ndarray:
 PREDICATES = {"intersects": 0, "contains": 1}
 
 
-def _pairs_to_host(ctx: Context, h) -> Tuple[np.ndarray, np.ndarray]:
+def _take_pairs(ctx: Context, h, with_distance: bool = False):
+    """(lhs uint64, rhs uint64[, d float64]) of a pair list, sorted by (lhs, rhs) as every join returns it; frees it"""
     try:
         n = int(ctx.lib.gpl_pairs_count(h))
-        lhs = np.empty(n, dtype=np.uint64)
-        rhs = np.empty(n, dtype=np.uint64)
+        a = np.empty(n, dtype=np.uint64)
+        b = np.empty(n, dtype=np.uint64)
+        d = np.empty(n, dtype=np.float64) if with_distance else None
         if n:
-            check(ctx.lib.gpl_pairs_copy(ctx._h, h, _np_ptr(lhs), _np_ptr(rhs), GPL_HOST))
+            check(ctx.lib.gpl_pairs_copy(ctx._h, h, _np_ptr(a), _np_ptr(b), GPL_HOST))
+            if with_distance:
+                check(ctx.lib.gpl_pairs_copy_distance(ctx._h, h, _np_ptr(d), GPL_HOST))
     finally:
         ctx.lib.gpl_pairs_free(h)
-    order = np.lexsort((rhs, lhs))  # the reference's order is unspecified (tree traversal): sorted by (lhs, rhs) here
-    return lhs[order], rhs[order]
+    return (a, b, d) if with_distance else (a, b)
 
 
 def spatial_join(lhs: DeviceArray, rhs: DeviceArray, predicate: str = "intersects") -> Tuple[np.ndarray, np.ndarray]:
@@ -549,7 +543,7 @@ def spatial_join(lhs: DeviceArray, rhs: DeviceArray, predicate: str = "intersect
         raise ValueError("predicate must be 'intersects' or 'contains'")
     h = C.c_void_p()
     check(lhs.ctx.lib.gpl_spatial_join(lhs.ctx._h, lhs._h, rhs._h, p, C.byref(h)))
-    return _pairs_to_host(lhs.ctx, h)
+    return _take_pairs(lhs.ctx, h)
 
 
 def relate(a: DeviceArray, b: DeviceArray) -> Tuple[np.ndarray, np.ndarray]:
@@ -600,15 +594,7 @@ def predicate_join(lhs: DeviceArray, rhs: DeviceArray, predicate: str = "interse
         raise ValueError("predicate_join needs a pattern that requires contact (II, IB, BI or BB not F or *)")
     h = C.c_void_p()
     check(lhs.ctx.lib.gpl_predicate_join(lhs.ctx._h, lhs._h, rhs._h, code, pat, C.byref(h)))
-    try:
-        n = int(lhs.ctx.lib.gpl_pairs_count(h))
-        a = np.empty(n, dtype=np.uint64)
-        b = np.empty(n, dtype=np.uint64)
-        if n:
-            check(lhs.ctx.lib.gpl_pairs_copy(lhs.ctx._h, h, _np_ptr(a), _np_ptr(b), GPL_HOST))
-    finally:
-        lhs.ctx.lib.gpl_pairs_free(h)
-    return a, b
+    return _take_pairs(lhs.ctx, h)
 
 
 def geom_type(a: DeviceArray) -> np.ndarray:
@@ -775,7 +761,7 @@ class PipIndex:
         """the same pair list for a Point column that already lives in HBM (no host round trip of the points)"""
         h = C.c_void_p()
         check(self.ctx.lib.gpl_contains_join_pairs_array(self.ctx._h, self._h, points._h, C.byref(h)))
-        return _pairs_to_host(self.ctx, h)
+        return _take_pairs(self.ctx, h)
 
     def free(self) -> None:
         if getattr(self, "_h", None) and self.ctx._h:
@@ -846,7 +832,7 @@ class NearestIndex:
         dist = np.empty(len(points), dtype=np.float64) if with_distance else None
         check(self.ctx.lib.gpl_nearest_join_pairs_array(self.ctx._h, self._h, points._h, self._maxd(max_distance), C.byref(h), _np_ptr(dist),
                                                         GPL_HOST))
-        lhs, rhs = _pairs_to_host(self.ctx, h)
+        lhs, rhs = _take_pairs(self.ctx, h)
         return (lhs, rhs, dist) if with_distance else (lhs, rhs)
 
     def query_geom(self, lhs: DeviceArray, max_distance=None):
@@ -868,7 +854,7 @@ class NearestIndex:
         dist = np.empty(len(lhs), dtype=np.float64) if with_distance else None
         check(self.ctx.lib.gpl_nearest_join_geom_pairs(self.ctx._h, self._h, lhs._h, self._maxd(max_distance), C.byref(h), _np_ptr(dist),
                                                        GPL_HOST))
-        lhs_rows, rhs_rows = _pairs_to_host(self.ctx, h)
+        lhs_rows, rhs_rows = _take_pairs(self.ctx, h)
         return (lhs_rows, rhs_rows, dist) if with_distance else (lhs_rows, rhs_rows)
 
     def count_within(self, lhs: DeviceArray, distance: float) -> np.ndarray:
@@ -882,18 +868,7 @@ class NearestIndex:
         """every (left row, right row) pair within `distance`, once, sorted by (lhs, rhs): (lhs uint64, rhs uint64[, d float64])"""
         h = C.c_void_p()
         check(self.ctx.lib.gpl_dwithin_join_pairs(self.ctx._h, self._h, lhs._h, float(distance), int(bool(with_distance)), C.byref(h)))
-        try:
-            n = int(self.ctx.lib.gpl_pairs_count(h))
-            a = np.empty(n, dtype=np.uint64)
-            b = np.empty(n, dtype=np.uint64)
-            d = np.empty(n, dtype=np.float64)
-            if n:
-                check(self.ctx.lib.gpl_pairs_copy(self.ctx._h, h, _np_ptr(a), _np_ptr(b), GPL_HOST))
-                if with_distance:
-                    check(self.ctx.lib.gpl_pairs_copy_distance(self.ctx._h, h, _np_ptr(d), GPL_HOST))
-        finally:
-            self.ctx.lib.gpl_pairs_free(h)
-        return (a, b, d) if with_distance else (a, b)
+        return _take_pairs(self.ctx, h, with_distance)
 
     def free(self) -> None:
         if getattr(self, "_h", None) and self.ctx._h:
@@ -905,22 +880,6 @@ class NearestIndex:
             self.free()
         except Exception:
             pass
-
-
-def _pairs_with_distance(ctx: Context, h, with_distance: bool):
-    """(lhs uint64, rhs uint64, d float64 or None) of a sorted pair list; frees it"""
-    try:
-        n = int(ctx.lib.gpl_pairs_count(h))
-        a = np.empty(n, dtype=np.uint64)
-        b = np.empty(n, dtype=np.uint64)
-        d = np.empty(n, dtype=np.float64) if with_distance else None
-        if n:
-            check(ctx.lib.gpl_pairs_copy(ctx._h, h, _np_ptr(a), _np_ptr(b), GPL_HOST))
-            if with_distance:
-                check(ctx.lib.gpl_pairs_copy_distance(ctx._h, h, _np_ptr(d), GPL_HOST))
-    finally:
-        ctx.lib.gpl_pairs_free(h)
-    return a, b, d
 
 
 class GeoIndex:
@@ -952,8 +911,7 @@ class GeoIndex:
         """every (left row, right row) pair within `distance` metres, once, sorted by (lhs, rhs): (lhs uint64, rhs uint64[, d])"""
         h = C.c_void_p()
         check(self.ctx.lib.gpl_geo_dwithin_join_pairs(self.ctx._h, self._h, lhs._h, float(distance), int(bool(with_distance)), C.byref(h)))
-        a, b, d = _pairs_with_distance(self.ctx, h, with_distance)
-        return (a, b, d) if with_distance else (a, b)
+        return _take_pairs(self.ctx, h, with_distance)
 
     def query(self, lhs: DeviceArray, max_distance=None):
         """(nearest_id int32 (-1: none), distance float64 metres (NaN: none), n_tied int32) for a Point column in HBM;
@@ -972,7 +930,7 @@ class GeoIndex:
         dist = np.empty(len(lhs), dtype=np.float64) if with_distance else None
         check(self.ctx.lib.gpl_geo_nearest_join_pairs(self.ctx._h, self._h, lhs._h, NearestIndex._maxd(max_distance), C.byref(h), _np_ptr(dist),
                                                       GPL_HOST))
-        a, b, _ = _pairs_with_distance(self.ctx, h, False)
+        a, b = _take_pairs(self.ctx, h)
         return (a, b, dist) if with_distance else (a, b)
 
     def free(self) -> None:

@@ -432,14 +432,9 @@ def spatial_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", predicate: 
     a = a.astype(np.int64)
     b = b.astype(np.int64)
     if how == "left":
-        n = len(lhs)
-        matched = np.zeros(n, dtype=bool)
+        matched = np.zeros(len(lhs), dtype=bool)
         matched[a] = True
-        miss = np.nonzero(~matched)[0]
-        a = np.concatenate([a, miss])
-        b = np.concatenate([b, np.full(len(miss), -1, dtype=np.int64)])
-        order = np.lexsort((b, a))
-        a, b = a[order], b[order]
+        a, b = _left_rows(a, b, None, np.nonzero(~matched)[0])
     return a, b
 
 
@@ -467,11 +462,7 @@ def predicate_join(lhs: GeoSeries, rhs: GeoSeries, predicate: str = "intersects"
     if how == "left":
         matched = np.zeros(len(lhs), dtype=bool)
         matched[a] = True
-        miss = np.nonzero(~matched)[0]
-        a = np.concatenate([a, miss])
-        b = np.concatenate([b, np.full(len(miss), -1, dtype=np.int64)])
-        order = np.lexsort((b, a))
-        a, b = a[order], b[order]
+        a, b = _left_rows(a, b, None, np.nonzero(~matched)[0])
     return a, b
 
 
@@ -498,12 +489,7 @@ def nearest_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", max_distanc
     b = b.astype(np.int64)
     d = dist[a]
     if how == "left":
-        miss = np.nonzero(np.isnan(dist))[0]
-        a = np.concatenate([a, miss])
-        b = np.concatenate([b, np.full(len(miss), -1, dtype=np.int64)])
-        d = np.concatenate([d, np.full(len(miss), np.nan)])
-        order = np.lexsort((b, a))
-        a, b, d = a[order], b[order], d[order]
+        a, b, d = _left_rows(a, b, d, np.nonzero(np.isnan(dist))[0])
     return a, b, d
 
 
@@ -526,21 +512,19 @@ def dwithin_join(lhs: GeoSeries, rhs: GeoSeries, distance: float, how: str = "in
     if how == "left":
         matched = np.zeros(len(lhs), dtype=bool)
         matched[a] = True
-        miss = np.nonzero(~matched)[0]
-        a = np.concatenate([a, miss])
-        b = np.concatenate([b, np.full(len(miss), -1, dtype=np.int64)])
-        d = np.concatenate([d, np.full(len(miss), np.nan)])
-        order = np.lexsort((b, a))
-        a, b, d = a[order], b[order], d[order]
+        a, b, d = _left_rows(a, b, d, np.nonzero(~matched)[0])
     return a, b, d
 
 
 def _left_rows(a, b, d, unmatched):
-    """how='left': the unmatched left rows once, with rhs_index -1 and distance NaN, merged in (lhs, rhs) order"""
+    """how='left': the unmatched left rows once, with rhs_index -1 (and distance NaN when there is a distance column d),
+    merged in (lhs, rhs) order: (a, b, d), or (a, b) when d is None"""
     a = np.concatenate([a, unmatched])
     b = np.concatenate([b, np.full(len(unmatched), -1, dtype=np.int64)])
-    d = np.concatenate([d, np.full(len(unmatched), np.nan)])
     order = np.lexsort((b, a))
+    if d is None:
+        return a[order], b[order]
+    d = np.concatenate([d, np.full(len(unmatched), np.nan)])
     return a[order], b[order], d[order]
 
 

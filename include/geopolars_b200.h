@@ -72,7 +72,10 @@ typedef struct gpl_array gpl_array;         /* GeoArrow geometry array resident 
 typedef struct gpl_pip_index gpl_pip_index;
 typedef struct gpl_nearest_index gpl_nearest_index; /* right side of a nearest join */
 typedef struct gpl_geo_index gpl_geo_index; /* right side of a great-circle join */
-typedef struct gpl_pairs gpl_pairs;         /* (lhs_index, rhs_index) pair list of a join, resident on the device */ /* polygon-side index of a contains join */
+/* (lhs_index, rhs_index) pair list of a join, resident on the device.  Every pair list the library returns is sorted by
+ * (lhs, rhs) and holds no pair twice.  An entry point that returns one through gpl_pairs **out stores it only when it returns
+ * GPL_OK; on any error *out is NULL and nothing is left to free. */
+typedef struct gpl_pairs gpl_pairs;
 
 /* Raw GeoArrow buffers (the zero-dependency form of an Arrow array; replaces the WKB BinaryArray the
  * reference re-parses on every op, util.rs:27-37).
@@ -311,7 +314,7 @@ int gpl_contains_polygon(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, u
  * envelopes intersect (closed intervals, :74-76), exact test by the reference's type-pair dispatch (:89-137: Point x
  * (Multi)Polygon / (Multi)LineString in either order -> contains(point) whatever the predicate; (Multi)Polygon x Polygon ->
  * contains or intersects; Polygon x MultiPolygon -> intersects only; every other pair of types -> no match).  The
- * result is the pair list the reference builds at :139-157; its order is unspecified there (tree traversal) and here. */
+ * result is the pair list the reference builds at :139-157 (whose order is the tree traversal's), sorted by (lhs, rhs). */
 #define GPL_PREDICATE_INTERSECTS 0
 #define GPL_PREDICATE_CONTAINS 1
 int gpl_spatial_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, int predicate, gpl_pairs **out);
@@ -426,7 +429,7 @@ int gpl_intersection_area(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, 
  * pairs for which gpl_intersects(lhs[i], rhs[j]) is true, touching pairs included — with the area of lhs[i] ∩ rhs[j], bit for
  * bit what gpl_intersection_area returns for that row pair (lhs as the first operand).  Touching pairs carry 0 (or rounding
  * noise clamped at 0), so the areas of the pairs of a row over a partition sum to the row's area.  A device-resident gpl_pairs
- * in an unspecified order; the area of each pair is read with gpl_pairs_copy_distance.  Fewer than 2^31 rows per side (else
+ * sorted by (lhs, rhs); the area of each pair is read with gpl_pairs_copy_distance.  Fewer than 2^31 rows per side (else
  * GPL_ERR_UNSUPPORTED); any other type: GPL_ERR_INVALID_TYPE. */
 int gpl_overlay_area_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **out);
 
