@@ -130,6 +130,10 @@ extern "C" {
     fn gpl_relate(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, matrix: *mut i8, out_validity: *mut u8, mem: c_int) -> c_int;
     fn gpl_relate_predicate(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, predicate: c_int, pattern: *const c_char, out_bitmap: *mut u8, mem: c_int) -> c_int;
     fn gpl_predicate_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, predicate: c_int, pattern: *const c_char, out: *mut *mut GplPairs) -> c_int;
+    fn gpl_clip(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, invert: c_int, out: *mut *mut GplArray) -> c_int;
+    fn gpl_clip_length(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, out: *mut f64, out_validity: *mut u8, mem: c_int) -> c_int;
+    fn gpl_clip_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, pairs: *mut *mut GplPairs, out: *mut *mut GplArray) -> c_int;
+    fn gpl_overlay_length_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, out: *mut *mut GplPairs) -> c_int;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -509,6 +513,20 @@ pub trait GeoSeriesB200Ext {
     /// geometry overlay join of two (Multi)Polygon columns (`overlay(how="intersection")`): every pair whose intersection has a
     /// member, sorted by (lhs, rhs), with that intersection (bit for bit what `intersection` gives for the pair)
     fn overlay_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Series)>;
+    /// geo's `BooleanOps::clip` of a (Multi)LineString or (Multi)Point column by a (Multi)Polygon column, row by row: the parts
+    /// in the closed polygon (`invert`: strictly outside it) as a MultiLineString (MultiPoint) column.  Cut points are
+    /// vertices, input vertices are kept bit for bit; null or non-finite rows give null, an empty result an empty row
+    fn clip(&self, mask: &Series, invert: bool) -> Result<Series>;
+    /// row-wise length of the part of a (Multi)LineString row in the closed (Multi)Polygon row, without building it; null
+    /// or non-finite rows give null
+    fn intersection_length(&self, other: &Series) -> Result<Series>;
+    /// geometry clip join of a line or point column with a (Multi)Polygon column: every pair whose clip has a member, sorted
+    /// by (lhs, rhs), with that clip (bit for bit what `clip` gives for the pair); a one-row mask is GeoPandas' `clip`
+    fn clip_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Series)>;
+    /// length-weighted overlay join of a (Multi)LineString column with a (Multi)Polygon column: every intersecting pair
+    /// (touching pairs included, with length 0), as (lhs_index, rhs_index, length) sorted by (lhs, rhs); the length is bit
+    /// for bit what `intersection_length` computes for the pair
+    fn overlay_length_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)>;
     /// the union of the rows of each group (GeoPandas' `dissolve(by=...)`, geo's `unary_union` per group): `group[i]` in
     /// [-1, n_groups) names row i's group (-1 skips it); row g of the MultiPolygon result is the union of its group's rows.
     /// Null rows are skipped, a non-finite row nulls its group, a group with no row is an empty MultiPolygon
@@ -783,6 +801,59 @@ impl GeoSeriesB200Ext for Series {
         unsafe { gpl_pairs_free(pairs) };
         check(rc)?;
         Ok((l, r, from_device(ctx, geoms)?))
+    }
+
+    fn clip(&self, mask: &Series, invert: bool) -> Result<Series> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, mask)?);
+        let mut out = std::ptr::null_mut();
+        check(unsafe { gpl_clip(ctx, a.0, b.0, invert as c_int, &mut out) })?;
+        from_device(ctx, Dev(out))
+    }
+
+    fn intersection_length(&self, other: &Series) -> Result<Series> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, other)?);
+        let mut v = vec![0f64; self.len()];
+        let mut valid = vec![0u8; (self.len() + 7) / 8];
+        check(unsafe { gpl_clip_length(ctx, a.0, b.0, v.as_mut_ptr(), valid.as_mut_ptr(), GPL_HOST) })?;
+        Ok(f64_series("intersection_length", v, valid))
+    }
+
+    fn clip_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Series)> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let (mut pairs, mut out) = (std::ptr::null_mut(), std::ptr::null_mut());
+        check(unsafe { gpl_clip_join(ctx, a.0, b.0, &mut pairs, &mut out) })?;
+        let geoms = Dev(out);
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r) = (vec![0u64; n], vec![0u64; n]);
+        let mut rc = 0;
+        if n > 0 {
+            rc = unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) };
+        }
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
+        Ok((l, r, from_device(ctx, geoms)?))
+    }
+
+    fn overlay_length_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Vec<f64>)> {
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let mut pairs = std::ptr::null_mut();
+        check(unsafe { gpl_overlay_length_join(ctx, a.0, b.0, &mut pairs) })?;
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r, mut d) = (vec![0u64; n], vec![0u64; n], vec![0f64; n]);
+        let mut rc = 0;
+        if n > 0 {
+            rc = unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) };
+            if rc == 0 {
+                rc = unsafe { gpl_pairs_copy_distance(ctx, pairs, d.as_mut_ptr(), GPL_HOST) };
+            }
+        }
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
+        Ok((l, r, d))
     }
 
     fn relate(&self, other: &Series) -> Result<Series> {

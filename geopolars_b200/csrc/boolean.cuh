@@ -1,6 +1,6 @@
-// boolean.cuh — the device code the boolean geometry ops (k_boolean.cu, DESIGN.md §4.19) and dissolve (k_dissolve.cu,
-// §4.21) share: the boundary node records and their enumeration, the exact order of the nodes along an edge, and the
-// linking of kept pieces into output rings.
+// boolean.cuh — the device code the boolean geometry ops (k_boolean.cu, DESIGN.md §4.19), dissolve (k_dissolve.cu, §4.21)
+// and the line clip (k_clip.cu, §4.22) share: the boundary node records and their enumeration, the exact order of the nodes
+// along an edge, and the linking of kept pieces into output rings.
 #pragma once
 
 #include <math.h>
@@ -31,6 +31,8 @@ struct BLoop {
     double a2;                                      // twice the f64 shoelace area, relative to the first coordinate
 };
 
+// Side 0 may instead be a line or point column (clip, k_clip.cu): v[0].ro gives the coordinates of each chain, mem[0] the
+// chains (points) of a row (NULL for LineString / Point), and sg[0] / box[0] are NULL.
 struct BOperands {
     Side v[2];
     const int64_t *mem[2];   // member offsets of a MultiPolygon column, NULL for Polygon
@@ -61,6 +63,15 @@ __device__ __forceinline__ double2 crossing_point(double2 a0, double2 a1, double
     const double o0 = orient2d(b0.x, b0.y, b1.x, b1.y, a0.x, a0.y), o1 = orient2d(b0.x, b0.y, b1.x, b1.y, a1.x, a1.y);
     const double t = o0 / (o0 - o1);
     return make_double2(a0.x + t * (a1.x - a0.x), a0.y + t * (a1.y - a0.y));
+}
+
+// the node the edge (s, g) of the other side puts on the directed edge (p, q): K_VERTEX when s lies strictly inside (p, q),
+// K_CROSS for a proper crossing, else -1 (s on the line of (p, q) rules a proper crossing out, so there is at most one)
+__device__ __forceinline__ int edge_node(double2 p, double2 q, double2 s, double2 g) {
+    const int os = orient_sign(p, q, s), og = orient_sign(p, q, g);
+    if (os == 0 && point_in_rect(s, p, q) && !same_pt(s, p) && !same_pt(s, q)) return K_VERTEX;
+    if (os * og < 0 && orient_sign(s, g, p) * orient_sign(s, g, q) < 0) return K_CROSS;
+    return -1;
 }
 
 // One enumeration pass: the nodes of the directed edges of rings [xr0, xr1) of side X against the rings [yr0, yr1) of the
@@ -102,15 +113,15 @@ __device__ int64_t node_pass(const BOperands &o, int X, int64_t xr0, int64_t xr1
                     const double2 s = cy[j], g = cy[j + 1];
                     if (same_pt(s, g)) continue;
                     if (ex1 < fmin(s.x, g.x) || fmax(s.x, g.x) < ex0 || ey1 < fmin(s.y, g.y) || fmax(s.y, g.y) < ey0) continue;
-                    const int os = orient_sign(p, q, s), og = orient_sign(p, q, g);
-                    if (os == 0 && point_in_rect(s, p, q) && !same_pt(s, p) && !same_pt(s, q)) {  // s: a vertex inside (p, q)
+                    const int kind = edge_node(p, q, s, g);
+                    if (kind == K_VERTEX) {  // s: a vertex inside (p, q)
                         ++cnt;
                         if (WRITE) {
                             const double t = ((s.x - p.x) * dx + (s.y - p.y) * dy) / dd;
                             base[atomicAdd(slot, 1)] = BNode{s, t, rx, -1, (int32_t)i, -1, (int8_t)X, K_VERTEX, 0, 0};
                         }
                     }
-                    if (os * og < 0 && orient_sign(s, g, p) * orient_sign(s, g, q) < 0) {  // a proper crossing
+                    if (kind == K_CROSS) {  // a proper crossing
                         ++cnt;
                         if (WRITE) {
                             const double2 pt = X == 0 ? crossing_point(u, w, s, g) : crossing_point(s, g, u, w);
@@ -120,6 +131,74 @@ __device__ int64_t node_pass(const BOperands &o, int X, int64_t xr0, int64_t xr1
                     }
                 }
             }
+        }
+    }
+    return cnt;
+}
+
+// The enumeration pass with a line chain as side X (side 0; clip, k_clip.cu): the chain is directed in stored order and has
+// no closing edge and no σ.  Segment i with distinct ends gets a K_START record, then one record per vertex of the rings
+// [yr0, yr1) of side 1 strictly inside it and per proper crossing, in enumeration order; a segment with equal ends gets
+// none.  The START record's keep is 1 when the segment's start lies on one of those rings (a contact).  Lanes form groups
+// per segment as in node_pass; the G lanes of a group place their records by group ballots, so the order is fixed and no
+// atomics are needed.  Count pass: nrec[i] = the segment's record count; WRITE: the records of segment i go to
+// nodes + roff[i].  Returns this lane's number of records.
+template <bool WRITE>
+__device__ int64_t line_node_pass(const BOperands &o, const Chain &cx, int64_t chain, int64_t yr0, int64_t yr1, int lane,
+                                  int64_t *nrec, const int64_t *roff, BNode *nodes) {
+    const Side &yv = o.v[1];
+    const int64_t nseg = cx.coords() - 1;
+    int64_t cnt = 0;
+    int groups = 32;
+    while (groups > 1 && groups / 2 >= nseg) groups >>= 1;
+    const int G = 32 / groups, grp = lane / G, sub = lane - grp * G;
+    const unsigned gmask = G == 32 ? 0xffffffffu : ((1u << G) - 1u) << (grp * G), below = (1u << lane) - 1u;
+    for (int64_t b0 = 0; b0 < nseg; b0 += groups) {
+        const int64_t i = b0 + grp;
+        if (i >= nseg) continue;
+        const double2 p = cx[i], q = cx[i + 1];
+        if (same_pt(p, q)) continue;
+        const double ex0 = fmin(p.x, q.x), ex1 = fmax(p.x, q.x), ey0 = fmin(p.y, q.y), ey1 = fmax(p.y, q.y);
+        const double dx = q.x - p.x, dy = q.y - p.y, dd = dx * dx + dy * dy;
+        BNode *base = WRITE ? nodes + roff[i] : nullptr;
+        int64_t k = 1;  // records of the segment so far (the START is record 0)
+        bool contact = false;
+        for (int64_t ry = yr0; ry < yr1; ++ry) {
+            if (o.sg[1][ry] == 0) continue;
+            const double4 rb = o.box[1][ry];
+            if (ex1 < rb.x || rb.z < ex0 || ey1 < rb.y || rb.w < ey0) continue;
+            const Chain cy = part_ring(yv, ry);
+            const int64_t ny = cy.coords() - 1;
+            for (int64_t jb = 0; jb < ny; jb += G) {
+                const int64_t j = jb + sub;
+                int kind = -1;
+                double2 s = p, g = p;
+                if (j < ny) {
+                    s = cy[j], g = cy[j + 1];
+                    if (!same_pt(s, g) && !(ex1 < fmin(s.x, g.x) || fmax(s.x, g.x) < ex0 || ey1 < fmin(s.y, g.y) || fmax(s.y, g.y) < ey0)) {
+                        kind = edge_node(p, q, s, g);
+                        contact = contact || (point_in_rect(p, s, g) && orient_sign(s, g, p) == 0);
+                    }
+                }
+                const unsigned hits = __ballot_sync(gmask, kind >= 0);
+                if (WRITE && kind >= 0) {
+                    const int64_t at = k + __popc(hits & below);
+                    if (kind == K_VERTEX) {
+                        const double t = ((s.x - p.x) * dx + (s.y - p.y) * dy) / dd;
+                        base[at] = BNode{s, t, chain, -1, (int32_t)i, -1, 0, K_VERTEX, 0, 0};
+                    } else {
+                        const double op = orient2d(s.x, s.y, g.x, g.y, p.x, p.y), oq = orient2d(s.x, s.y, g.x, g.y, q.x, q.y);
+                        base[at] = BNode{crossing_point(p, q, s, g), op / (op - oq), chain, ry, (int32_t)i, (int32_t)j, 0, K_CROSS, 0, 0};
+                    }
+                }
+                k += __popc(hits);
+            }
+        }
+        contact = __ballot_sync(gmask, contact) != 0;
+        if (sub == 0) {
+            cnt += k;
+            if (WRITE) base[0] = BNode{p, 0.0, chain, -1, (int32_t)i, -1, 0, K_START, 0, (int8_t)(contact ? 1 : 0)};
+            else nrec[i] = k;
         }
     }
     return cnt;

@@ -478,6 +478,43 @@ def overlay_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, np.nda
     return a, b, geoms
 
 
+def clip(a: DeviceArray, b: DeviceArray, invert: bool = False) -> DeviceArray:
+    """row-wise clip of a (Multi)LineString or (Multi)Point column by a (Multi)Polygon column (DESIGN.md §4.22): the parts of
+    a[i] in closed(b[i]), or strictly outside it with invert, as a MultiLineString (MultiPoint) column; a null or non-finite
+    row gives a null row, an empty result an empty row"""
+    return _out_array(a.ctx, a.ctx.lib.gpl_clip, a._h, b._h, 1 if invert else 0)
+
+
+def clip_length(a: DeviceArray, b: DeviceArray) -> Tuple[np.ndarray, np.ndarray]:
+    """row-wise length of the part of a (Multi)LineString row in the closed (Multi)Polygon row, without building it
+    (DESIGN.md §4.22); (values, valid) — a null row or a non-finite coordinate gives an invalid row"""
+    n = len(a)
+    out = np.empty(n, dtype=np.float64)
+    bm = np.zeros((n + 7) // 8, dtype=np.uint8)
+    check(a.ctx.lib.gpl_clip_length(a.ctx._h, a._h, b._h, _np_ptr(out), _np_ptr(bm), GPL_HOST))
+    return out, _bits(bm, n)
+
+
+def clip_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, np.ndarray, DeviceArray]:
+    """(lhs uint64, rhs uint64, MultiLineString / MultiPoint column) for every pair of a line or point column and a
+    (Multi)Polygon column whose clip has a member, sorted by (lhs, rhs); row k is bit for bit `clip(lhs[i], rhs[j])`"""
+    ctx = lhs.ctx
+    hp, ha = C.c_void_p(), C.c_void_p()
+    check(ctx.lib.gpl_clip_join(ctx._h, lhs._h, rhs._h, C.byref(hp), C.byref(ha)))
+    geoms = DeviceArray(ctx, ha)
+    a, b = _take_pairs(ctx, hp)
+    return a, b, geoms
+
+
+def overlay_length_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """(lhs uint64, rhs uint64, length float64) for every pair of a (Multi)LineString and a (Multi)Polygon row that intersect
+    (touching pairs included, with length 0), sorted by (lhs, rhs); the length of a pair is bit for bit what `clip_length`
+    returns for it"""
+    h = C.c_void_p()
+    check(lhs.ctx.lib.gpl_overlay_length_join(lhs.ctx._h, lhs._h, rhs._h, C.byref(h)))
+    return _take_pairs(lhs.ctx, h, True)
+
+
 def dissolve(d: DeviceArray, codes, n_groups: int) -> DeviceArray:
     """the union of the rows of each group of a (Multi)Polygon column (DESIGN.md §4.21): row g of the MultiPolygon result is
     the union of the rows whose code is g, for g in [0, n_groups); code -1 and null rows are skipped, a row with a non-finite

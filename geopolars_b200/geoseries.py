@@ -333,6 +333,22 @@ class GeoRustSeries:
         """row-wise difference self[i] - other[i] (GeoPandas' `a.difference(b)`), as `intersection`"""
         return self._wrap(E.boolean_op(self._d(), other.device, "difference"))
 
+    def clip(self, mask: GeoSeries, invert: bool = False) -> GeoSeries:
+        """row-wise clip of self[i], a (Multi)LineString or (Multi)Point column, by mask[i], a (Multi)Polygon column
+        (GeoPandas' `a.intersection(b)` for lines, geo's `BooleanOps::clip`; DESIGN.md §4.22): the parts of self[i] in the
+        closed polygon (pieces along its boundary included), or with invert=True the parts strictly outside it, as a
+        MultiLineString (MultiPoint) column.  Cut points are vertices and input vertices are kept bit for bit.  Null when
+        either row is null or has a non-finite coordinate; an empty result is an empty row.  The polygons must be valid (OGC);
+        `is_valid()` tells.  For GeoPandas' `clip(series, mask)` with one mask, use `clip_join` with a one-row mask column."""
+        return self._wrap(E.clip(self._d(), mask.device, invert))
+
+    def intersection_length(self, other: GeoSeries):
+        """row-wise length of the part of self[i], a (Multi)LineString column, in the closed (Multi)Polygon other[i]
+        (GeoPandas' `a.intersection(b).length`, without building the geometry; DESIGN.md §4.22).  Null when either row is null
+        or has a non-finite coordinate; 0 when there is no overlap of positive length."""
+        out, valid = E.clip_length(self._d(), other.device)
+        return _f64(out, valid)
+
     def union_all(self) -> GeoSeries:
         """the union of every row, a (Multi)Polygon column, as a GeoSeries of one MultiPolygon row (GeoPandas'
         `union_all()`, formerly `unary_union`; DESIGN.md §4.21).  Null rows are skipped; a row with a non-finite coordinate
@@ -555,6 +571,35 @@ def overlay_join(lhs: GeoSeries, rhs: GeoSeries):
     `lhs.geo.intersection` of the pair (DESIGN.md §4.19).  Valid (OGC) operands only; filter with `is_valid()` first."""
     a, b, g = E.overlay_join(lhs.device, rhs.device)
     return a.astype(np.int64), b.astype(np.int64), GeoSeries(_device=g, name=lhs.name)
+
+
+def clip_join(lhs: GeoSeries, rhs: GeoSeries):
+    """Geometry clip join of a (Multi)LineString or (Multi)Point column with a (Multi)Polygon column (GeoPandas'
+    `overlay(lines, polys, how="intersection")` with keep_geom_type=True): (lhs_index int64, rhs_index int64, GeoSeries of
+    MultiLineStrings or MultiPoints) for every pair whose clip has at least one member, sorted by (lhs, rhs); lines that only
+    touch a polygon are dropped.  Geometry k is bit for bit `lhs.geo.clip` of the pair (DESIGN.md §4.22).  With a one-row
+    `rhs` this is GeoPandas' `clip(lhs, mask)`: the clipped rows, with their left indices.  Valid (OGC) polygons only."""
+    a, b, g = E.clip_join(lhs.device, rhs.device)
+    return a.astype(np.int64), b.astype(np.int64), GeoSeries(_device=g, name=lhs.name)
+
+
+def overlay_length_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner"):
+    """Length-weighted overlay join of a (Multi)LineString column with a (Multi)Polygon column ("the length of each road in
+    each county"): (lhs_index int64, rhs_index int64, length float64) for every pair that intersects — exactly the pairs
+    `lhs.geo.intersects` accepts row-wise — sorted by (lhs, rhs).  The length is bit for bit what
+    `lhs.geo.intersection_length` computes for the pair.  Pairs that only touch are kept with length 0, so the lengths of a
+    line over a partition sum to its length; keep `length > 0` to drop them.  how='inner' -> matched left rows only;
+    how='left' -> unmatched left rows once, with rhs_index -1 and length NaN (DESIGN.md §4.22).  Valid (OGC) polygons only."""
+    if how not in ("inner", "left"):
+        raise ValueError("how must be 'inner' or 'left'")
+    a, b, d = E.overlay_length_join(lhs.device, rhs.device)
+    a = a.astype(np.int64)
+    b = b.astype(np.int64)
+    if how == "left":
+        matched = np.zeros(len(lhs), dtype=bool)
+        matched[a] = True
+        a, b, d = _left_rows(a, b, d, np.nonzero(~matched)[0])
+    return a, b, d
 
 
 def geo_nearest_join(lhs: GeoSeries, rhs: GeoSeries, how: str = "inner", max_distance: Optional[float] = None):

@@ -412,7 +412,8 @@ int gpl_dwithin_count(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_arra
 int gpl_dwithin_join_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int with_distance,
                            gpl_pairs **out);
 /* the distance of each pair of a list built with distances (any other list: GPL_ERR_INVALID_ARG); distance[n] in `mem`.
- * For a list from gpl_overlay_area_join the value of each pair is its intersection area. */
+ * For a list from gpl_overlay_area_join the value of each pair is its intersection area, from gpl_overlay_length_join its
+ * intersection length. */
 int gpl_pairs_copy_distance(gpl_ctx *ctx, const gpl_pairs *pairs, double *distance, int mem);
 
 /* ---------------------------------------------------------------- intersection area ------ */
@@ -466,6 +467,42 @@ int gpl_overlay_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, g
  * a code outside [-1, n_groups) or n_groups < 0: GPL_ERR_INVALID_ARG; 2^31 or more rows or groups, or a group with 2^30 or more
  * boundary nodes: GPL_ERR_UNSUPPORTED. */
 int gpl_dissolve(gpl_ctx *ctx, const gpl_array *in, const int64_t *group, int mem, int64_t n_groups, gpl_array **out);
+
+/* ---------------------------------------------------------------- clipping ---------------- */
+/* Clip of a line or point column by a polygon column (GeoPandas' clip / overlay with lines, geo's BooleanOps::clip),
+ * DESIGN.md §4.22.  a: LineString or MultiLineString (or, for gpl_clip and gpl_clip_join, Point or MultiPoint); b: Polygon or
+ * MultiPolygon (any other pair: GPL_ERR_INVALID_TYPE); unequal lengths: GPL_ERR_LENGTH_MISMATCH; both before any launch.
+ * invert = 0 keeps what lies in closed(b[i]) (its interior or boundary: pieces along a polygon edge are kept); invert != 0
+ * keeps what lies strictly outside it.  Line output is a MultiLineString column: one member per maximal run of consecutive
+ * kept pieces of one input chain, in input order (difference also splits a run at a point where the line touches the
+ * boundary); runs are never joined across chains or across the start of a closed chain.  Every cut point is a vertex: a
+ * crossing is a0 + t (a1 - a0) along the line's own segment, a polygon vertex on the line keeps its coordinates, input
+ * vertices are copied bit for bit; consecutive equal coordinates are written once and a member left with fewer than 2
+ * distinct points is dropped.  Point output is a MultiPoint column of the points of a[i] in closed(b[i]) (strictly outside
+ * with invert), in input order, duplicates kept.  Polygon rings are read as gpl_boolean_op reads them; line chains in stored
+ * order, never closed implicitly.  A null row or a row with a non-finite coordinate on either side gives a null row; an
+ * empty result is an empty Multi* row.  Every in / on / out decision is an exact sign of input coordinates; only crossing
+ * points are rounded.  The polygon operand must be valid (OGC): on invalid polygons the output is a well-formed column whose
+ * geometry is not specified.  A row's output depends on that row only, bit for bit.  A row with 2^30 or more nodes:
+ * GPL_ERR_UNSUPPORTED. */
+int gpl_clip(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, int invert, gpl_array **out);
+/* Length of the intersection of a (Multi)LineString row with closed(b[i]), computed without writing geometry: the f64 sum of
+ * the kept pieces' lengths, >= 0, 0 when there is no 1-dimensional overlap; null (NaN, validity 0) under gpl_clip's rules.
+ * Equal to the euclidean length of gpl_clip's row within a few ulps per piece.  out[n] f64, out_validity bitmap (may be
+ * NULL), both in `mem`.  Types and errors as gpl_clip (point columns: GPL_ERR_INVALID_TYPE).  Deterministic. */
+int gpl_clip_length(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, double *out, uint8_t *out_validity, int mem);
+/* Geometry clip join of a line or point column with a (Multi)Polygon column: every pair (i, j) whose intersection has at
+ * least one member (one point), sorted by (lhs, rhs), as a device-resident gpl_pairs; row k of *out (MultiLineString or
+ * MultiPoint) is bit for bit gpl_clip(lhs[i], rhs[j], 0).  Candidates are the pairs gpl_intersects accepts; lines that only
+ * touch are dropped.  A one-row rhs is GeoPandas' clip(lhs, mask).  Fewer than 2^31 rows per side (else GPL_ERR_UNSUPPORTED);
+ * any other type: GPL_ERR_INVALID_TYPE.  *pairs and *out are set only on success. */
+int gpl_clip_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **pairs, gpl_array **out);
+/* Length-weighted overlay join of a (Multi)LineString column with a (Multi)Polygon column: every pair (i, j) for which
+ * gpl_intersects(lhs[i], rhs[j]) is true, touching pairs included with length 0 (so the lengths of a line over a partition
+ * sum to its length), with the length of lhs[i] in closed(rhs[j]), bit for bit what gpl_clip_length returns for that row
+ * pair.  A device-resident gpl_pairs sorted by (lhs, rhs); the length of each pair is read with gpl_pairs_copy_distance.
+ * Fewer than 2^31 rows per side (else GPL_ERR_UNSUPPORTED); any other type: GPL_ERR_INVALID_TYPE. */
+int gpl_overlay_length_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **out);
 
 /* ---------------------------------------------------------------- validity ---------------- */
 /* OGC validity of every row, any geometry type, DESIGN.md §4.18: reason[n] (int8, in `mem`) is the first failing rule in the

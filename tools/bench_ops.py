@@ -4,7 +4,7 @@ fraction for the coordinate bytes read, and of the nearest join (100 M points ag
 reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic|valid|boolean|relate] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic|valid|boolean|relate|dissolve|clip] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
@@ -41,12 +41,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve"), default="all",
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve", "clip"), default="all",
                     help="run only the §8 rows, only the point nearest join, only the geometry nearest join, only the "
                          "distance-within join, only the great-circle joins, only the intersection area and overlay join or "
                          "only the geodesic area and perimeter (1 M stars, 10 M parcels, naturalearth_lowres to 1 M rows), or only "
                          "the boolean geometry ops and the geometry overlay join, or only the DE-9IM relate, predicates and "
-                         "predicate join, or only dissolve / union_all; "
+                         "predicate join, or only dissolve / union_all, or only the line clip, intersection length and their joins; "
                          "'all' runs every arm")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
@@ -91,11 +91,13 @@ def main():
             relate_rows(args, ctx, dev, st, res)
         if args.only in ("all", "dissolve"):
             dissolve_rows(args, ctx, dev, st, res)
+        if args.only in ("all", "clip"):
+            clip_rows(args, ctx, dev, st, res)
         if args.only in ("all", "geodesic"):
             geodesic_rows(args, ctx, dev, st, res)
         if args.only in ("all", "valid"):
             valid_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve"):
+        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve", "clip"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -709,6 +711,85 @@ def relate_rows(args, ctx, dev, st, res):
     rec("points within polygons, index route (%d points x %d stars, index build included)" % (m, len(stars)), cnt[0], "pairs", t, {})
     t = timed(st, lambda: join(pts, stars, E.RELATE_PREDICATES["within"], cnt), reps=3, warm=1)
     rec("points within polygons, relate route (%d points x %d stars)" % (m, len(stars)), cnt[0], "pairs", t, {})
+
+
+def clip_rows(args, ctx, dev, st, res):
+    """line clipping (DESIGN.md §4.22): clip, clip(invert) and clip_length of 1 M config-3 walks (16 coordinates), each
+    against config 2's star whose 10 m cell holds the walk's start, with relate on the same row pairs for context; the
+    length-weighted overlay join of the 1 M walks against the 10 000 stars and of 100 000 walks against a 1000 x 1000 grid
+    of unit squares (candidates, sort and the per-pair kernels, host synchronisations included)"""
+    import numpy as np
+
+    from geopolars_b200 import synth
+
+    lib = ctx.lib
+
+    def rec(name, units, unit_name, t, extra):
+        r = {"op": name, "units": units, "unit": unit_name, "ms_min": t[0], "ms_avg": t[1], "units_per_s": units / (t[1] * 1e-3),
+             "card": res["card"], "power_limit": res["power_limit"], **extra}
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    def polygons(xy_t, ring_off, geom_off):
+        t = [torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in (ring_off, geom_off)]
+        n = len(geom_off) - 1
+        return ctx.wrap_device(GeometryType.POLYGON, n, xy_t.shape[0], xy_t.data_ptr(), geom_off_ptr=t[1].data_ptr(), ring_off_ptr=t[0].data_ptr(),
+                               n_rings=len(ring_off) - 1, keepalive=(xy_t, *t))
+
+    def walks(n, stream):
+        xy = torch.empty((n * 16, 2), dtype=torch.float64, device=dev)
+        off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+        E.check(lib.gpl_gen_walk_linestrings(ctx._h, stream, -1, 0, n, 16, xy.data_ptr(), off.data_ptr()))
+        return xy, ctx.wrap_device(GeometryType.LINESTRING, n, n * 16, xy.data_ptr(), geom_off_ptr=off.data_ptr(), keepalive=(xy, off))
+
+    n = int(1_000_000 * args.scale)
+    wxy, lines = walks(n, 3)
+    sxy, sro, sgo = synth.star_polygons()
+    stars_t = torch.from_numpy(sxy).to(dev)
+    start = wxy.view(n, 16, 2)[:, 0, :]
+    cell = (torch.clamp(torch.floor(start[:, 1] / 10.0), 0, 99) * 100 + torch.clamp(torch.floor(start[:, 0] / 10.0), 0, 99)).long()
+    mine = stars_t.view(-1, 65, 2)[cell].reshape(-1, 2).contiguous()
+    polys = polygons(mine, np.arange(n + 1, dtype=np.int64) * 65, np.arange(n + 1, dtype=np.int64))
+    out = torch.empty(n, dtype=torch.float64, device=dev)
+    mat = torch.empty(n * 9, dtype=torch.int8, device=dev)
+    for inv in (0, 1):
+        coords = [0]
+
+        def run():
+            h = C.c_void_p()
+            E.check(lib.gpl_clip(ctx._h, lines._h, polys._h, inv, C.byref(h)))
+            d = E.DeviceArray(ctx, h)
+            coords[0] = int(d.view().n_coords)
+            d.free()
+
+        t = timed(st, run, reps=3, warm=1)
+        rec("clip%s (%d walks x their cell's star, 15 x 64 edges)" % (" invert" if inv else "", n), n, "row pairs", t, {"out_coords": coords[0]})
+    t = timed(st, lambda: E.check(lib.gpl_clip_length(ctx._h, lines._h, polys._h, C.c_void_p(out.data_ptr()), None, E.GPL_DEVICE)), reps=3, warm=1)
+    rec("clip_length (%d walks x their cell's star)" % n, n, "row pairs", t, {"total_length": float(out.sum().item())})
+    t = timed(st, lambda: E.check(lib.gpl_relate(ctx._h, lines._h, polys._h, C.c_void_p(mat.data_ptr()), None, E.GPL_DEVICE)), reps=3, warm=1)
+    rec("relate (the same %d row pairs)" % n, n, "row pairs", t, {})
+    del polys, mine
+
+    def join(lhs, rhs, out):
+        h = C.c_void_p()
+        E.check(lib.gpl_overlay_length_join(ctx._h, lhs._h, rhs._h, C.byref(h)))
+        out[0] = int(lib.gpl_pairs_count(h))
+        lib.gpl_pairs_free(h)
+
+    stars = polygons(stars_t, sro, sgo)
+    cnt = [0]
+    t = timed(st, lambda: join(lines, stars, cnt), reps=3, warm=1)
+    rec("overlay_length_join (%d walks x 10 000 stars)" % n, cnt[0], "pairs", t, {})
+    m = int(100_000 * args.scale)
+    _, few = walks(m, 4)
+    k = int(1000 * np.sqrt(args.scale))
+    i, j = np.meshgrid(np.arange(k, dtype=np.float64), np.arange(k, dtype=np.float64), indexing="xy")
+    x0, y0 = i.ravel() * (1000.0 / k), j.ravel() * (1000.0 / k)
+    w = 1000.0 / k
+    gxy = np.stack([np.stack([x0, x0 + w, x0 + w, x0, x0], 1), np.stack([y0, y0, y0 + w, y0 + w, y0], 1)], 2).reshape(-1, 2)
+    cells = polygons(torch.from_numpy(gxy).to(dev), np.arange(k * k + 1, dtype=np.int64) * 5, np.arange(k * k + 1, dtype=np.int64))
+    t = timed(st, lambda: join(few, cells, cnt), reps=3, warm=1)
+    rec("overlay_length_join (%d walks x %d unit squares)" % (m, k * k), cnt[0], "pairs", t, {})
 
 
 def geodesic_rows(args, ctx, dev, st, res):
