@@ -127,6 +127,7 @@ extern "C" {
     fn gpl_boolean_op(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, op: c_int, out: *mut *mut GplArray) -> c_int;
     fn gpl_overlay_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, pairs: *mut *mut GplPairs, out: *mut *mut GplArray) -> c_int;
     fn gpl_dissolve(ctx: *mut GplCtx, input: *const GplArray, group: *const i64, mem: c_int, n_groups: i64, out: *mut *mut GplArray) -> c_int;
+    fn gpl_overlay(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, how: c_int, pairs: *mut *mut GplPairs, out: *mut *mut GplArray) -> c_int;
     fn gpl_relate(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, matrix: *mut i8, out_validity: *mut u8, mem: c_int) -> c_int;
     fn gpl_relate_predicate(ctx: *mut GplCtx, a: *const GplArray, b: *const GplArray, predicate: c_int, pattern: *const c_char, out_bitmap: *mut u8, mem: c_int) -> c_int;
     fn gpl_predicate_join(ctx: *mut GplCtx, lhs: *const GplArray, rhs: *const GplArray, predicate: c_int, pattern: *const c_char, out: *mut *mut GplPairs) -> c_int;
@@ -510,6 +511,15 @@ pub trait GeoSeriesB200Ext {
     fn union(&self, other: &Series) -> Result<Series>;
     /// geo's `BooleanOps::difference` (self - other), as `intersection`
     fn difference(&self, other: &Series) -> Result<Series>;
+    /// geo's `BooleanOps::xor` (the parts covered by exactly one row), as `intersection`; members of self - other and
+    /// other - self that touch at a point stay separate members
+    fn symmetric_difference(&self, other: &Series) -> Result<Series>;
+    /// GeoPandas' `overlay(self, rhs, how)` of two (Multi)Polygon columns, `how` one of "intersection", "union", "identity",
+    /// "symmetric_difference", "difference": intersection rows (Some(i), Some(j)), exactly `overlay_join_pairs`' rows; left
+    /// remainders (Some(i), None), self[i] minus every rhs row it intersects; right remainders (None, Some(j)), as the mode
+    /// selects.  Remainders with no member are dropped.  Sorted by (lhs, rhs) with None after every index.  Valid (OGC)
+    /// operands only
+    fn overlay_pairs(&self, rhs: &Series, how: &str) -> Result<(Vec<Option<u64>>, Vec<Option<u64>>, Series)>;
     /// geometry overlay join of two (Multi)Polygon columns (`overlay(how="intersection")`): every pair whose intersection has a
     /// member, sorted by (lhs, rhs), with that intersection (bit for bit what `intersection` gives for the pair)
     fn overlay_join_pairs(&self, rhs: &Series) -> Result<(Vec<u64>, Vec<u64>, Series)>;
@@ -771,6 +781,36 @@ impl GeoSeriesB200Ext for Series {
         boolean_op(self, other, GPL_BOOLEAN_DIFFERENCE)
     }
 
+    fn symmetric_difference(&self, other: &Series) -> Result<Series> {
+        boolean_op(self, other, GPL_BOOLEAN_SYMMETRIC_DIFFERENCE)
+    }
+
+    fn overlay_pairs(&self, rhs: &Series, how: &str) -> Result<(Vec<Option<u64>>, Vec<Option<u64>>, Series)> {
+        let code: c_int = match how {
+            "intersection" => 0,
+            "union" => 1,
+            "identity" => 2,
+            "symmetric_difference" => 3,
+            "difference" => 4,
+            _ => return Err(PolarsError::ComputeError(format!("overlay: unknown how {how:?}").into()).into()),
+        };
+        let ctx = ctx()?;
+        let (a, b) = (to_device(ctx, self)?, to_device(ctx, rhs)?);
+        let (mut pairs, mut out) = (std::ptr::null_mut(), std::ptr::null_mut());
+        check(unsafe { gpl_overlay(ctx, a.0, b.0, code, &mut pairs, &mut out) })?;
+        let geoms = Dev(out);
+        let n = unsafe { gpl_pairs_count(pairs) } as usize;
+        let (mut l, mut r) = (vec![0u64; n], vec![0u64; n]);
+        let mut rc = 0;
+        if n > 0 {
+            rc = unsafe { gpl_pairs_copy(ctx, pairs, l.as_mut_ptr(), r.as_mut_ptr(), GPL_HOST) };
+        }
+        unsafe { gpl_pairs_free(pairs) };
+        check(rc)?;
+        let side = |v: Vec<u64>| v.into_iter().map(|k| if k == u64::MAX { None } else { Some(k) }).collect();
+        Ok((side(l), side(r), from_device(ctx, geoms)?))
+    }
+
     fn dissolve(&self, group: &[i64], n_groups: i64) -> Result<Series> {
         if group.len() != self.len() {
             return Err(PolarsError::ShapeMismatch(format!("dissolve: {} group codes for {} rows", group.len(), self.len()).into()).into());
@@ -943,6 +983,7 @@ fn relate_predicate(a: &Series, b: &Series, predicate: c_int, pattern: Option<&s
 const GPL_BOOLEAN_INTERSECTION: c_int = 0;
 const GPL_BOOLEAN_UNION: c_int = 1;
 const GPL_BOOLEAN_DIFFERENCE: c_int = 2;
+const GPL_BOOLEAN_SYMMETRIC_DIFFERENCE: c_int = 3;
 
 /// gpl_boolean_op of two (Multi)Polygon columns: a MultiPolygon column
 fn boolean_op(a: &Series, b: &Series, op: c_int) -> Result<Series> {

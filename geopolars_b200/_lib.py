@@ -177,6 +177,7 @@ SIGNATURES = {
     "gpl_boolean_op": (_INT, [_P, _P, _P, _INT, C.POINTER(_P)]),
     "gpl_overlay_join": (_INT, [_P, _P, _P, C.POINTER(_P), C.POINTER(_P)]),
     "gpl_dissolve": (_INT, [_P, _P, _P, _INT, C.c_int64, C.POINTER(_P)]),
+    "gpl_overlay": (_INT, [_P, _P, _P, _INT, C.POINTER(_P), C.POINTER(_P)]),
     "gpl_clip": (_INT, [_P, _P, _P, _INT, C.POINTER(_P)]),
     "gpl_clip_length": (_INT, [_P, _P, _P, _P, _P, _INT]),
     "gpl_clip_join": (_INT, [_P, _P, _P, C.POINTER(_P), C.POINTER(_P)]),

@@ -272,14 +272,17 @@ __device__ void heap_sort(T *a, int64_t n, const Less &less) {
 }
 
 // ---- linking and ring assembly: one thread per row ----------------------------------------------------------------------
-// the kept pieces of one row, in output direction (B pieces of a difference reversed)
+// the kept pieces of one row, in output direction.  BY_STATE: a kept piece in state S_IN is written reversed (either side's
+// pieces in the other of a symmetric difference, a remainder's cutter pieces, §4.23); else, with rev_b, B's pieces (a
+// difference)
+template <bool BY_STATE>
 struct Pieces {
     const BOperands *o;
     const BNode *nd;  // the row's nodes
     int64_t nn;
     const int32_t *kp;  // kept piece -> node index
     bool rev_b;
-    __device__ bool rev(int j) const { return rev_b && nd[kp[j]].side == 1; }
+    __device__ bool rev(int j) const { return BY_STATE ? nd[kp[j]].state == S_IN : rev_b && nd[kp[j]].side == 1; }
     __device__ bool next_on_edge(int64_t k) const {
         return k + 1 < nn && nd[k + 1].side == nd[k].side && nd[k + 1].ring == nd[k].ring && nd[k + 1].seg == nd[k].seg;
     }
@@ -307,8 +310,9 @@ struct Pieces {
 
 __device__ __forceinline__ int pt_cmp(double2 a, double2 b) { return a.x != b.x ? (a.x < b.x ? -1 : 1) : (a.y != b.y ? (a.y < b.y ? -1 : 1) : 0); }
 
+template <bool BY_STATE>
 struct FromPtLess {  // pieces by the output coordinates of their start
-    const Pieces *pc;
+    const Pieces<BY_STATE> *pc;
     __device__ bool operator()(int32_t a, int32_t b) const {
         const int c = pt_cmp(pc->from_pt(a), pc->from_pt(b));
         return c ? c < 0 : a < b;
@@ -316,7 +320,8 @@ struct FromPtLess {  // pieces by the output coordinates of their start
 };
 
 // 0 outside / 1 on the boundary / 2 inside of the loop through the from-points of its pieces
-static __device__ int point_in_loop(const Pieces &pc, const int32_t *lp, const BLoop &L, double2 v) {
+template <bool BY_STATE>
+static __device__ int point_in_loop(const Pieces<BY_STATE> &pc, const int32_t *lp, const BLoop &L, double2 v) {
     int wn = 0;
     for (int i = 0; i < L.len; ++i) {
         const double2 s = pc.from_pt(lp[L.start + i]), e = pc.from_pt(lp[L.start + (i + 1 == L.len ? 0 : i + 1)]);
@@ -348,8 +353,10 @@ struct LoopLess {  // members by their shell's first vertex, holes after their s
 // Link the kept pieces of the nodes nd[0, nn) (ordered by edge) into output rings: scratch ws (8 int32 per node, at stride
 // ws_stride) and L (one BLoop per node); lbox (one double4 per node, or NULL) lets the hole-to-shell search skip the shells
 // whose box does not contain the hole's first vertex, and give a hole to the only shell whose box does without walking it.  Counting pass: the members, rings and coordinates (nm, nr, nc);
-// WRITE: the MultiPolygon's part / ring offsets and coordinates from the bases mb, rb, cb.
-template <bool WRITE>
+// WRITE: the MultiPolygon's part / ring offsets and coordinates from the bases mb, rb, cb.  The pieces written reversed: with
+// BY_STATE those in state S_IN, else with rev_b those of side 1 (Pieces).  BY_STATE is a template argument so that the ops
+// that do not need it compile to what they did before it existed.
+template <bool WRITE, bool BY_STATE>
 __device__ void assemble_pieces(const BOperands &o, bool rev_b, const BNode *__restrict__ nd, int64_t nn, int32_t *__restrict__ ws,
                                 int64_t ws_stride, BLoop *__restrict__ L, double4 *__restrict__ lbox, int64_t &nm_out, int64_t &nr_out,
                                 int64_t &nc_out, int64_t mb, int64_t rb, int64_t cb, int64_t *__restrict__ part_off,
@@ -359,7 +366,7 @@ __device__ void assemble_pieces(const BOperands &o, bool rev_b, const BNode *__r
     int J = 0;
     for (int64_t k = 0; k < nn; ++k)
         if (nd[k].keep) kp[J++] = (int32_t)k;
-    const Pieces pc{&o, nd, nn, kp, rev_b};
+    const Pieces<BY_STATE> pc{&o, nd, nn, kp, rev_b};
     // a piece whose two ends round to one point (between two crossings within half an ulp of each other) has no length
     int Jp = 0;
     for (int j = 0; j < J; ++j)
@@ -371,7 +378,7 @@ __device__ void assemble_pieces(const BOperands &o, bool rev_b, const BNode *__r
     // coordinates require, where linking by input node would leave a ring through the point twice or rings touching in
     // a cycle of such points
     for (int j = 0; j < J; ++j) ord[j] = j;
-    heap_sort(ord, (int64_t)J, FromPtLess{&pc});
+    heap_sort(ord, (int64_t)J, FromPtLess<BY_STATE>{&pc});
     for (int i = 0; i < J; ++i) {
         rank[ord[i]] = i;
         gs[i] = (i > 0 && same_pt(pc.from_pt(ord[i]), pc.from_pt(ord[i - 1]))) ? gs[i - 1] : i;
@@ -525,5 +532,14 @@ __device__ void assemble_pieces(const BOperands &o, bool rev_b, const BNode *__r
         oxy[cb++] = lo.first;
     }
 }
+
+// out[k] = the first position of keys (sorted, length m) that is >= k, for k in [0, nq] (k_dissolve.cu)
+__global__ void __launch_bounds__(256) k_lower_bounds(const uint64_t *__restrict__ keys, int64_t m, int64_t nq, int64_t *__restrict__ out);
+// Row k of the MultiPolygon column *out is row row[k] of srcs[src[k]] (each a Polygon or MultiPolygon column, or NULL when no
+// row names it), validity included, with offsets rebased; src and row on the device (k_overlay_modes.cu)
+int gather_polygons(gpl_ctx *ctx, const gpl_array *const srcs[3], const int8_t *src, const uint64_t *row, int64_t m, gpl_array **out);
+// The remainder of every row of subj: the row minus the union of the rows of cut its closed geometry intersects, as a
+// MultiPolygon column of subj's length (DESIGN.md §4.23; k_dissolve.cu).  Fewer than 2^31 rows in the two columns together.
+int remainder_rows(gpl_ctx *ctx, const gpl_array *subj, const gpl_array *cut, gpl_array **out);
 
 }  // namespace gpl

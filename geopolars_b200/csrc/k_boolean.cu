@@ -1,4 +1,4 @@
-// k_boolean.cu — intersection, union and difference geometry of two (Multi)Polygon columns, row-wise (gpl_boolean_op) and as
+// k_boolean.cu — intersection, union, difference and symmetric difference geometry of two (Multi)Polygon columns, row-wise (gpl_boolean_op) and as
 // a geometry overlay join (gpl_overlay_join).  geo 0.27 has them as BooleanOps::{intersection, union, difference} (recalled),
 // each returning a MultiPolygon.  DESIGN.md §4.19 has the derivation.
 //
@@ -87,6 +87,9 @@ __global__ void __launch_bounds__(kBoolThreads) k_bool_nodes(int64_t n, BOperand
 }
 
 __device__ __forceinline__ bool keep_piece(int op, int side, int st) {
+    // symmetric difference, either side: outside the other operand as it is, inside it reversed; on a shared edge both sides
+    // of the edge are in the same number of operands (same direction) or both in the result (opposite): never kept
+    if (op == GPL_BOOLEAN_SYMMETRIC_DIFFERENCE) return st == S_OUT || st == S_IN;
     if (side == 0) {
         if (op == GPL_BOOLEAN_INTERSECTION) return st == S_IN || st == S_ON_SAME;
         if (op == GPL_BOOLEAN_UNION) return st == S_OUT || st == S_ON_SAME;
@@ -166,7 +169,7 @@ __global__ void __launch_bounds__(kBoolThreads) k_bool_classify(int64_t n, BOper
 
 // One thread per row.  Scratch (8 int32 per node, one BLoop per node) is indexed by the row's node offset.  Counting pass:
 // members, rings and coordinates of the row; WRITE: the MultiPolygon's part / ring offsets and coordinates at the row's bases.
-template <bool WRITE>
+template <bool WRITE, bool BY_STATE>
 __global__ void __launch_bounds__(128) k_bool_assemble(int64_t n, BOperands o, int op, const int64_t *__restrict__ off, const BNode *__restrict__ nodes,
                                                        int32_t *__restrict__ ws, int64_t ws_stride, BLoop *__restrict__ loops,
                                                        int64_t *__restrict__ cm, int64_t *__restrict__ cr, int64_t *__restrict__ cc,
@@ -177,7 +180,7 @@ __global__ void __launch_bounds__(128) k_bool_assemble(int64_t n, BOperands o, i
     for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += stride) {
         const int64_t o0 = off[r], nn = off[r + 1] - o0;
         int64_t nm, nr, nc;
-        assemble_pieces<WRITE>(o, op == GPL_BOOLEAN_DIFFERENCE, nodes + o0, nn, ws + o0, ws_stride, loops + o0, nullptr, nm, nr, nc,
+        assemble_pieces<WRITE, BY_STATE>(o, op == GPL_BOOLEAN_DIFFERENCE, nodes + o0, nn, ws + o0, ws_stride, loops + o0, nullptr, nm, nr, nc,
                                WRITE ? mbase[r] : 0, WRITE ? rbase[r] : 0, WRITE ? cbase[r] : 0, part_off, ring_off, oxy);
         if (!WRITE) cm[r] = nm, cr[r] = nr, cc[r] = nc;
     }
@@ -222,11 +225,12 @@ static int boolean_rows(gpl_ctx *ctx, const BOperands &ops, int64_t n, const uin
     GPL_TRY(rbase.get(ctx, (size_t)n + 1));
     GPL_TRY(cbase.get(ctx, (size_t)n + 1));
     const int tgrid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 128), (int64_t)kSMs * 16));
+    const bool sym = op == GPL_BOOLEAN_SYMMETRIC_DIFFERENCE;  // pieces reversed by their state
     if (n > 0) {
         GPL_LAUNCH(ctx, k_bool_nodes<true>, grid, kBoolThreads, 0, n, ops, ia, ib, cnt.p, rv.p, off.p, nodes.p, too_big.p);
         GPL_LAUNCH(ctx, k_bool_classify, grid, kBoolThreads, 0, n, ops, ia, ib, op, off.p, nodes.p);
-        GPL_LAUNCH(ctx, k_bool_assemble<false>, tgrid, 128, 0, n, ops, op, off.p, nodes.p, ws.p, h_nodes, loops.p, cm.p, cr.p, cc.p,
-                   nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+        GPL_LAUNCH(ctx, (sym ? k_bool_assemble<false, true> : k_bool_assemble<false, false>), tgrid, 128, 0, n, ops, op, off.p, nodes.p, ws.p,
+                   h_nodes, loops.p, cm.p, cr.p, cc.p, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
     }
     GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cm.p, n, geom_off.p, tot.p)));
     GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cr.p, n, rbase.p, tot.p + 1)));
@@ -238,8 +242,8 @@ static int boolean_rows(gpl_ctx *ctx, const BOperands &ops, int64_t n, const uin
     GPL_TRY(ring_off.get(ctx, (size_t)h_tot[1] + 1));
     GPL_TRY(oxy.get(ctx, (size_t)h_tot[2] * 2));
     if (n > 0)
-        GPL_LAUNCH(ctx, k_bool_assemble<true>, tgrid, 128, 0, n, ops, op, off.p, nodes.p, ws.p, h_nodes, loops.p, cm.p, cr.p, cc.p,
-                   geom_off.p, rbase.p, cbase.p, part_off.p, ring_off.p, reinterpret_cast<double2 *>(oxy.p));
+        GPL_LAUNCH(ctx, (sym ? k_bool_assemble<true, true> : k_bool_assemble<true, false>), tgrid, 128, 0, n, ops, op, off.p, nodes.p, ws.p,
+                   h_nodes, loops.p, cm.p, cr.p, cc.p, geom_off.p, rbase.p, cbase.p, part_off.p, ring_off.p, reinterpret_cast<double2 *>(oxy.p));
     GPL_CUDA(cudaMemcpyAsync(part_off.p + h_tot[0], rbase.p + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
     GPL_CUDA(cudaMemcpyAsync(ring_off.p + h_tot[1], cbase.p + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
     GPL_TRY(bm.get(ctx, (size_t)(n + 7) / 8));
@@ -277,7 +281,9 @@ using namespace gpl;
 
 extern "C" int gpl_boolean_op(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, int op, gpl_array **out) {
     GPL_REQUIRE(ctx && a && b && out, GPL_ERR_INVALID_ARG, "gpl_boolean_op: NULL argument");
-    GPL_REQUIRE(op == GPL_BOOLEAN_INTERSECTION || op == GPL_BOOLEAN_UNION || op == GPL_BOOLEAN_DIFFERENCE, GPL_ERR_INVALID_ARG,
+    GPL_REQUIRE(op == GPL_BOOLEAN_INTERSECTION || op == GPL_BOOLEAN_UNION || op == GPL_BOOLEAN_DIFFERENCE ||
+                    op == GPL_BOOLEAN_SYMMETRIC_DIFFERENCE,
+                GPL_ERR_INVALID_ARG,
                 "gpl_boolean_op: unknown op %d", op);
     GPL_REQUIRE(is_area(a->type) && is_area(b->type), GPL_ERR_INVALID_TYPE, "Expected (Multi)Polygon x (Multi)Polygon (found %s x %s)",
                 type_name(a->type), type_name(b->type));

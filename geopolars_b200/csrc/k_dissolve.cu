@@ -23,6 +23,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <memory>
 
 #include "boolean.cuh"
 #include "common.cuh"
@@ -148,20 +149,20 @@ struct DisLess {
 };
 
 // per row: 0 skipped (null, code -1), 1 present, 2 present with a non-finite coordinate (nulls its group); the row of
-// every ring
+// every ring.  group NULL: every row in group 0, and gnull (then NULL too) is not written
 __global__ void __launch_bounds__(128) k_dis_rows(int64_t n, Side v, const int64_t *__restrict__ mem, const uint8_t *__restrict__ valid,
                                                   const int64_t *__restrict__ group, uint8_t *__restrict__ status, uint8_t *__restrict__ gnull,
                                                   int64_t *__restrict__ ring_row) {
     const int lane = threadIdx.x & 31;
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t r = warp; r < n; r += nwarps) {
-        const int64_t m0 = mem ? mem[r] : r, m1 = mem ? mem[r + 1] : r + 1, g = group[r];
+        const int64_t m0 = mem ? mem[r] : r, m1 = mem ? mem[r + 1] : r + 1, g = group ? group[r] : 0;
         for (int64_t e = v.go[m0] + lane; e < v.go[m1]; e += 32) ring_row[e] = r;
         const bool present = g >= 0 && bit_get(valid, r);
         const bool finite = present ? members_finite(v, m0, m1, lane) : true;
         if (lane == 0) {
             status[r] = !present ? 0 : finite ? 1 : 2;
-            if (present && !finite) gnull[g] = 1;
+            if (present && !finite && gnull) gnull[g] = 1;
         }
     }
 }
@@ -217,23 +218,26 @@ __global__ void __launch_bounds__(256) k_lower_bounds(const uint64_t *__restrict
         out[k] = lo;
     }
 }
+// the partner list of position p: partners[poff[q] .. poff[q + 1]) with q = pkey[p] (dissolve: the row), or q = p when pkey
+// is NULL (remainder: the partners depend on the group)
+__device__ __forceinline__ int64_t pos_key(const uint64_t *pkey, int64_t p) { return pkey ? (int64_t)pkey[p] : p; }
 // the items of the row at position p: its edge starts, then one per partner
-__global__ void __launch_bounds__(256) k_dis_item_count(int64_t m, const uint64_t *__restrict__ prow, const int64_t *__restrict__ poff,
+__global__ void __launch_bounds__(256) k_dis_item_count(int64_t m, const uint64_t *__restrict__ pkey, const int64_t *__restrict__ poff,
                                                         int64_t *__restrict__ cnt) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < m; p += stride) {
-        const int64_t r = (int64_t)prow[p];
-        cnt[p] = 1 + poff[r + 1] - poff[r];
+        const int64_t q = pos_key(pkey, p);
+        cnt[p] = 1 + poff[q + 1] - poff[q];
     }
 }
-__global__ void __launch_bounds__(256) k_dis_items(int64_t m, const uint64_t *__restrict__ prow, const int64_t *__restrict__ poff,
-                                                   const uint64_t *__restrict__ partners, const int64_t *__restrict__ ib, int64_t *__restrict__ irow,
-                                                   int64_t *__restrict__ ipart) {
+__global__ void __launch_bounds__(256) k_dis_items(int64_t m, const uint64_t *__restrict__ prow, const uint64_t *__restrict__ pkey,
+                                                   const int64_t *__restrict__ poff, const uint64_t *__restrict__ partners,
+                                                   const int64_t *__restrict__ ib, int64_t *__restrict__ irow, int64_t *__restrict__ ipart) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < m; p += stride) {
-        const int64_t r = (int64_t)prow[p], b = ib[p];
+        const int64_t r = (int64_t)prow[p], q = pos_key(pkey, p), b = ib[p];
         irow[b] = r, ipart[b] = -1;
-        for (int64_t t = poff[r]; t < poff[r + 1]; ++t) irow[b + 1 + t - poff[r]] = r, ipart[b + 1 + t - poff[r]] = (int64_t)partners[t];
+        for (int64_t t = poff[q]; t < poff[q + 1]; ++t) irow[b + 1 + t - poff[q]] = r, ipart[b + 1 + t - poff[q]] = (int64_t)partners[t];
     }
 }
 
@@ -298,9 +302,12 @@ __device__ int locate_row(const BOperands &o, int64_t j, double2 pt, double2 q, 
     return onb ? S_ON_OPP : S_OUT;
 }
 
-// One warp per row: sort the row's records, give every node met by several records one point, count the partners blocking
-// the piece after each record and keep the unblocked pieces
-__global__ void __launch_bounds__(kBoolThreads) k_dis_classify(int64_t m, BOperands o, const uint64_t *__restrict__ prow, const int64_t *__restrict__ ib,
+// One warp per position: sort the row's records, give every node met by several records one point, count the partners
+// blocking the piece after each record and keep the unblocked pieces.  pinv (NULL for dissolve): the position's inverted
+// partner, the subject of a remainder (§4.23), which blocks a cutter's piece unless the piece is strictly inside it; the
+// subject's own pieces are blocked by a cutter they are inside or on running the same way
+__global__ void __launch_bounds__(kBoolThreads) k_dis_classify(int64_t m, BOperands o, const uint64_t *__restrict__ prow, const uint64_t *__restrict__ pkey,
+                                                               const uint64_t *__restrict__ pinv, const int64_t *__restrict__ ib,
                                                                const int64_t *__restrict__ off, const int64_t *__restrict__ poff,
                                                                const uint64_t *__restrict__ partners, const int64_t *__restrict__ ring_row,
                                                                BNode *__restrict__ nodes, double *__restrict__ x4) {
@@ -308,7 +315,7 @@ __global__ void __launch_bounds__(kBoolThreads) k_dis_classify(int64_t m, BOpera
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     const DisLess less{&o, x4 + warp * kX4};
     for (int64_t p = warp; p < m; p += nwarps) {
-        const int64_t r = (int64_t)prow[p], o0 = off[ib[p]], o1 = off[ib[p + 1]];
+        const int64_t r = (int64_t)prow[p], q0 = pos_key(pkey, p), inv = pinv ? (int64_t)pinv[p] : -1, o0 = off[ib[p]], o1 = off[ib[p + 1]];
         if (o1 == o0) continue;
         BNode *nd = nodes + o0;
         const int64_t nn = o1 - o0;
@@ -362,13 +369,16 @@ __global__ void __launch_bounds__(kBoolThreads) k_dis_classify(int64_t m, BOpera
             if (n.kind == K_CROSS) {
                 double2 s, g;
                 dir_edge(o, 0, n.oring, n.oseg, s, g);
-                blocked += orient_sign(s, g, q) > 0 ? 1 : -1;  // entering the partner (its interior left of its edge) or leaving it
+                const int enter = orient_sign(s, g, q) > 0 ? 1 : -1;  // entering the partner (its interior left of its edge) or leaving it
+                blocked += inv >= 0 && ring_row[n.oring] == inv ? -enter : enter;
             } else {
                 blocked = 0;
-                for (int64_t t = poff[r]; t < poff[r + 1]; ++t) {
+                for (int64_t t = poff[q0]; t < poff[q0 + 1]; ++t) {
                     const int64_t j = (int64_t)partners[t];
                     const int st = locate_row(o, j, n.pt, q, lane);
-                    blocked += st == S_IN || st == S_ON_OPP || (st == S_ON_SAME && j < r);
+                    if (j == inv) blocked += st != S_IN;
+                    else if (r == inv) blocked += st == S_IN || st == S_ON_SAME;
+                    else blocked += st == S_IN || st == S_ON_OPP || (st == S_ON_SAME && j < r);
                 }
             }
             // a piece between two coincident vertices has no length
@@ -378,7 +388,7 @@ __global__ void __launch_bounds__(kBoolThreads) k_dis_classify(int64_t m, BOpera
             const bool empty = n.kind != K_CROSS && end_vertex && same_pt(n.pt, end);
             if (lane == 0) {
                 nd[k].side = 0;
-                nd[k].state = (int8_t)(blocked > 0 ? S_IN : S_OUT);
+                nd[k].state = (int8_t)(inv >= 0 && r != inv ? S_IN : S_OUT);  // S_IN: written reversed (a cutter's piece)
                 nd[k].keep = (!empty && blocked == 0) ? 1 : 0;
             }
         }
@@ -396,8 +406,9 @@ __global__ void __launch_bounds__(256) k_dis_groups(int64_t ng, const int64_t *_
     }
 }
 
-// One thread per group (§4.19's assembly over the group's records); a null group has no output
-template <bool WRITE>
+// One thread per group (§4.19's assembly over the group's records); a null group has no output.  BY_STATE (the remainders):
+// kept pieces in state S_IN, the cutters', are written reversed
+template <bool WRITE, bool BY_STATE>
 __global__ void __launch_bounds__(128) k_dis_assemble(int64_t ng, BOperands o, const int64_t *__restrict__ gnode, const uint8_t *__restrict__ gnull,
                                                       const BNode *__restrict__ nodes, int32_t *__restrict__ ws, int64_t ws_stride,
                                                       BLoop *__restrict__ loops, double4 *__restrict__ lbox, int64_t *__restrict__ cm,
@@ -408,7 +419,7 @@ __global__ void __launch_bounds__(128) k_dis_assemble(int64_t ng, BOperands o, c
     for (int64_t g = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; g < ng; g += stride) {
         const int64_t o0 = gnode[g], nn = gnull[g] ? 0 : gnode[g + 1] - o0;
         int64_t nm, nr, nc;
-        assemble_pieces<WRITE>(o, false, nodes + o0, nn, ws + o0, ws_stride, loops + o0, lbox + o0, nm, nr, nc, WRITE ? mbase[g] : 0,
+        assemble_pieces<WRITE, BY_STATE>(o, false, nodes + o0, nn, ws + o0, ws_stride, loops + o0, lbox + o0, nm, nr, nc, WRITE ? mbase[g] : 0,
                                WRITE ? rbase[g] : 0, WRITE ? cbase[g] : 0, part_off, ring_off, oxy);
         if (!WRITE) cm[g] = nm, cr[g] = nr, cc[g] = nc;
     }
@@ -422,6 +433,251 @@ __global__ void __launch_bounds__(256) k_dis_check_codes(int64_t n, const int64_
 __global__ void __launch_bounds__(256) k_dis_valid(int64_t ng, const uint8_t *__restrict__ gnull, uint8_t *__restrict__ rv) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t g = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; g < ng; g += stride) rv[g] = gnull[g] ? 0 : 1;
+}
+
+// The union pipeline over groups of positions (§4.21; the remainders of §4.23 run it too).  Positions [0, m) are rows
+// prow[p] of the one column o reads on both sides, ordered by group (gpos[g]: the first position of group g, gpos[ng] = m)
+// and by row within a group.  The partners of position p are partners[poff[q] .. poff[q + 1]), q = pkey[p] (p when pkey is
+// NULL), and pinv[p] (none when pinv is NULL) is its inverted partner.  *out: the MultiPolygon column of the ng groups, row g
+// null when gnull[g].
+static int group_rings(gpl_ctx *ctx, const BOperands &o, int64_t ng, const int64_t *gpos, int64_t m, const uint64_t *prow,
+                       const uint64_t *pkey, const uint64_t *pinv, const int64_t *poff, const uint64_t *partners,
+                       const int64_t *ring_row, const uint8_t *gnull, const char *who, gpl_array **out) {
+    Scratch<int> flag;
+    GPL_TRY(flag.get(ctx, 2));
+    GPL_CUDA(cudaMemsetAsync(flag.p, 0, 2 * sizeof(int), ctx->stream));
+    Scratch<int64_t> icnt, ib, tot;
+    GPL_TRY(icnt.get(ctx, (size_t)m));
+    GPL_TRY(ib.get(ctx, (size_t)m + 1));
+    GPL_TRY(tot.get(ctx, 3));
+    if (m > 0) GPL_LAUNCH(ctx, k_dis_item_count, flat_grid(m), 256, 0, m, pkey, poff, icnt.p);
+    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, icnt.p, m, ib.p, tot.p)));
+    int64_t ni = 0;
+    GPL_CUDA(cudaMemcpyAsync(&ni, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    Scratch<int64_t> irow, ipart, ncnt, noff;
+    GPL_TRY(irow.get(ctx, (size_t)ni));
+    GPL_TRY(ipart.get(ctx, (size_t)ni));
+    GPL_TRY(ncnt.get(ctx, (size_t)ni));
+    GPL_TRY(noff.get(ctx, (size_t)ni + 1));
+    if (m > 0) GPL_LAUNCH(ctx, k_dis_items, flat_grid(m), 256, 0, m, prow, pkey, poff, partners, ib.p, irow.p, ipart.p);
+    // nodes: count, scan, write
+    const int igrid = warp_grid(ni, kBoolThreads / 32);
+    if (ni > 0) GPL_LAUNCH(ctx, k_dis_nodes<false>, igrid, kBoolThreads, 0, ni, o, irow.p, ipart.p, ncnt.p, nullptr, nullptr, flag.p);
+    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, ncnt.p, ni, noff.p, tot.p)));
+    Scratch<int64_t> gnode;
+    GPL_TRY(gnode.get(ctx, (size_t)ng + 1));
+    GPL_LAUNCH(ctx, k_dis_groups, flat_grid(ng + 1), 256, 0, ng, gpos, ib.p, noff.p, gnode.p, flag.p + 1);
+    int64_t h_nodes = 0;
+    int h_big[2] = {0, 0};
+    GPL_CUDA(cudaMemcpyAsync(&h_nodes, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaMemcpyAsync(h_big, flag.p, sizeof(h_big), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    GPL_REQUIRE(!h_big[0] && !h_big[1], GPL_ERR_UNSUPPORTED, "%s: a group has 2^30 or more boundary nodes", who);
+    Scratch<BNode> nodes;
+    Scratch<int32_t> ws;
+    Scratch<BLoop> loops;
+    Scratch<double4> lbox;
+    Scratch<double> x4;
+    GPL_TRY(nodes.get(ctx, (size_t)h_nodes));
+    GPL_TRY(ws.get(ctx, (size_t)h_nodes * 8));
+    GPL_TRY(loops.get(ctx, (size_t)h_nodes));
+    GPL_TRY(lbox.get(ctx, (size_t)h_nodes));
+    const int cgrid = warp_grid(m, kBoolThreads / 32);
+    GPL_TRY(x4.get(ctx, (size_t)cgrid * (kBoolThreads / 32) * kX4));
+    if (ni > 0) GPL_LAUNCH(ctx, k_dis_nodes<true>, igrid, kBoolThreads, 0, ni, o, irow.p, ipart.p, ncnt.p, noff.p, nodes.p, flag.p);
+    if (m > 0)
+        GPL_LAUNCH(ctx, k_dis_classify, cgrid, kBoolThreads, 0, m, o, prow, pkey, pinv, ib.p, noff.p, poff, partners, ring_row, nodes.p, x4.p);
+    // assembly: counts, scans, write
+    Scratch<int64_t> cm, cr, cc, geom_off, rbase, cbase, part_off, ring_off;
+    Scratch<double> oxy;
+    Scratch<uint8_t> rv, bm;
+    GPL_TRY(cm.get(ctx, (size_t)ng));
+    GPL_TRY(cr.get(ctx, (size_t)ng));
+    GPL_TRY(cc.get(ctx, (size_t)ng));
+    GPL_TRY(geom_off.get(ctx, (size_t)ng + 1));
+    GPL_TRY(rbase.get(ctx, (size_t)ng + 1));
+    GPL_TRY(cbase.get(ctx, (size_t)ng + 1));
+    const int tgrid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(ng, 128), (int64_t)kSMs * 16));
+    if (ng > 0)
+        GPL_LAUNCH(ctx, (pinv ? k_dis_assemble<false, true> : k_dis_assemble<false, false>), tgrid, 128, 0, ng, o, gnode.p, gnull, nodes.p, ws.p, h_nodes, loops.p, lbox.p, cm.p, cr.p, cc.p,
+                   nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cm.p, ng, geom_off.p, tot.p)));
+    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cr.p, ng, rbase.p, tot.p + 1)));
+    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cc.p, ng, cbase.p, tot.p + 2)));
+    int64_t h_tot[3] = {0, 0, 0};
+    GPL_CUDA(cudaMemcpyAsync(h_tot, tot.p, sizeof(h_tot), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    GPL_TRY(part_off.get(ctx, (size_t)h_tot[0] + 1));
+    GPL_TRY(ring_off.get(ctx, (size_t)h_tot[1] + 1));
+    GPL_TRY(oxy.get(ctx, (size_t)h_tot[2] * 2));
+    if (ng > 0)
+        GPL_LAUNCH(ctx, (pinv ? k_dis_assemble<true, true> : k_dis_assemble<true, false>), tgrid, 128, 0, ng, o, gnode.p, gnull, nodes.p, ws.p, h_nodes, loops.p, lbox.p, cm.p, cr.p, cc.p,
+                   geom_off.p, rbase.p, cbase.p, part_off.p, ring_off.p, reinterpret_cast<double2 *>(oxy.p));
+    GPL_CUDA(cudaMemcpyAsync(part_off.p + h_tot[0], rbase.p + ng, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
+    GPL_CUDA(cudaMemcpyAsync(ring_off.p + h_tot[1], cbase.p + ng, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
+    GPL_TRY(rv.get(ctx, (size_t)ng));
+    GPL_TRY(bm.get(ctx, (size_t)(ng + 7) / 8));
+    if (ng > 0) {
+        GPL_LAUNCH(ctx, k_dis_valid, flat_grid(ng), 256, 0, ng, gnull, rv.p);
+        GPL_TRY(pack_bits(ctx, rv.p, bm.p, ng));
+    }
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
+    gpl_array *res = array_new(ctx, GPL_MULTIPOLYGON);
+    res->n_geoms = ng, res->n_parts = h_tot[0], res->n_rings = h_tot[1], res->n_coords = h_tot[2];
+    res->geom_off = geom_off.take(), res->own_geom = true;
+    res->part_off = part_off.take(), res->own_part = true;
+    res->ring_off = ring_off.take(), res->own_ring = true;
+    res->xy = oxy.take(), res->own_xy = true;
+    res->validity = bm.take(), res->own_valid = true;
+    *out = res;
+    return GPL_OK;
+}
+
+// ---- remainders (§4.23): subject i minus the union of the cutters C(i) it intersects, as a group of positions of the
+// concatenated column (subjects [0, ns), then cutters ns + j), so the subject's row is below every cutter's and its stored
+// edge comes first in every crossing point, as in gpl_boolean_op(s, c, difference)
+
+// the positions: every present subject i and, for each candidate pair (i, j) of present rows, the cutter ns + j, grouped by
+// subject for pair_list
+__global__ void __launch_bounds__(256) k_rem_pos_count(int64_t ncand, const uint64_t *__restrict__ l, const uint64_t *__restrict__ r, int64_t ns,
+                                                       const uint8_t *__restrict__ status, int32_t *__restrict__ cnt) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < ncand + ns; k += stride) {
+        const int64_t i = k < ncand ? (int64_t)l[k] : k - ncand, j = k < ncand ? ns + (int64_t)r[k] : i;
+        if (status[i] == 1 && status[j] == 1) atomicAdd(&cnt[i], 1);
+    }
+}
+__global__ void __launch_bounds__(256) k_rem_pos_write(int64_t ncand, const uint64_t *__restrict__ l, const uint64_t *__restrict__ r, int64_t ns,
+                                                       const uint8_t *__restrict__ status, const int64_t *__restrict__ off,
+                                                       int32_t *__restrict__ cursor, int32_t *__restrict__ raw) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < ncand + ns; k += stride) {
+        const int64_t i = k < ncand ? (int64_t)l[k] : k - ncand, j = k < ncand ? ns + (int64_t)r[k] : i;
+        if (status[i] == 1 && status[j] == 1) raw[off[i] + atomicAdd(&cursor[i], 1)] = (int32_t)j;
+    }
+}
+
+// The partners of position p = (subject i, row r), ascending: a subject's are its cutters (the other positions of its group);
+// a cutter's are the subject and the cutters of the group it intersects (ccr[ccoff[j] .. ccoff[j + 1]): the cutter x cutter
+// candidates of cutter j, membership by binary search in the group).  out NULL: count only.
+__device__ int64_t rem_partners(int64_t p, int64_t ns, const uint64_t *pgrp, const uint64_t *prow, const int64_t *gpos, const uint64_t *ccr,
+                                const int64_t *ccoff, uint64_t *out) {
+    const int64_t i = (int64_t)pgrp[p], r = (int64_t)prow[p], g0 = gpos[i] + 1, g1 = gpos[i + 1];
+    if (r == i) {
+        if (out)
+            for (int64_t t = g0; t < g1; ++t) out[t - g0] = prow[t];
+        return g1 - g0;
+    }
+    int64_t c = 0;
+    if (out) out[c] = (uint64_t)i;
+    ++c;
+    for (int64_t t = ccoff[r - ns]; t < ccoff[r - ns + 1]; ++t) {
+        const int64_t k = ns + (int64_t)ccr[t];
+        if (k == r) continue;
+        int64_t lo = g0, hi = g1;
+        while (lo < hi) {
+            const int64_t mid = (lo + hi) >> 1;
+            if ((int64_t)prow[mid] < k) lo = mid + 1;
+            else hi = mid;
+        }
+        if (lo < g1 && (int64_t)prow[lo] == k) {
+            if (out) out[c] = (uint64_t)k;
+            ++c;
+        }
+    }
+    return c;
+}
+__global__ void __launch_bounds__(256) k_rem_partner_count(int64_t m, int64_t ns, const uint64_t *__restrict__ pgrp, const uint64_t *__restrict__ prow,
+                                                           const int64_t *__restrict__ gpos, const uint64_t *__restrict__ ccr,
+                                                           const int64_t *__restrict__ ccoff, int64_t *__restrict__ cnt) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < m; p += stride) cnt[p] = rem_partners(p, ns, pgrp, prow, gpos, ccr, ccoff, nullptr);
+}
+__global__ void __launch_bounds__(256) k_rem_partner_write(int64_t m, int64_t ns, const uint64_t *__restrict__ pgrp, const uint64_t *__restrict__ prow,
+                                                           const int64_t *__restrict__ gpos, const uint64_t *__restrict__ ccr,
+                                                           const int64_t *__restrict__ ccoff, const int64_t *__restrict__ poff,
+                                                           uint64_t *__restrict__ partners) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < m; p += stride) rem_partners(p, ns, pgrp, prow, gpos, ccr, ccoff, partners + poff[p]);
+}
+// output row k of the concatenation: row k of source 0, then row k - ns of source 1
+__global__ void __launch_bounds__(256) k_concat_index(int64_t ns, int64_t n, int8_t *__restrict__ src, uint64_t *__restrict__ row) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += stride) src[k] = k < ns ? 0 : 1, row[k] = (uint64_t)(k < ns ? k : k - ns);
+}
+
+int remainder_rows(gpl_ctx *ctx, const gpl_array *subj, const gpl_array *cut, gpl_array **out) {
+    const int64_t ns = subj->n_geoms, nc = cut->n_geoms, n = ns + nc;
+    Pairs cand(nullptr, gpl_pairs_free), cc(nullptr, gpl_pairs_free);
+    GPL_TRY(join_candidate_pairs(ctx, subj, cut, JOIN_INTERSECTS, "gpl_overlay", false, cand));
+    GPL_TRY(join_candidate_pairs(ctx, cut, cut, JOIN_INTERSECTS, "gpl_overlay", false, cc));
+    // the concatenated column, read on both sides
+    Scratch<int8_t> csrc;
+    Scratch<uint64_t> crow;
+    GPL_TRY(csrc.get(ctx, (size_t)n));
+    GPL_TRY(crow.get(ctx, (size_t)n));
+    if (n > 0) GPL_LAUNCH(ctx, k_concat_index, flat_grid(n), 256, 0, ns, n, csrc.p, crow.p);
+    const gpl_array *srcs[3] = {subj, cut, nullptr};
+    gpl_array *both_raw = nullptr;
+    GPL_TRY(gather_polygons(ctx, srcs, csrc.p, crow.p, n, &both_raw));
+    std::unique_ptr<gpl_array, void (*)(gpl_array *)> both(both_raw, gpl_array_free);
+    RingPrep pr;
+    GPL_TRY(ring_prep(ctx, both.get(), pr));
+    BOperands o;
+    o.v[0] = o.v[1] = pr.view;
+    o.mem[0] = o.mem[1] = pr.members;
+    o.valid[0] = o.valid[1] = both->validity;
+    o.sg[0] = o.sg[1] = pr.sigma.p;
+    o.box[0] = o.box[1] = pr.box.p;
+    Scratch<uint8_t> status;
+    Scratch<int64_t> ring_row;
+    GPL_TRY(status.get(ctx, (size_t)n));
+    GPL_TRY(ring_row.get(ctx, (size_t)both->n_rings));
+    if (n > 0) GPL_LAUNCH(ctx, k_dis_rows, warp_grid(n, 4), 128, 0, n, pr.view, pr.members, both->validity, nullptr, status.p, nullptr, ring_row.p);
+    // positions, sorted by (subject, row): the subject first
+    const int64_t ncand = cand->n;
+    Scratch<int32_t> cursor;
+    GPL_TRY(cursor.get(ctx, (size_t)ns));
+    gpl_pairs *plist_raw = nullptr;
+    GPL_TRY(pair_list(
+        ctx, ns, false, &plist_raw,
+        [&](int32_t *cnt) -> int {
+            GPL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int32_t) * (size_t)ns, ctx->stream));
+            GPL_LAUNCH(ctx, k_rem_pos_count, flat_grid(ncand + ns), 256, 0, ncand, cand->lhs, cand->rhs, ns, status.p, cnt);
+            return GPL_OK;
+        },
+        [&](const int64_t *off, int32_t *raw, double *) -> int {
+            GPL_CUDA(cudaMemsetAsync(cursor.p, 0, sizeof(int32_t) * (size_t)ns, ctx->stream));
+            GPL_LAUNCH(ctx, k_rem_pos_write, flat_grid(ncand + ns), 256, 0, ncand, cand->lhs, cand->rhs, ns, status.p, off, cursor.p, raw);
+            return GPL_OK;
+        }));
+    Pairs plist(plist_raw, gpl_pairs_free);
+    cand.reset();
+    const int64_t m = plist->n;
+    Scratch<int64_t> gpos, ccoff, pcnt, poff, tot;
+    GPL_TRY(gpos.get(ctx, (size_t)ns + 1));
+    GPL_TRY(ccoff.get(ctx, (size_t)nc + 1));
+    GPL_TRY(pcnt.get(ctx, (size_t)m));
+    GPL_TRY(poff.get(ctx, (size_t)m + 1));
+    GPL_TRY(tot.get(ctx, 1));
+    GPL_LAUNCH(ctx, k_lower_bounds, flat_grid(ns + 1), 256, 0, plist->lhs, m, ns, gpos.p);
+    GPL_LAUNCH(ctx, k_lower_bounds, flat_grid(nc + 1), 256, 0, cc->lhs, cc->n, nc, ccoff.p);
+    if (m > 0) GPL_LAUNCH(ctx, k_rem_partner_count, flat_grid(m), 256, 0, m, ns, plist->lhs, plist->rhs, gpos.p, cc->rhs, ccoff.p, pcnt.p);
+    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, pcnt.p, m, poff.p, tot.p)));
+    int64_t h_part = 0;
+    GPL_CUDA(cudaMemcpyAsync(&h_part, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    Scratch<uint64_t> partners;
+    GPL_TRY(partners.get(ctx, (size_t)h_part));
+    if (m > 0)
+        GPL_LAUNCH(ctx, k_rem_partner_write, flat_grid(m), 256, 0, m, ns, plist->lhs, plist->rhs, gpos.p, cc->rhs, ccoff.p, poff.p, partners.p);
+    // the subject of each position (its group) is its inverted partner; no remainder is null (a null or non-finite subject has
+    // no position)
+    Scratch<uint8_t> gnull;
+    GPL_TRY(gnull.get(ctx, (size_t)ns));
+    GPL_CUDA(cudaMemsetAsync(gnull.p, 0, (size_t)ns, ctx->stream));
+    return group_rings(ctx, o, ns, gpos.p, m, plist->rhs, nullptr, plist->lhs, poff.p, partners.p, ring_row.p, gnull.p, "overlay", out);
 }
 
 }  // namespace gpl
@@ -443,8 +699,8 @@ extern "C" int gpl_dissolve(gpl_ctx *ctx, const gpl_array *in, const int64_t *gr
     Scratch<int64_t> dgroup;
     const int64_t *grp = group;
     Scratch<int> flag;
-    GPL_TRY(flag.get(ctx, 2));
-    GPL_CUDA(cudaMemsetAsync(flag.p, 0, 2 * sizeof(int), ctx->stream));
+    GPL_TRY(flag.get(ctx, 1));
+    GPL_CUDA(cudaMemsetAsync(flag.p, 0, sizeof(int), ctx->stream));
     if (mem == GPL_HOST) {
         GPL_TRY(dgroup.get(ctx, (size_t)n));
         if (n) GPL_CUDA(cudaMemcpyAsync(dgroup.p, group, sizeof(int64_t) * (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
@@ -512,93 +768,8 @@ extern "C" int gpl_dissolve(gpl_ctx *ctx, const gpl_array *in, const int64_t *gr
         }));
     Pairs glist(glist_raw, gpl_pairs_free);
     const int64_t m = glist->n;
-    const uint64_t *prow = glist->rhs;
-    Scratch<int64_t> gpos, icnt, ib, tot;
+    Scratch<int64_t> gpos;
     GPL_TRY(gpos.get(ctx, (size_t)ng + 1));
-    GPL_TRY(icnt.get(ctx, (size_t)m));
-    GPL_TRY(ib.get(ctx, (size_t)m + 1));
-    GPL_TRY(tot.get(ctx, 3));
     GPL_LAUNCH(ctx, k_lower_bounds, flat_grid(ng + 1), 256, 0, glist->lhs, m, ng, gpos.p);
-    if (m > 0) GPL_LAUNCH(ctx, k_dis_item_count, flat_grid(m), 256, 0, m, prow, poff.p, icnt.p);
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, icnt.p, m, ib.p, tot.p)));
-    int64_t ni = 0;
-    GPL_CUDA(cudaMemcpyAsync(&ni, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    Scratch<int64_t> irow, ipart, ncnt, noff;
-    GPL_TRY(irow.get(ctx, (size_t)ni));
-    GPL_TRY(ipart.get(ctx, (size_t)ni));
-    GPL_TRY(ncnt.get(ctx, (size_t)ni));
-    GPL_TRY(noff.get(ctx, (size_t)ni + 1));
-    if (m > 0) GPL_LAUNCH(ctx, k_dis_items, flat_grid(m), 256, 0, m, prow, poff.p, plist->rhs, ib.p, irow.p, ipart.p);
-    // nodes: count, scan, write
-    const int igrid = warp_grid(ni, kBoolThreads / 32);
-    if (ni > 0) GPL_LAUNCH(ctx, k_dis_nodes<false>, igrid, kBoolThreads, 0, ni, o, irow.p, ipart.p, ncnt.p, nullptr, nullptr, flag.p);
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, ncnt.p, ni, noff.p, tot.p)));
-    Scratch<int64_t> gnode;
-    GPL_TRY(gnode.get(ctx, (size_t)ng + 1));
-    GPL_LAUNCH(ctx, k_dis_groups, flat_grid(ng + 1), 256, 0, ng, gpos.p, ib.p, noff.p, gnode.p, flag.p + 1);
-    int64_t h_nodes = 0;
-    int h_big[2] = {0, 0};
-    GPL_CUDA(cudaMemcpyAsync(&h_nodes, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaMemcpyAsync(h_big, flag.p, sizeof(h_big), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    GPL_REQUIRE(!h_big[0] && !h_big[1], GPL_ERR_UNSUPPORTED, "dissolve: a group has 2^30 or more boundary nodes");
-    Scratch<BNode> nodes;
-    Scratch<int32_t> ws;
-    Scratch<BLoop> loops;
-    Scratch<double4> lbox;
-    Scratch<double> x4;
-    GPL_TRY(nodes.get(ctx, (size_t)h_nodes));
-    GPL_TRY(ws.get(ctx, (size_t)h_nodes * 8));
-    GPL_TRY(loops.get(ctx, (size_t)h_nodes));
-    GPL_TRY(lbox.get(ctx, (size_t)h_nodes));
-    const int cgrid = warp_grid(m, kBoolThreads / 32);
-    GPL_TRY(x4.get(ctx, (size_t)cgrid * (kBoolThreads / 32) * kX4));
-    if (ni > 0) GPL_LAUNCH(ctx, k_dis_nodes<true>, igrid, kBoolThreads, 0, ni, o, irow.p, ipart.p, ncnt.p, noff.p, nodes.p, flag.p);
-    if (m > 0)
-        GPL_LAUNCH(ctx, k_dis_classify, cgrid, kBoolThreads, 0, m, o, prow, ib.p, noff.p, poff.p, plist->rhs, ring_row.p, nodes.p, x4.p);
-    // assembly: counts, scans, write
-    Scratch<int64_t> cm, cr, cc, geom_off, rbase, cbase, part_off, ring_off;
-    Scratch<double> oxy;
-    Scratch<uint8_t> rv, bm;
-    GPL_TRY(cm.get(ctx, (size_t)ng));
-    GPL_TRY(cr.get(ctx, (size_t)ng));
-    GPL_TRY(cc.get(ctx, (size_t)ng));
-    GPL_TRY(geom_off.get(ctx, (size_t)ng + 1));
-    GPL_TRY(rbase.get(ctx, (size_t)ng + 1));
-    GPL_TRY(cbase.get(ctx, (size_t)ng + 1));
-    const int tgrid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(ng, 128), (int64_t)kSMs * 16));
-    if (ng > 0)
-        GPL_LAUNCH(ctx, k_dis_assemble<false>, tgrid, 128, 0, ng, o, gnode.p, gnull.p, nodes.p, ws.p, h_nodes, loops.p, lbox.p, cm.p, cr.p, cc.p,
-                   nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cm.p, ng, geom_off.p, tot.p)));
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cr.p, ng, rbase.p, tot.p + 1)));
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cc.p, ng, cbase.p, tot.p + 2)));
-    int64_t h_tot[3] = {0, 0, 0};
-    GPL_CUDA(cudaMemcpyAsync(h_tot, tot.p, sizeof(h_tot), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    GPL_TRY(part_off.get(ctx, (size_t)h_tot[0] + 1));
-    GPL_TRY(ring_off.get(ctx, (size_t)h_tot[1] + 1));
-    GPL_TRY(oxy.get(ctx, (size_t)h_tot[2] * 2));
-    if (ng > 0)
-        GPL_LAUNCH(ctx, k_dis_assemble<true>, tgrid, 128, 0, ng, o, gnode.p, gnull.p, nodes.p, ws.p, h_nodes, loops.p, lbox.p, cm.p, cr.p, cc.p,
-                   geom_off.p, rbase.p, cbase.p, part_off.p, ring_off.p, reinterpret_cast<double2 *>(oxy.p));
-    GPL_CUDA(cudaMemcpyAsync(part_off.p + h_tot[0], rbase.p + ng, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    GPL_CUDA(cudaMemcpyAsync(ring_off.p + h_tot[1], cbase.p + ng, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    GPL_TRY(rv.get(ctx, (size_t)ng));
-    GPL_TRY(bm.get(ctx, (size_t)(ng + 7) / 8));
-    if (ng > 0) {
-        GPL_LAUNCH(ctx, k_dis_valid, flat_grid(ng), 256, 0, ng, gnull.p, rv.p);
-        GPL_TRY(pack_bits(ctx, rv.p, bm.p, ng));
-    }
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
-    gpl_array *res = array_new(ctx, GPL_MULTIPOLYGON);
-    res->n_geoms = ng, res->n_parts = h_tot[0], res->n_rings = h_tot[1], res->n_coords = h_tot[2];
-    res->geom_off = geom_off.take(), res->own_geom = true;
-    res->part_off = part_off.take(), res->own_part = true;
-    res->ring_off = ring_off.take(), res->own_ring = true;
-    res->xy = oxy.take(), res->own_xy = true;
-    res->validity = bm.take(), res->own_valid = true;
-    *out = res;
-    return GPL_OK;
+    return group_rings(ctx, o, ng, gpos.p, m, glist->rhs, glist->rhs, nullptr, poff.p, plist->rhs, ring_row.p, gnull.p, "dissolve", out);
 }

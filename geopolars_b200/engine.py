@@ -455,15 +455,16 @@ def overlay_area_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, n
     return _take_pairs(lhs.ctx, h, True)
 
 
-BOOLEAN_OPS = {"intersection": 0, "union": 1, "difference": 2}
+BOOLEAN_OPS = {"intersection": 0, "union": 1, "difference": 2, "symmetric_difference": 3}
 
 
 def boolean_op(a: DeviceArray, b: DeviceArray, op: str) -> DeviceArray:
-    """row-wise intersection, union or difference (a - b) of two (Multi)Polygon columns as a MultiPolygon column
-    (DESIGN.md §4.19): geo's BooleanOps; a null or non-finite row gives a null row, an empty result an empty MultiPolygon"""
+    """row-wise intersection, union, difference (a - b) or symmetric difference of two (Multi)Polygon columns as a
+    MultiPolygon column (DESIGN.md §4.19, §4.23): geo's BooleanOps; a null or non-finite row gives a null row, an empty result
+    an empty MultiPolygon"""
     code = BOOLEAN_OPS.get(op)
     if code is None:
-        raise ValueError("op must be 'intersection', 'union' or 'difference'")
+        raise ValueError("op must be 'intersection', 'union', 'difference' or 'symmetric_difference'")
     return _out_array(a.ctx, a.ctx.lib.gpl_boolean_op, a._h, b._h, code)
 
 
@@ -473,6 +474,26 @@ def overlay_join(lhs: DeviceArray, rhs: DeviceArray) -> Tuple[np.ndarray, np.nda
     ctx = lhs.ctx
     hp, ha = C.c_void_p(), C.c_void_p()
     check(ctx.lib.gpl_overlay_join(ctx._h, lhs._h, rhs._h, C.byref(hp), C.byref(ha)))
+    geoms = DeviceArray(ctx, ha)
+    a, b = _take_pairs(ctx, hp)
+    return a, b, geoms
+
+
+OVERLAY_HOWS = {"intersection": 0, "union": 1, "identity": 2, "symmetric_difference": 3, "difference": 4}
+ABSENT = np.uint64(0xFFFFFFFFFFFFFFFF)
+
+
+def overlay(lhs: DeviceArray, rhs: DeviceArray, how: str = "intersection") -> Tuple[np.ndarray, np.ndarray, DeviceArray]:
+    """(lhs uint64, rhs uint64, MultiPolygon column) of GeoPandas' overlay(lhs, rhs, how) for two (Multi)Polygon columns
+    (DESIGN.md §4.23): intersection rows (i, j) as `overlay_join` gives them, left remainders (i, ABSENT) — lhs[i] minus every
+    rhs row it intersects — and right remainders (ABSENT, j), as `how` selects; remainders with no member are dropped.  Sorted
+    by (lhs, rhs) as unsigned values, ABSENT = 2^64 - 1 after every row index."""
+    code = OVERLAY_HOWS.get(how)
+    if code is None:
+        raise ValueError("how must be one of " + ", ".join(repr(k) for k in OVERLAY_HOWS))
+    ctx = lhs.ctx
+    hp, ha = C.c_void_p(), C.c_void_p()
+    check(ctx.lib.gpl_overlay(ctx._h, lhs._h, rhs._h, code, C.byref(hp), C.byref(ha)))
     geoms = DeviceArray(ctx, ha)
     a, b = _take_pairs(ctx, hp)
     return a, b, geoms

@@ -157,6 +157,25 @@ class GeoDataFrame:
         keys, geoms = dissolve(self.geometry, self._table.column(by))
         return GeoDataFrame(pa.table({by: keys, self._geometry_name: geoms.to_arrow()}), geometry=self._geometry_name)
 
+    def overlay(self, other: "GeoDataFrame", how: str = "intersection") -> "GeoDataFrame":
+        """GeoPandas' `overlay(self, other, how)` for two (Multi)Polygon frames, keep_geom_type=True (see `overlay` below): the
+        left columns, then the right columns, then the geometry (named as this frame's).  A remainder row's other-side
+        columns are null; a column name both frames have gets GeoPandas' suffixes, `_1` on the left and `_2` on the right, and
+        a right column named as this frame's geometry gets `_2`.
+        Attributes are not aggregated.  The rows are `overlay`'s, so their order differs from GeoPandas' (which concatenates
+        its parts) but the set of rows is the same.  Both frames' geometries must be valid (OGC); `is_valid()` tells."""
+        pa = _pa()
+        a, b, geoms = overlay(self.geometry, other.geometry, how)
+        lt = self._table.drop_columns([self._geometry_name])
+        rt = other._table.drop_columns([other._geometry_name])
+        lt = lt.take(pa.array(a, mask=a < 0))  # a null index takes a null row
+        rt = rt.take(pa.array(b, mask=b < 0))
+        common = set(lt.column_names) & set(rt.column_names)
+        names = [n + "_1" if n in common else n for n in lt.column_names]
+        names += [n + "_2" if n in common or n == self._geometry_name else n for n in rt.column_names]
+        cols = list(lt.columns) + list(rt.columns) + [geoms.to_arrow()]
+        return GeoDataFrame(pa.table(cols, names=names + [self._geometry_name]), geometry=self._geometry_name)
+
 
 def from_arrow(data):
     """geopolars.from_arrow (py-geopolars/python/geopolars/convert.py:33-56): a Table becomes a GeoDataFrame, an Array or
@@ -332,6 +351,12 @@ class GeoRustSeries:
     def difference(self, other: GeoSeries) -> GeoSeries:
         """row-wise difference self[i] - other[i] (GeoPandas' `a.difference(b)`), as `intersection`"""
         return self._wrap(E.boolean_op(self._d(), other.device, "difference"))
+
+    def symmetric_difference(self, other: GeoSeries) -> GeoSeries:
+        """row-wise symmetric difference of self[i] and other[i], the parts covered by exactly one of them (GeoPandas'
+        `a.symmetric_difference(b)`, geo's `BooleanOps::xor`; DESIGN.md §4.23), as `intersection`.  Members of
+        self[i] - other[i] and other[i] - self[i] that touch at a point stay separate members."""
+        return self._wrap(E.boolean_op(self._d(), other.device, "symmetric_difference"))
 
     def clip(self, mask: GeoSeries, invert: bool = False) -> GeoSeries:
         """row-wise clip of self[i], a (Multi)LineString or (Multi)Point column, by mask[i], a (Multi)Polygon column
@@ -571,6 +596,25 @@ def overlay_join(lhs: GeoSeries, rhs: GeoSeries):
     `lhs.geo.intersection` of the pair (DESIGN.md §4.19).  Valid (OGC) operands only; filter with `is_valid()` first."""
     a, b, g = E.overlay_join(lhs.device, rhs.device)
     return a.astype(np.int64), b.astype(np.int64), GeoSeries(_device=g, name=lhs.name)
+
+
+def overlay(lhs: GeoSeries, rhs: GeoSeries, how: str = "intersection"):
+    """GeoPandas' `overlay(lhs, rhs, how)` for two (Multi)Polygon columns, keep_geom_type=True (DESIGN.md §4.23):
+    (lhs_index int64, rhs_index int64, GeoSeries of MultiPolygons), -1 marking the absent side.  The rows are:
+
+    - intersection rows (i, j), for how 'intersection', 'identity' and 'union': exactly `overlay_join`'s rows;
+    - left remainders (i, -1), for every how but 'intersection': lhs[i] minus the union of every rhs row it intersects;
+    - right remainders (-1, j), for 'symmetric_difference' and 'union': rhs[j] minus every lhs row it intersects.
+
+    'difference' gives the left remainders alone.  A remainder with no member is dropped; null and non-finite rows have no
+    remainder and cut nothing.  Rows are sorted by (lhs, rhs) with -1 after every index: each left row's intersections, then
+    its remainder, then the right remainders.  GeoPandas concatenates its parts in another order, but the set of rows is the
+    same.  The operands must be valid (OGC); filter with `is_valid()` first."""
+    a, b, g = E.overlay(lhs.device, rhs.device, how)
+    la, lb = a.astype(np.int64), b.astype(np.int64)
+    la[a == E.ABSENT] = -1
+    lb[b == E.ABSENT] = -1
+    return la, lb, GeoSeries(_device=g, name=lhs.name)
 
 
 def clip_join(lhs: GeoSeries, rhs: GeoSeries):

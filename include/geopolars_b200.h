@@ -435,9 +435,9 @@ int gpl_intersection_area(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, 
 int gpl_overlay_area_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **out);
 
 /* ---------------------------------------------------------------- boolean geometry ------- */
-enum { GPL_BOOLEAN_INTERSECTION = 0, GPL_BOOLEAN_UNION = 1, GPL_BOOLEAN_DIFFERENCE = 2 };
-/* Intersection, union or difference (a - b) of the closed regions a[i] and b[i] (geo's BooleanOps::{intersection, union,
- * difference}), DESIGN.md §4.19: the regularised result (lower-dimensional contact is dropped) as a MultiPolygon column, always.
+enum { GPL_BOOLEAN_INTERSECTION = 0, GPL_BOOLEAN_UNION = 1, GPL_BOOLEAN_DIFFERENCE = 2, GPL_BOOLEAN_SYMMETRIC_DIFFERENCE = 3 };
+/* Intersection, union, difference (a - b) or symmetric difference ((a - b) ∪ (b - a)) of the closed regions a[i] and b[i]
+ * (geo's BooleanOps::{intersection, union, difference, xor}), DESIGN.md §4.19 and §4.23: the regularised result (lower-dimensional contact is dropped) as a MultiPolygon column, always.
  * Both columns Polygon or MultiPolygon, in any combination (else GPL_ERR_INVALID_TYPE); unequal lengths: GPL_ERR_LENGTH_MISMATCH;
  * any other op: GPL_ERR_INVALID_ARG; all before any launch.  Input rings are read as gpl_intersection_area reads them (any
  * orientation, closed implicitly, fewer than 4 coordinates after closing: no contribution).  A null row or a row with a
@@ -467,6 +467,29 @@ int gpl_overlay_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, g
  * a code outside [-1, n_groups) or n_groups < 0: GPL_ERR_INVALID_ARG; 2^31 or more rows or groups, or a group with 2^30 or more
  * boundary nodes: GPL_ERR_UNSUPPORTED. */
 int gpl_dissolve(gpl_ctx *ctx, const gpl_array *in, const int64_t *group, int mem, int64_t n_groups, gpl_array **out);
+enum {
+    GPL_OVERLAY_INTERSECTION = 0,
+    GPL_OVERLAY_UNION = 1,
+    GPL_OVERLAY_IDENTITY = 2,
+    GPL_OVERLAY_SYMMETRIC_DIFFERENCE = 3,
+    GPL_OVERLAY_DIFFERENCE = 4,
+};
+/* Overlay of two (Multi)Polygon columns (GeoPandas' overlay(lhs, rhs, how), keep_geom_type=True), DESIGN.md §4.23.  The rows
+ * are of three kinds:
+ *   intersection rows (i, j): bit for bit the rows of gpl_overlay_join (how INTERSECTION, IDENTITY, UNION);
+ *   left remainders (i, UINT64_MAX): lhs[i] minus the union of every rhs row it intersects (DIFFERENCE, IDENTITY,
+ *   SYMMETRIC_DIFFERENCE, UNION);
+ *   right remainders (UINT64_MAX, j): rhs[j] minus the union of every lhs row it intersects (SYMMETRIC_DIFFERENCE, UNION).
+ * A remainder with no member is dropped; a null lhs / rhs row, or one with a non-finite coordinate, has no remainder and cuts
+ * nothing.  A remainder with no cutter is bit for bit gpl_boolean_op(row, <empty row>, GPL_BOOLEAN_DIFFERENCE), and a left
+ * remainder with one cutter gpl_boolean_op(lhs[i], rhs[j], GPL_BOOLEAN_DIFFERENCE) except where a crossing passes through a
+ * vertex of another ring of the cutter.  *pairs is sorted by (lhs, rhs) as unsigned values (so a left row's intersections come
+ * before its remainder, and the right remainders last); *out is one MultiPolygon column aligned with it, every row valid, in
+ * gpl_boolean_op's output form.  Any other how: GPL_ERR_INVALID_ARG; any other type: GPL_ERR_INVALID_TYPE; 2^31 or more rows
+ * in the two columns together: GPL_ERR_UNSUPPORTED; all before any launch.  A remainder with 2^30 or more boundary nodes:
+ * GPL_ERR_UNSUPPORTED.  The operands must be valid (OGC); on invalid
+ * operands the output is well formed but not specified.  Deterministic. */
+int gpl_overlay(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, int how, gpl_pairs **pairs, gpl_array **out);
 
 /* ---------------------------------------------------------------- clipping ---------------- */
 /* Clip of a line or point column by a polygon column (GeoPandas' clip / overlay with lines, geo's BooleanOps::clip),

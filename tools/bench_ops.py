@@ -4,7 +4,7 @@ fraction for the coordinate bytes read, and of the nearest join (100 M points ag
 reference points and 1 M walk linestrings).  Not the flagship bench (that is bench.py, config 2); config 5 runs at
 4 M polygons so that its input and output columns fit one 80 GB H100.
 
-  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic|valid|boolean|relate|dissolve|clip] [--out ops_roofline.json]
+  python tools/bench_ops.py [--scale 1.0] [--only all|ops|nearest|nearest_geom|dwithin|geo|overlay|geodesic|valid|boolean|relate|dissolve|clip|overlay_modes] [--out ops_roofline.json]
 """
 import argparse
 import ctypes as C
@@ -41,12 +41,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scale", type=float, default=1.0, help="fraction of the BASELINE sizes")
     ap.add_argument("--out", default="ops_roofline.json")
-    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve", "clip"), default="all",
+    ap.add_argument("--only", choices=("all", "ops", "nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve", "clip", "overlay_modes"), default="all",
                     help="run only the §8 rows, only the point nearest join, only the geometry nearest join, only the "
                          "distance-within join, only the great-circle joins, only the intersection area and overlay join or "
                          "only the geodesic area and perimeter (1 M stars, 10 M parcels, naturalearth_lowres to 1 M rows), or only "
                          "the boolean geometry ops and the geometry overlay join, or only the DE-9IM relate, predicates and "
-                         "predicate join, or only dissolve / union_all, or only the line clip, intersection length and their joins; "
+                         "predicate join, or only dissolve / union_all, or only the line clip, intersection length and their joins, or "
+                         "only the symmetric difference and the five overlay modes; "
                          "'all' runs every arm")
     args = ap.parse_args()
     peak = 3350.0  # H100 SXM data sheet, replaced by a measured value when MEASURED_PEAKS.json exists
@@ -93,11 +94,13 @@ def main():
             dissolve_rows(args, ctx, dev, st, res)
         if args.only in ("all", "clip"):
             clip_rows(args, ctx, dev, st, res)
+        if args.only in ("all", "overlay_modes"):
+            overlay_modes_rows(args, ctx, dev, st, res)
         if args.only in ("all", "geodesic"):
             geodesic_rows(args, ctx, dev, st, res)
         if args.only in ("all", "valid"):
             valid_rows(args, ctx, dev, st, res)
-        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve", "clip"):
+        if args.only in ("nearest", "nearest_geom", "dwithin", "geo", "overlay", "geodesic", "valid", "boolean", "relate", "dissolve", "clip", "overlay_modes"):
             ctx.synchronize()
             _write(args, res)
             return
@@ -534,6 +537,24 @@ def boolean_rows(args, ctx, dev, st, res):
     rec("overlay_join (10 000 stars x %d squares)" % (k * k), n_pairs[0], "pairs", t, {})
 
 
+def phases(fn):
+    """the GPU time of each kernel of one call of fn (torch.profiler), in ms, the 12 largest"""
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    out = {}
+    for e in prof.key_averages():
+        t = getattr(e, "device_time_total", None)
+        if t is None:
+            t = getattr(e, "cuda_time_total", 0.0)
+        if t > 0:
+            key = e.key.split("<")[0].split("(")[0].replace("void ", "").replace("gpl::", "")
+            out[key] = round(out.get(key, 0.0) + t / 1e3, 3)
+    return dict(sorted(out.items(), key=lambda kv: -kv[1])[:12])
+
+
 def dissolve_rows(args, ctx, dev, st, res):
     """dissolve / union_all (DESIGN.md §4.21): 1 M two-row groups (config 2's stars and the same stars shifted by (3, 2)) beside
     the row-wise union of the same rows; the overlay round trip of the 10 000 stars (overlay_join with the 200 x 200 grid of
@@ -545,22 +566,6 @@ def dissolve_rows(args, ctx, dev, st, res):
     from geopolars_b200 import datasets, synth
 
     lib = ctx.lib
-
-    def phases(fn):
-        from torch.profiler import ProfilerActivity, profile
-
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        out = {}
-        for e in prof.key_averages():
-            t = getattr(e, "device_time_total", None)
-            if t is None:
-                t = getattr(e, "cuda_time_total", 0.0)
-            if t > 0:
-                key = e.key.split("<")[0].split("(")[0].replace("void ", "").replace("gpl::", "")
-                out[key] = round(out.get(key, 0.0) + t / 1e3, 3)
-        return dict(sorted(out.items(), key=lambda kv: -kv[1])[:12])
 
     def rec(name, units, unit_name, t, extra):
         r = {"op": name, "units": units, "unit": unit_name, "ms_min": t[0], "ms_avg": t[1], "units_per_s": units / (t[1] * 1e-3),
@@ -632,6 +637,86 @@ def dissolve_rows(args, ctx, dev, st, res):
     run = dissolve_call(ne, zeros, 1, size)
     t = timed(st, run, reps=3, warm=1)
     rec("union_all (naturalearth_lowres, %d rows)" % len(ne), len(ne), "rows", t, {"out_coords": size[0], "phases_ms": phases(run)})
+
+
+def overlay_modes_rows(args, ctx, dev, st, res):
+    """symmetric difference and the overlay modes (DESIGN.md §4.23): the row-wise symmetric difference of 1 M pairs of config
+    2's stars against the same stars shifted by (3, 2), beside the row-wise union of the same pairs; overlay in all five modes
+    of config 2's 10 000 stars against the same stars shifted by (3, 2); identity of naturalearth_lowres against the 5-degree
+    grid; difference of one large polygon (a 256-gon of radius 220 over the middle of 2 000 stars spread over 450 x 450) against
+    those stars, one remainder with about 1 500 cutters, which one thread assembles.  Each row carries the per-kernel GPU time of one call (torch.profiler)."""
+    import numpy as np
+
+    from geopolars_b200 import datasets, synth
+
+    lib = ctx.lib
+
+    def rec(name, units, unit_name, t, extra):
+        r = {"op": name, "units": units, "unit": unit_name, "ms_min": t[0], "ms_avg": t[1], "units_per_s": units / (t[1] * 1e-3),
+             "card": res["card"], "power_limit": res["power_limit"], **extra}
+        res["rows"].append(r)
+        print(json.dumps(r), flush=True)
+
+    def upload(xy, ring_off, geom_off):
+        t = [torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in (xy, ring_off, geom_off)]
+        n = len(geom_off) - 1
+        return ctx.wrap_device(GeometryType.POLYGON, n, len(xy), t[0].data_ptr(), geom_off_ptr=t[2].data_ptr(), ring_off_ptr=t[1].data_ptr(),
+                               n_rings=len(ring_off) - 1, keepalive=tuple(t))
+
+    def boolean_call(a, b, code, size):
+        def run():
+            h = C.c_void_p()
+            E.check(lib.gpl_boolean_op(ctx._h, a._h, b._h, code, C.byref(h)))
+            size[0] = int(E.DeviceArray(ctx, h).view().n_coords)
+        return run
+
+    def overlay_call(lhs, rhs, how, size):
+        def run():
+            hp, ha = C.c_void_p(), C.c_void_p()
+            E.check(lib.gpl_overlay(ctx._h, lhs._h, rhs._h, E.OVERLAY_HOWS[how], C.byref(hp), C.byref(ha)))
+            size[0] = int(lib.gpl_pairs_count(hp))
+            lib.gpl_pairs_free(hp)
+            E.DeviceArray(ctx, ha)
+        return run
+
+    size = [0]
+    n = int(1_000_000 * args.scale)
+    g = int(np.ceil(np.sqrt(n)))
+    xy, ro, go = synth.star_polygons(m=n, grid=g)
+    a, b = upload(xy, ro, go), upload(xy + np.array([3.0, 2.0]), ro, go)
+    for name, code in (("symmetric_difference", 3), ("union", 1)):
+        run = boolean_call(a, b, code, size)
+        t = timed(st, run, reps=3, warm=1)
+        rec("boolean_op %s (%d star pairs, 64 x 64 edges)" % (name, n), n, "row pairs", t, {"out_coords": size[0], "phases_ms": phases(run)})
+    del a, b
+
+    sxy, sro, sgo = synth.star_polygons()
+    stars, shifted = upload(sxy, sro, sgo), upload(sxy + np.array([3.0, 2.0]), sro, sgo)
+    for how in ("intersection", "union", "identity", "symmetric_difference", "difference"):
+        run = overlay_call(stars, shifted, how, size)
+        t = timed(st, run, reps=3, warm=1)
+        rec("overlay %s (10 000 stars x the same shifted by (3, 2))" % how, size[0], "rows", t, {"phases_ms": phases(run)})
+
+    k = 72 * 36
+    i, j = np.meshgrid(np.arange(72, dtype=np.float64), np.arange(36, dtype=np.float64), indexing="xy")
+    x0, y0 = -180.0 + i.ravel() * 5.0, -90.0 + j.ravel() * 5.0
+    gxy = np.stack([np.stack([x0, x0 + 5.0, x0 + 5.0, x0, x0], 1), np.stack([y0, y0, y0 + 5.0, y0 + 5.0, y0], 1)], 2).reshape(-1, 2)
+    cells = upload(gxy, np.arange(k + 1, dtype=np.int64) * 5, np.arange(k + 1, dtype=np.int64))
+    ne = datasets.read_dataset("naturalearth_lowres").geometry.device
+    run = overlay_call(ne, cells, "identity", size)
+    t = timed(st, run, reps=3, warm=1)
+    rec("overlay identity (naturalearth_lowres x the 5-degree grid)", size[0], "rows", t, {"phases_ms": phases(run)})
+
+    mxy, mro, mgo = synth.star_polygons(m=2000, grid=45)
+    few = upload(mxy, mro, mgo)
+    c = mxy.min(0) + (mxy.max(0) - mxy.min(0)) / 2
+    ang = np.arange(256) * (2 * np.pi / 256)
+    big_xy = np.concatenate([np.stack([c[0] + 220 * np.cos(ang), c[1] + 220 * np.sin(ang)], 1), [[c[0] + 220, c[1]]]])
+    big = upload(big_xy, np.array([0, 257], dtype=np.int64), np.array([0, 1], dtype=np.int64))
+    pl, _ = E.spatial_join(big, few, "intersects")
+    run = overlay_call(big, few, "difference", size)
+    t = timed(st, run, reps=1, warm=0)
+    rec("overlay difference (one 256-gon x 2 000 stars, %d cutters)" % len(pl), 1, "remainders", t, {"phases_ms": phases(run)})
 
 
 def relate_rows(args, ctx, dev, st, res):
