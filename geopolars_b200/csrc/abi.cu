@@ -5,6 +5,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "output.cuh"
 
 namespace gpl {
 
@@ -42,6 +43,38 @@ __global__ void k_widen(const int32_t *__restrict__ in, int64_t *__restrict__ ou
     int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (; i < n; i += stride) out[i] = in[i];
+}
+
+// bytes (one per row) -> Arrow LSB bitmap
+__global__ void k_pack_bits(const uint8_t *__restrict__ bytes, uint8_t *__restrict__ bitmap, int64_t n) {
+    int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;  // output byte
+    int64_t nb = (n + 7) / 8;
+    if (i >= nb) return;
+    uint8_t v = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        int64_t j = i * 8 + k;
+        if (j < n && bytes[j]) v |= (uint8_t)(1u << k);
+    }
+    bitmap[i] = v;
+}
+int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n) {
+    if (n == 0) return GPL_OK;
+    int64_t nb = (n + 7) / 8;
+    GPL_LAUNCH(ctx, k_pack_bits, (int)ceil_div(nb, 256), 256, 0, bytes_dev, bitmap_dev, n);
+    return GPL_OK;
+}
+
+// copy a device result to the caller's buffer (host: stream-ordered D2H + sync)
+int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem) {
+    if (bytes == 0) return GPL_OK;
+    if (mem == GPL_HOST) {
+        GPL_CUDA(cudaMemcpyAsync(dst, src_dev, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    } else if (dst != src_dev) {
+        GPL_CUDA(cudaMemcpyAsync(dst, src_dev, bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+    }
+    return GPL_OK;
 }
 
 }  // namespace gpl
@@ -430,6 +463,7 @@ extern "C" int gpl_array_view(const gpl_array *a, gpl_device_view *v) {
 extern "C" int gpl_array_copy_out(gpl_ctx *ctx, const gpl_array *a, double *xy, int64_t *geom_offsets,
                                   int64_t *part_offsets, int64_t *ring_offsets, uint8_t *validity, int mem) {
     GPL_REQUIRE(ctx && a, GPL_ERR_INVALID_ARG, "gpl_array_copy_out: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_array_copy_out"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     cudaMemcpyKind k = mem == GPL_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
     if (xy && a->n_coords) GPL_CUDA(cudaMemcpyAsync(xy, a->xy, sizeof(double) * 2 * a->n_coords, k, ctx->stream));

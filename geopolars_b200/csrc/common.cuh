@@ -48,10 +48,10 @@ constexpr int kSMs = 132;  // H100 SXM
 
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// CTAs for one warp per row, at most 16 per SM (the warps stride over the remaining rows)
-static int warp_grid(int64_t rows, int warps_per_cta) {
+// CTAs for one warp per row, at most ctas_per_sm per SM (the warps stride over the remaining rows)
+static int warp_grid(int64_t rows, int warps_per_cta, int ctas_per_sm = 16) {
     int64_t want = ceil_div(rows, warps_per_cta);
-    return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * 16));
+    return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * ctas_per_sm));
 }
 // CTAs of 256 threads for one thread per item, at most 16 per SM (the threads stride over the remaining items)
 static int flat_grid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)kSMs * 16)); }
@@ -67,6 +67,13 @@ static const char *type_name(int t) {
     default: return "Unknown";
     }
 }
+
+// geometry type tests of the host side
+static inline bool is_point(int t) { return t == GPL_POINT || t == GPL_MULTIPOINT; }
+static inline bool is_line(int t) { return t == GPL_LINESTRING || t == GPL_MULTILINESTRING; }
+static inline bool is_area(int t) { return t == GPL_POLYGON || t == GPL_MULTIPOLYGON; }
+static inline bool is_multi(int t) { return t == GPL_MULTIPOINT || t == GPL_MULTILINESTRING || t == GPL_MULTIPOLYGON; }
+static inline bool known_type(int t) { return is_point(t) || is_line(t) || is_area(t); }  // the six OGC types
 
 }  // namespace gpl
 
@@ -185,6 +192,13 @@ static int pairs_new(gpl_ctx *ctx, int64_t n, bool with_dist, Pairs &out) {
 
 gpl_array *array_new(gpl_ctx *ctx, int32_t type);
 void array_retain(gpl_array *a);
+
+// the two columns of a row-wise binary op have one row each per output row
+static int require_same_length(const gpl_array *a, const gpl_array *b, const char *who) {
+    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "%s: lengths differ (%lld vs %lld)", who, (long long)a->n_geoms,
+                (long long)b->n_geoms);
+    return GPL_OK;
+}
 
 // ------------------------------------------------------------------------------------------------
 // launch helper: counts launches for bench.py's gpu_launches and checks the launch error.

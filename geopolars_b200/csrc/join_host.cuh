@@ -6,11 +6,10 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "output.cuh"
 #include "scan.cuh"
 
 namespace gpl {
-
-int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
 
 // The dense outputs of a nearest pass: run(nid, dist, ntied) fills device buffers (dist / ntied may be NULL).  Outputs in host
 // memory are filled through scratch.

@@ -12,6 +12,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "output.cuh"
 
 namespace gpl {
 
@@ -131,7 +132,6 @@ int affine_fixed(gpl_ctx *ctx, const gpl_array *in, Affine m, gpl_array **out) {
 }
 
 // defined in k_measure.cu: per-geometry origin table (centroid or bbox centre)
-int origin_table(gpl_ctx *ctx, const gpl_array *in, int origin, double2 *out_dev);
 
 int affine_about_origin(gpl_ctx *ctx, const gpl_array *in, int kind, double p0, double p1, int origin, double ox,
                         double oy, gpl_array **out) {

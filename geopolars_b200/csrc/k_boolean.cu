@@ -36,6 +36,7 @@
 #include "common.cuh"
 #include "join_grid.cuh"
 #include "join_host.cuh"
+#include "output.cuh"
 #include "overlay.cuh"
 #include "pair_dist.cuh"
 #include "scan.cuh"
@@ -190,26 +191,23 @@ __global__ void __launch_bounds__(128) k_bool_assemble(int64_t n, BOperands o, i
 // device) receives the member count of each row
 static int boolean_rows(gpl_ctx *ctx, const BOperands &ops, int64_t n, const uint64_t *ia, const uint64_t *ib, int op, gpl_array **out,
                         Scratch<int64_t> *members) {
-    Scratch<int64_t> cnt, off, cm_own, cr, cc, rbase, cbase, tot;
-    Scratch<int64_t> &cm = members ? *members : cm_own;
-    Scratch<uint8_t> rv, bm;
+    RaggedOut res;
+    Scratch<int64_t> cnt, off;
+    Scratch<uint8_t> rv;
     Scratch<int> too_big;
-    Scratch<int64_t> geom_off, part_off, ring_off;
-    Scratch<double> oxy;
+    GPL_TRY(res.init(ctx, n, 3));
     GPL_TRY(cnt.get(ctx, (size_t)n));
     GPL_TRY(off.get(ctx, (size_t)n + 1));
     GPL_TRY(rv.get(ctx, (size_t)n));
     GPL_TRY(too_big.get(ctx, 1));
-    GPL_TRY(tot.get(ctx, 3));
-    GPL_TRY(geom_off.get(ctx, (size_t)n + 1));
     GPL_CUDA(cudaMemsetAsync(too_big.p, 0, sizeof(int), ctx->stream));
     const int grid = warp_grid(n, kBoolThreads / 32);
     if (n > 0)
         GPL_LAUNCH(ctx, k_bool_nodes<false>, grid, kBoolThreads, 0, n, ops, ia, ib, cnt.p, rv.p, nullptr, nullptr, too_big.p);
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cnt.p, n, off.p, tot.p)));
+    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cnt.p, n, off.p, res.tot.p)));
     int64_t h_nodes = 0;
     int h_big = 0;
-    GPL_CUDA(cudaMemcpyAsync(&h_nodes, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaMemcpyAsync(&h_nodes, res.tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
     GPL_CUDA(cudaMemcpyAsync(&h_big, too_big.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     GPL_CUDA(cudaStreamSynchronize(ctx->stream));
     GPL_REQUIRE(!h_big, GPL_ERR_UNSUPPORTED, "boolean_op: a row has 2^30 or more boundary nodes");
@@ -219,44 +217,22 @@ static int boolean_rows(gpl_ctx *ctx, const BOperands &ops, int64_t n, const uin
     GPL_TRY(nodes.get(ctx, (size_t)h_nodes));
     GPL_TRY(ws.get(ctx, (size_t)h_nodes * 8));
     GPL_TRY(loops.get(ctx, (size_t)h_nodes));
-    GPL_TRY(cm.get(ctx, (size_t)n));
-    GPL_TRY(cr.get(ctx, (size_t)n));
-    GPL_TRY(cc.get(ctx, (size_t)n));
-    GPL_TRY(rbase.get(ctx, (size_t)n + 1));
-    GPL_TRY(cbase.get(ctx, (size_t)n + 1));
     const int tgrid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 128), (int64_t)kSMs * 16));
     const bool sym = op == GPL_BOOLEAN_SYMMETRIC_DIFFERENCE;  // pieces reversed by their state
+    int64_t *cm = res.count[0].p, *cr = res.count[1].p, *cc = res.count[2].p;
     if (n > 0) {
         GPL_LAUNCH(ctx, k_bool_nodes<true>, grid, kBoolThreads, 0, n, ops, ia, ib, cnt.p, rv.p, off.p, nodes.p, too_big.p);
         GPL_LAUNCH(ctx, k_bool_classify, grid, kBoolThreads, 0, n, ops, ia, ib, op, off.p, nodes.p);
         GPL_LAUNCH(ctx, (sym ? k_bool_assemble<false, true> : k_bool_assemble<false, false>), tgrid, 128, 0, n, ops, op, off.p, nodes.p, ws.p,
-                   h_nodes, loops.p, cm.p, cr.p, cc.p, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+                   h_nodes, loops.p, cm, cr, cc, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
     }
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cm.p, n, geom_off.p, tot.p)));
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cr.p, n, rbase.p, tot.p + 1)));
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cc.p, n, cbase.p, tot.p + 2)));
-    int64_t h_tot[3] = {0, 0, 0};
-    GPL_CUDA(cudaMemcpyAsync(h_tot, tot.p, sizeof(h_tot), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    GPL_TRY(part_off.get(ctx, (size_t)h_tot[0] + 1));
-    GPL_TRY(ring_off.get(ctx, (size_t)h_tot[1] + 1));
-    GPL_TRY(oxy.get(ctx, (size_t)h_tot[2] * 2));
+    GPL_TRY(res.scan_and_allocate());
     if (n > 0)
         GPL_LAUNCH(ctx, (sym ? k_bool_assemble<true, true> : k_bool_assemble<true, false>), tgrid, 128, 0, n, ops, op, off.p, nodes.p, ws.p,
-                   h_nodes, loops.p, cm.p, cr.p, cc.p, geom_off.p, rbase.p, cbase.p, part_off.p, ring_off.p, reinterpret_cast<double2 *>(oxy.p));
-    GPL_CUDA(cudaMemcpyAsync(part_off.p + h_tot[0], rbase.p + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    GPL_CUDA(cudaMemcpyAsync(ring_off.p + h_tot[1], cbase.p + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    GPL_TRY(bm.get(ctx, (size_t)(n + 7) / 8));
-    if (n > 0) GPL_TRY(pack_bits(ctx, rv.p, bm.p, n));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
-    gpl_array *res = array_new(ctx, GPL_MULTIPOLYGON);
-    res->n_geoms = n, res->n_parts = h_tot[0], res->n_rings = h_tot[1], res->n_coords = h_tot[2];
-    res->geom_off = geom_off.take(), res->own_geom = true;
-    res->part_off = part_off.take(), res->own_part = true;
-    res->ring_off = ring_off.take(), res->own_ring = true;
-    res->xy = oxy.take(), res->own_xy = true;
-    res->validity = bm.take(), res->own_valid = true;
-    *out = res;
+                   h_nodes, loops.p, cm, cr, cc, res.base[0].p, res.base[1].p, res.base[2].p, res.off[0].p, res.off[1].p,
+                   reinterpret_cast<double2 *>(res.xy.p));
+    GPL_TRY(res.finish(rv.p, GPL_MULTIPOLYGON, out));
+    if (members) members->ctx = ctx, members->p = res.count[0].take();
     return GPL_OK;
 }
 
@@ -275,6 +251,67 @@ __global__ void __launch_bounds__(256) k_nonempty(int64_t n, const int64_t *__re
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) keep[i] = members[i] > 0;
 }
+
+int keep_nonempty_rows(gpl_ctx *ctx, const gpl_pairs *cand, gpl_array *all, const int64_t *members, gpl_pairs **pairs, gpl_array **out) {
+    const int64_t n = cand->n;
+    Scratch<uint8_t> keep;
+    Scratch<int64_t> goff;
+    GPL_TRY(keep.get(ctx, (size_t)n));
+    if (n > 0) GPL_LAUNCH(ctx, k_nonempty, flat_grid(n), 256, 0, n, members, keep.p);
+    Pairs res(nullptr, gpl_pairs_free);
+    GPL_TRY(keep_pairs(ctx, cand, keep.p, res, all->geom_off, &goff));
+    const int64_t m = res->n;
+    // every output row is valid: a null or non-finite pair has no member and is dropped
+    Scratch<uint8_t> bm;
+    GPL_TRY(bm.get(ctx, (size_t)(m + 7) / 8));
+    GPL_CUDA(cudaMemsetAsync(bm.p, 0xff, (size_t)(m + 7) / 8, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    gpl_array *o = array_new(ctx, all->type);
+    o->n_geoms = m, o->n_parts = all->n_parts, o->n_rings = all->n_rings, o->n_coords = all->n_coords;
+    o->geom_off = goff.take(), o->own_geom = true;
+    o->part_off = all->part_off, o->ring_off = all->ring_off, o->xy = all->xy;  // shared with the uncompacted result
+    o->validity = bm.take(), o->own_valid = true;
+    o->parent = all;
+    *pairs = res.release();
+    *out = o;
+    return GPL_OK;
+}
+
+int RaggedOut::init(gpl_ctx *c, int64_t rows, int nlevels) {
+    ctx = c, n = rows, levels = nlevels;
+    for (int k = 0; k < levels; ++k) {
+        GPL_TRY(count[k].get(ctx, (size_t)n));
+        GPL_TRY(base[k].get(ctx, (size_t)n + 1));
+    }
+    return tot.get(ctx, 3);
+}
+
+int RaggedOut::scan_and_allocate() {
+    for (int k = 0; k < levels; ++k) GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, count[k].p, n, base[k].p, tot.p + k)));
+    GPL_CUDA(cudaMemcpyAsync(total, tot.p, sizeof(int64_t) * levels, cudaMemcpyDeviceToHost, ctx->stream));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
+    for (int k = 0; k + 1 < levels; ++k) GPL_TRY(off[k].get(ctx, (size_t)total[k] + 1));
+    return xy.get(ctx, (size_t)total[levels - 1] * 2);
+}
+
+int RaggedOut::finish(const uint8_t *row_valid_bytes, int type, gpl_array **out) {
+    // the last offset of each lower level: the total of the level below, which the scan left at base[k + 1][n]
+    for (int k = 0; k + 1 < levels; ++k)
+        GPL_CUDA(cudaMemcpyAsync(off[k].p + total[k], base[k + 1].p + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
+    Scratch<uint8_t> bm;
+    GPL_TRY(bm.get(ctx, (size_t)(n + 7) / 8));
+    GPL_TRY(pack_bits(ctx, row_valid_bytes, bm.p, n));
+    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the caller's scratch returns to the cache after this
+    gpl_array *res = array_new(ctx, type);
+    res->n_geoms = n, res->n_coords = total[levels - 1];
+    res->geom_off = base[0].take(), res->own_geom = true;
+    if (levels == 3) res->n_parts = total[0], res->part_off = off[0].take(), res->own_part = true;
+    if (levels >= 2) res->n_rings = total[levels - 2], res->ring_off = off[levels - 2].take(), res->own_ring = true;
+    res->xy = xy.take(), res->own_xy = true;
+    res->validity = bm.take(), res->own_valid = true;
+    *out = res;
+    return GPL_OK;
+}
 }  // namespace gpl
 
 using namespace gpl;
@@ -287,8 +324,7 @@ extern "C" int gpl_boolean_op(gpl_ctx *ctx, const gpl_array *a, const gpl_array 
                 "gpl_boolean_op: unknown op %d", op);
     GPL_REQUIRE(is_area(a->type) && is_area(b->type), GPL_ERR_INVALID_TYPE, "Expected (Multi)Polygon x (Multi)Polygon (found %s x %s)",
                 type_name(a->type), type_name(b->type));
-    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "boolean_op: lengths differ (%lld vs %lld)", (long long)a->n_geoms,
-                (long long)b->n_geoms);
+    GPL_TRY(require_same_length(a, b, "boolean_op"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     RingPrep pa, pb;
     GPL_TRY(ring_prep(ctx, a, pa));
@@ -315,26 +351,7 @@ extern "C" int gpl_overlay_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_ar
     GPL_TRY(boolean_rows(ctx, operands(lhs, pl, rhs, pr), n, cand->lhs, cand->rhs, GPL_BOOLEAN_INTERSECTION, &all, &members));
     std::unique_ptr<gpl_array, void (*)(gpl_array *)> geo(all, gpl_array_free);
     // drop the pairs whose intersection has no member (touching pairs)
-    Scratch<uint8_t> keep;
-    Scratch<int64_t> goff;
-    GPL_TRY(keep.get(ctx, (size_t)n));
-    if (n > 0) GPL_LAUNCH(ctx, k_nonempty, flat_grid(n), 256, 0, n, members.p, keep.p);
-    Pairs res(nullptr, gpl_pairs_free);
-    GPL_TRY(keep_pairs(ctx, cand.get(), keep.p, res, all->geom_off, &goff));
-    const int64_t m = res->n;
-    // every output row is valid: a null or non-finite pair has no member and is dropped
-    Scratch<uint8_t> bm;
-    GPL_TRY(bm.get(ctx, (size_t)(m + 7) / 8));
-    GPL_CUDA(cudaMemsetAsync(bm.p, 0xff, (size_t)(m + 7) / 8, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    gpl_array *o = array_new(ctx, GPL_MULTIPOLYGON);
-    o->n_geoms = m, o->n_parts = all->n_parts, o->n_rings = all->n_rings, o->n_coords = all->n_coords;
-    o->geom_off = goff.take(), o->own_geom = true;
-    o->part_off = all->part_off, o->ring_off = all->ring_off, o->xy = all->xy;  // shared with the uncompacted result
-    o->validity = bm.take(), o->own_valid = true;
-    o->parent = all;
-    geo.release();  // o holds the reference
-    *pairs = res.release();
-    *out = o;
+    GPL_TRY(keep_nonempty_rows(ctx, cand.get(), all, members.p, pairs, out));
+    geo.release();  // *out holds the reference
     return GPL_OK;
 }

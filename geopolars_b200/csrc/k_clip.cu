@@ -33,6 +33,7 @@
 #include "common.cuh"
 #include "join_grid.cuh"
 #include "join_host.cuh"
+#include "output.cuh"
 #include "overlay.cuh"
 #include "pair_dist.cuh"
 #include "scan.cuh"
@@ -477,9 +478,6 @@ __global__ void __launch_bounds__(kClipThreads, 3) k_clip_points(int64_t n, BOpe
 }
 
 // ---- host side --------------------------------------------------------------------------------------------------------
-static bool is_line(int t) { return t == GPL_LINESTRING || t == GPL_MULTILINESTRING; }
-static bool is_point(int t) { return t == GPL_POINT || t == GPL_MULTIPOINT; }
-
 static BOperands clip_operands(const gpl_array *a, const gpl_array *b, const RingPrep &pb) {
     BOperands o;
     const bool multi = a->type == GPL_MULTILINESTRING || a->type == GPL_MULTIPOINT;
@@ -541,71 +539,37 @@ static int line_stage(gpl_ctx *ctx, const BOperands &o, int64_t n, const uint64_
 // column; members[r] (optional, device) receives the member (point) count of each row
 static int clip_rows(gpl_ctx *ctx, const BOperands &o, bool lines, int64_t n, const uint64_t *ia, const uint64_t *ib, bool invert, gpl_array **out,
                      Scratch<int64_t> *members) {
-    Scratch<int64_t> cm_own, cc, cbase, tot, geom_off, ring_off;
-    Scratch<int64_t> &cm = members ? *members : cm_own;
-    Scratch<uint8_t> bm;
-    Scratch<double> oxy;
+    RaggedOut res;
     LineStage st;
     const int grid = warp_grid(n, kClipThreads / 32);
-    GPL_TRY(cm.get(ctx, (size_t)n));
-    GPL_TRY(geom_off.get(ctx, (size_t)n + 1));
-    GPL_TRY(tot.get(ctx, 2));
-    int64_t h_tot[2] = {0, 0};
+    GPL_TRY(res.init(ctx, n, lines ? 2 : 1));
+    int64_t *cm = res.count[0].p;
     if (lines) {
+        int64_t *cc = res.count[1].p;
         GPL_TRY(line_stage(ctx, o, n, ia, ib, nullptr, st));
-        GPL_TRY(cc.get(ctx, (size_t)n));
-        GPL_TRY(cbase.get(ctx, (size_t)n + 1));
         if (n > 0)
-            GPL_LAUNCH(ctx, k_clip_emit<false>, grid, kClipThreads, 0, n, o, ia, st.rv.p, st.sbase.p, st.sflag.p, st.roff.p, st.nodes.p, invert, cm.p,
-                       cc.p, nullptr, nullptr, nullptr, nullptr);
-        GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cm.p, n, geom_off.p, tot.p)));
-        GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cc.p, n, cbase.p, tot.p + 1)));
-        GPL_CUDA(cudaMemcpyAsync(h_tot, tot.p, sizeof(h_tot), cudaMemcpyDeviceToHost, ctx->stream));
-        GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-        GPL_TRY(ring_off.get(ctx, (size_t)h_tot[0] + 1));
-        GPL_TRY(oxy.get(ctx, (size_t)h_tot[1] * 2));
+            GPL_LAUNCH(ctx, k_clip_emit<false>, grid, kClipThreads, 0, n, o, ia, st.rv.p, st.sbase.p, st.sflag.p, st.roff.p, st.nodes.p, invert, cm,
+                       cc, nullptr, nullptr, nullptr, nullptr);
+        GPL_TRY(res.scan_and_allocate());
         if (n > 0)
-            GPL_LAUNCH(ctx, k_clip_emit<true>, grid, kClipThreads, 0, n, o, ia, st.rv.p, st.sbase.p, st.sflag.p, st.roff.p, st.nodes.p, invert, cm.p,
-                       cc.p, geom_off.p, cbase.p, ring_off.p, reinterpret_cast<double2 *>(oxy.p));
-        GPL_CUDA(cudaMemcpyAsync(ring_off.p + h_tot[0], cbase.p + n, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
+            GPL_LAUNCH(ctx, k_clip_emit<true>, grid, kClipThreads, 0, n, o, ia, st.rv.p, st.sbase.p, st.sflag.p, st.roff.p, st.nodes.p, invert, cm,
+                       cc, res.base[0].p, res.base[1].p, res.off[0].p, reinterpret_cast<double2 *>(res.xy.p));
     } else {
         Scratch<int64_t> ncoord;
         GPL_TRY(st.rv.get(ctx, (size_t)n));
         GPL_TRY(ncoord.get(ctx, (size_t)n));
         if (n > 0) {
             GPL_LAUNCH(ctx, k_clip_prep, grid, kClipThreads, 0, n, o, false, ia, ib, ncoord.p, st.rv.p);
-            GPL_LAUNCH(ctx, k_clip_points<false>, grid, kClipThreads, 0, n, o, ia, ib, st.rv.p, invert, cm.p, nullptr, nullptr);
+            GPL_LAUNCH(ctx, k_clip_points<false>, grid, kClipThreads, 0, n, o, ia, ib, st.rv.p, invert, cm, nullptr, nullptr);
         }
-        GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cm.p, n, geom_off.p, tot.p)));
-        GPL_CUDA(cudaMemcpyAsync(h_tot, tot.p, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-        GPL_TRY(oxy.get(ctx, (size_t)h_tot[0] * 2));
+        GPL_TRY(res.scan_and_allocate());
         if (n > 0)
-            GPL_LAUNCH(ctx, k_clip_points<true>, grid, kClipThreads, 0, n, o, ia, ib, st.rv.p, invert, nullptr, geom_off.p,
-                       reinterpret_cast<double2 *>(oxy.p));
+            GPL_LAUNCH(ctx, k_clip_points<true>, grid, kClipThreads, 0, n, o, ia, ib, st.rv.p, invert, nullptr, res.base[0].p,
+                       reinterpret_cast<double2 *>(res.xy.p));
     }
-    GPL_TRY(bm.get(ctx, (size_t)(n + 7) / 8));
-    if (n > 0) GPL_TRY(pack_bits(ctx, st.rv.p, bm.p, n));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
-    gpl_array *res = array_new(ctx, lines ? GPL_MULTILINESTRING : GPL_MULTIPOINT);
-    res->n_geoms = n;
-    res->geom_off = geom_off.take(), res->own_geom = true;
-    if (lines) {
-        res->n_rings = h_tot[0], res->n_coords = h_tot[1];
-        res->ring_off = ring_off.take(), res->own_ring = true;
-    } else {
-        res->n_coords = h_tot[0];
-    }
-    res->xy = oxy.take(), res->own_xy = true;
-    res->validity = bm.take(), res->own_valid = true;
-    *out = res;
+    GPL_TRY(res.finish(st.rv.p, lines ? GPL_MULTILINESTRING : GPL_MULTIPOINT, out));
+    if (members) members->ctx = ctx, members->p = res.count[0].take();
     return GPL_OK;
-}
-
-// keep[k] = 1 when row k of the join's output has a member (a point)
-__global__ void __launch_bounds__(256) k_clip_nonempty(int64_t n, const int64_t *__restrict__ members, uint8_t *__restrict__ keep) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) keep[i] = members[i] > 0;
 }
 
 }  // namespace gpl
@@ -616,8 +580,7 @@ extern "C" int gpl_clip(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, in
     GPL_REQUIRE(ctx && a && b && out, GPL_ERR_INVALID_ARG, "gpl_clip: NULL argument");
     GPL_REQUIRE((is_line(a->type) || is_point(a->type)) && is_area(b->type), GPL_ERR_INVALID_TYPE,
                 "Expected (Multi)LineString or (Multi)Point x (Multi)Polygon (found %s x %s)", type_name(a->type), type_name(b->type));
-    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "clip: lengths differ (%lld vs %lld)", (long long)a->n_geoms,
-                (long long)b->n_geoms);
+    GPL_TRY(require_same_length(a, b, "clip"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     RingPrep pb;
     GPL_TRY(ring_prep(ctx, b, pb));
@@ -626,25 +589,21 @@ extern "C" int gpl_clip(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, in
 
 extern "C" int gpl_clip_length(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, double *out, uint8_t *out_validity, int mem) {
     GPL_REQUIRE(ctx && a && b && out, GPL_ERR_INVALID_ARG, "gpl_clip_length: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_clip_length"));
     GPL_REQUIRE(is_line(a->type) && is_area(b->type), GPL_ERR_INVALID_TYPE, "Expected (Multi)LineString x (Multi)Polygon (found %s x %s)",
                 type_name(a->type), type_name(b->type));
-    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "clip_length: lengths differ (%lld vs %lld)", (long long)a->n_geoms,
-                (long long)b->n_geoms);
+    GPL_TRY(require_same_length(a, b, "clip_length"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = a->n_geoms;
     if (n == 0) return GPL_OK;
     RingPrep pb;
     GPL_TRY(ring_prep(ctx, b, pb));
-    Scratch<double> tmp;
-    double *dst = out;
-    if (mem == GPL_HOST) {
-        GPL_TRY(tmp.get(ctx, (size_t)n));
-        dst = tmp.p;
-    }
+    RowOut<double> res;
+    GPL_TRY(res.get(ctx, out, n, mem));
     LineStage st;
-    GPL_TRY(line_stage(ctx, clip_operands(a, b, pb), n, nullptr, nullptr, dst, st));
+    GPL_TRY(line_stage(ctx, clip_operands(a, b, pb), n, nullptr, nullptr, res.p, st));
     if (out_validity) GPL_TRY(finish_bitmap(ctx, st.rv.p, n, out_validity, mem));
-    return deliver(ctx, out, dst, sizeof(double) * n, mem);
+    return res.deliver(ctx);
 }
 
 extern "C" int gpl_clip_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **pairs, gpl_array **out) {
@@ -666,27 +625,8 @@ extern "C" int gpl_clip_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array
     GPL_TRY(clip_rows(ctx, clip_operands(lhs, rhs, pr), lines, n, cand->lhs, cand->rhs, false, &all, &members));
     std::unique_ptr<gpl_array, void (*)(gpl_array *)> geo(all, gpl_array_free);
     // drop the pairs whose intersection has no member (lines that only touch)
-    Scratch<uint8_t> keep;
-    Scratch<int64_t> goff;
-    GPL_TRY(keep.get(ctx, (size_t)n));
-    if (n > 0) GPL_LAUNCH(ctx, k_clip_nonempty, flat_grid(n), 256, 0, n, members.p, keep.p);
-    Pairs res(nullptr, gpl_pairs_free);
-    GPL_TRY(keep_pairs(ctx, cand.get(), keep.p, res, all->geom_off, &goff));
-    const int64_t m = res->n;
-    // every output row is valid: a null or non-finite pair has no member and is dropped
-    Scratch<uint8_t> bm;
-    GPL_TRY(bm.get(ctx, (size_t)(m + 7) / 8));
-    GPL_CUDA(cudaMemsetAsync(bm.p, 0xff, (size_t)(m + 7) / 8, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    gpl_array *o = array_new(ctx, all->type);
-    o->n_geoms = m, o->n_rings = all->n_rings, o->n_coords = all->n_coords;
-    o->geom_off = goff.take(), o->own_geom = true;
-    o->ring_off = all->ring_off, o->xy = all->xy;  // shared with the uncompacted result
-    o->validity = bm.take(), o->own_valid = true;
-    o->parent = all;
-    geo.release();  // o holds the reference
-    *pairs = res.release();
-    *out = o;
+    GPL_TRY(keep_nonempty_rows(ctx, cand.get(), all, members.p, pairs, out));
+    geo.release();  // *out holds the reference
     return GPL_OK;
 }
 

@@ -29,6 +29,7 @@
 #include "common.cuh"
 #include "join_grid.cuh"
 #include "join_host.cuh"
+#include "output.cuh"
 #include "overlay.cuh"
 #include "pair_dist.cuh"
 #include "scan.cuh"
@@ -489,49 +490,22 @@ static int group_rings(gpl_ctx *ctx, const BOperands &o, int64_t ng, const int64
     if (m > 0)
         GPL_LAUNCH(ctx, k_dis_classify, cgrid, kBoolThreads, 0, m, o, prow, pkey, pinv, ib.p, noff.p, poff, partners, ring_row, nodes.p, x4.p);
     // assembly: counts, scans, write
-    Scratch<int64_t> cm, cr, cc, geom_off, rbase, cbase, part_off, ring_off;
-    Scratch<double> oxy;
-    Scratch<uint8_t> rv, bm;
-    GPL_TRY(cm.get(ctx, (size_t)ng));
-    GPL_TRY(cr.get(ctx, (size_t)ng));
-    GPL_TRY(cc.get(ctx, (size_t)ng));
-    GPL_TRY(geom_off.get(ctx, (size_t)ng + 1));
-    GPL_TRY(rbase.get(ctx, (size_t)ng + 1));
-    GPL_TRY(cbase.get(ctx, (size_t)ng + 1));
+    RaggedOut res;
+    Scratch<uint8_t> rv;
+    GPL_TRY(res.init(ctx, ng, 3));
+    GPL_TRY(rv.get(ctx, (size_t)ng));
+    int64_t *cm = res.count[0].p, *cr = res.count[1].p, *cc = res.count[2].p;
     const int tgrid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(ng, 128), (int64_t)kSMs * 16));
     if (ng > 0)
-        GPL_LAUNCH(ctx, (pinv ? k_dis_assemble<false, true> : k_dis_assemble<false, false>), tgrid, 128, 0, ng, o, gnode.p, gnull, nodes.p, ws.p, h_nodes, loops.p, lbox.p, cm.p, cr.p, cc.p,
+        GPL_LAUNCH(ctx, (pinv ? k_dis_assemble<false, true> : k_dis_assemble<false, false>), tgrid, 128, 0, ng, o, gnode.p, gnull, nodes.p, ws.p, h_nodes, loops.p, lbox.p, cm, cr, cc,
                    nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cm.p, ng, geom_off.p, tot.p)));
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cr.p, ng, rbase.p, tot.p + 1)));
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cc.p, ng, cbase.p, tot.p + 2)));
-    int64_t h_tot[3] = {0, 0, 0};
-    GPL_CUDA(cudaMemcpyAsync(h_tot, tot.p, sizeof(h_tot), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    GPL_TRY(part_off.get(ctx, (size_t)h_tot[0] + 1));
-    GPL_TRY(ring_off.get(ctx, (size_t)h_tot[1] + 1));
-    GPL_TRY(oxy.get(ctx, (size_t)h_tot[2] * 2));
-    if (ng > 0)
-        GPL_LAUNCH(ctx, (pinv ? k_dis_assemble<true, true> : k_dis_assemble<true, false>), tgrid, 128, 0, ng, o, gnode.p, gnull, nodes.p, ws.p, h_nodes, loops.p, lbox.p, cm.p, cr.p, cc.p,
-                   geom_off.p, rbase.p, cbase.p, part_off.p, ring_off.p, reinterpret_cast<double2 *>(oxy.p));
-    GPL_CUDA(cudaMemcpyAsync(part_off.p + h_tot[0], rbase.p + ng, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    GPL_CUDA(cudaMemcpyAsync(ring_off.p + h_tot[1], cbase.p + ng, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    GPL_TRY(rv.get(ctx, (size_t)ng));
-    GPL_TRY(bm.get(ctx, (size_t)(ng + 7) / 8));
+    GPL_TRY(res.scan_and_allocate());
     if (ng > 0) {
+        GPL_LAUNCH(ctx, (pinv ? k_dis_assemble<true, true> : k_dis_assemble<true, false>), tgrid, 128, 0, ng, o, gnode.p, gnull, nodes.p, ws.p, h_nodes, loops.p, lbox.p, cm, cr, cc,
+                   res.base[0].p, res.base[1].p, res.base[2].p, res.off[0].p, res.off[1].p, reinterpret_cast<double2 *>(res.xy.p));
         GPL_LAUNCH(ctx, k_dis_valid, flat_grid(ng), 256, 0, ng, gnull, rv.p);
-        GPL_TRY(pack_bits(ctx, rv.p, bm.p, ng));
     }
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
-    gpl_array *res = array_new(ctx, GPL_MULTIPOLYGON);
-    res->n_geoms = ng, res->n_parts = h_tot[0], res->n_rings = h_tot[1], res->n_coords = h_tot[2];
-    res->geom_off = geom_off.take(), res->own_geom = true;
-    res->part_off = part_off.take(), res->own_part = true;
-    res->ring_off = ring_off.take(), res->own_ring = true;
-    res->xy = oxy.take(), res->own_xy = true;
-    res->validity = bm.take(), res->own_valid = true;
-    *out = res;
-    return GPL_OK;
+    return res.finish(rv.p, GPL_MULTIPOLYGON, out);
 }
 
 // ---- remainders (§4.23): subject i minus the union of the cutters C(i) it intersects, as a group of positions of the
@@ -686,7 +660,7 @@ using namespace gpl;
 
 extern "C" int gpl_dissolve(gpl_ctx *ctx, const gpl_array *in, const int64_t *group, int mem, int64_t n_groups, gpl_array **out) {
     GPL_REQUIRE(ctx && in && out && (group || in->n_geoms == 0), GPL_ERR_INVALID_ARG, "gpl_dissolve: NULL argument");
-    GPL_REQUIRE(mem == GPL_HOST || mem == GPL_DEVICE, GPL_ERR_INVALID_ARG, "gpl_dissolve: unknown mem %d", mem);
+    GPL_TRY(check_mem(mem, "gpl_dissolve"));
     GPL_REQUIRE(n_groups >= 0, GPL_ERR_INVALID_ARG, "gpl_dissolve: n_groups must be >= 0 (found %lld)", (long long)n_groups);
     GPL_REQUIRE(is_area(in->type), GPL_ERR_INVALID_TYPE, "Expected (Multi)Polygon (found %s)", type_name(in->type));
     const int64_t n = in->n_geoms, ng = n_groups;

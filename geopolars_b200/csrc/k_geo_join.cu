@@ -28,6 +28,7 @@
 #include "haversine.cuh"
 #include "join_grid.cuh"
 #include "join_host.cuh"
+#include "output.cuh"
 #include "scan.cuh"
 
 namespace gpl {
@@ -285,8 +286,6 @@ __global__ void __launch_bounds__(256) k_haversine_rows(int64_t n, const double2
     out_valid[i] = valid ? 1 : 0;
 }
 
-int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n);
-
 static int geo_grid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, kGeoWarps * 32), (int64_t)kSMs * 8)); }
 
 static int check_geo_left(const gpl_array *lhs, const char *join) {
@@ -337,33 +336,21 @@ using namespace gpl;
 
 extern "C" int gpl_haversine_distance(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, double *out, uint8_t *out_validity, int mem) {
     GPL_REQUIRE(ctx && lhs && rhs && out, GPL_ERR_INVALID_ARG, "gpl_haversine_distance: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_haversine_distance"));
     GPL_REQUIRE(lhs->type == GPL_POINT && rhs->type == GPL_POINT, GPL_ERR_INVALID_TYPE,
                 "haversine_distance: both sides must be Point (found %s x %s)", type_name(lhs->type), type_name(rhs->type));
-    GPL_REQUIRE(lhs->n_geoms == rhs->n_geoms, GPL_ERR_LENGTH_MISMATCH, "haversine_distance: lengths differ (%lld vs %lld)",
-                (long long)lhs->n_geoms, (long long)rhs->n_geoms);
+    GPL_TRY(require_same_length(lhs, rhs, "haversine_distance"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = lhs->n_geoms;
     if (n == 0) return GPL_OK;
-    Scratch<double> tmp;
-    Scratch<uint8_t> vb, bm;
-    double *dst = out;
-    if (mem != GPL_DEVICE) {
-        GPL_TRY(tmp.get(ctx, (size_t)n));
-        dst = tmp.p;
-    }
-    GPL_TRY(vb.get(ctx, (size_t)n));
+    RowOut<double> res;
+    ValidOut valid;
+    GPL_TRY(res.get(ctx, out, n, mem));
+    GPL_TRY(valid.get(ctx, out_validity, n, mem, true));
     GPL_LAUNCH(ctx, k_haversine_rows, (int)ceil_div(n, 256), 256, 0, n, reinterpret_cast<const double2 *>(lhs->xy), lhs->validity,
-               reinterpret_cast<const double2 *>(rhs->xy), rhs->validity, dst, vb.p);
-    if (out_validity) {
-        if (mem == GPL_DEVICE) {
-            GPL_TRY(pack_bits(ctx, vb.p, out_validity, n));
-        } else {
-            GPL_TRY(bm.get(ctx, (size_t)(n + 7) / 8));
-            GPL_TRY(pack_bits(ctx, vb.p, bm.p, n));
-            GPL_TRY(deliver(ctx, out_validity, bm.p, (size_t)(n + 7) / 8, GPL_HOST));
-        }
-    }
-    return deliver(ctx, out, dst, sizeof(double) * n, mem);
+               reinterpret_cast<const double2 *>(rhs->xy), rhs->validity, res.p, valid.p);
+    GPL_TRY(valid.deliver(ctx));
+    return res.deliver(ctx);
 }
 
 extern "C" void gpl_geo_index_free(gpl_geo_index *idx) {
@@ -457,19 +444,14 @@ static int check_geo_max_distance(double maxd) {
 
 extern "C" int gpl_geo_dwithin_count(gpl_ctx *ctx, const gpl_geo_index *idx, const gpl_array *lhs, double distance, int32_t *count, int mem) {
     GPL_REQUIRE(ctx && idx && lhs && (count || lhs->n_geoms == 0), GPL_ERR_INVALID_ARG, "gpl_geo_dwithin_count: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_geo_dwithin_count"));
     GPL_TRY(check_geo_left(lhs, "great-circle dwithin join"));
     GPL_TRY(check_geo_distance(distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
-    const int64_t n = lhs->n_geoms;
-    Scratch<int32_t> dc;
-    int32_t *out = count;
-    if (mem != GPL_DEVICE) {
-        GPL_TRY(dc.get(ctx, (size_t)n));
-        out = dc.p;
-    }
-    GPL_TRY(geo_within_run(ctx, idx, lhs, distance, nullptr, out, nullptr, nullptr, nullptr));
-    if (mem != GPL_DEVICE) GPL_TRY(deliver(ctx, count, dc.p, sizeof(int32_t) * (size_t)n, mem));
-    return GPL_OK;
+    RowOut<int32_t> res;
+    GPL_TRY(res.get(ctx, count, lhs->n_geoms, mem));
+    GPL_TRY(geo_within_run(ctx, idx, lhs, distance, nullptr, res.p, nullptr, nullptr, nullptr));
+    return res.deliver(ctx);
 }
 
 extern "C" int gpl_geo_dwithin_join_pairs(gpl_ctx *ctx, const gpl_geo_index *idx, const gpl_array *lhs, double distance, int with_distance,
@@ -489,6 +471,7 @@ extern "C" int gpl_geo_dwithin_join_pairs(gpl_ctx *ctx, const gpl_geo_index *idx
 extern "C" int gpl_geo_nearest_join(gpl_ctx *ctx, const gpl_geo_index *idx, const gpl_array *lhs, double max_distance, int32_t *nearest_id,
                                     double *distance, int32_t *n_tied, int mem) {
     GPL_REQUIRE(ctx && idx && lhs && (nearest_id || lhs->n_geoms == 0), GPL_ERR_INVALID_ARG, "gpl_geo_nearest_join: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_geo_nearest_join"));
     GPL_TRY(check_geo_left(lhs, "great-circle nearest join"));
     GPL_TRY(check_geo_max_distance(max_distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
@@ -501,6 +484,7 @@ extern "C" int gpl_geo_nearest_join_pairs(gpl_ctx *ctx, const gpl_geo_index *idx
                                           double *distance, int mem) {
     GPL_REQUIRE(ctx && idx && lhs && out, GPL_ERR_INVALID_ARG, "gpl_geo_nearest_join_pairs: NULL argument");
     *out = nullptr;
+    GPL_TRY(check_mem(mem, "gpl_geo_nearest_join_pairs"));
     GPL_TRY(check_geo_left(lhs, "great-circle nearest join"));
     GPL_TRY(check_geo_max_distance(max_distance));
     GPL_CUDA(cudaSetDevice(ctx->device));

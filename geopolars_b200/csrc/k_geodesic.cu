@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include "geodesic.cuh"
 #include "haversine.cuh"
+#include "output.cuh"
 
 namespace gpl {
 
@@ -66,9 +67,6 @@ __global__ void __launch_bounds__(128) k_geodesic_length(int type, int64_t n_geo
     }
 }
 
-int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n);
-int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
-
 }  // namespace gpl
 
 using namespace gpl;
@@ -77,30 +75,19 @@ extern "C" int gpl_geodesic_length(gpl_ctx *ctx, const gpl_array *in, int method
     GPL_REQUIRE(ctx && in && out, GPL_ERR_INVALID_ARG, "gpl_geodesic_length: NULL argument");
     GPL_REQUIRE(method >= 0 && method <= 2, GPL_ERR_INVALID_ARG,
                 "Geodesic calculation method not valid. Use one of geodesic, haversine or vincenty");
+    GPL_TRY(check_mem(mem, "gpl_geodesic_length"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = in->n_geoms;
     if (n == 0) return GPL_OK;
-    Scratch<double> tmp;
-    Scratch<uint8_t> vb, bm;
-    double *dst = out;
-    if (mem == GPL_HOST) {
-        GPL_TRY(tmp.get(ctx, (size_t)n));
-        dst = tmp.p;
-    }
-    GPL_TRY(vb.get(ctx, (size_t)n));
+    RowOut<double> res;
+    ValidOut valid;
+    GPL_TRY(res.get(ctx, out, n, mem));
+    GPL_TRY(valid.get(ctx, out_validity, n, mem, true));
     const double2 *xy = reinterpret_cast<const double2 *>(in->xy);
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 4), (int64_t)kSMs * 16));
-    if (method == 0) GPL_LAUNCH(ctx, k_geodesic_length<0>, grid, 128, 0, in->type, n, xy, in->geom_off, in->part_off, in->ring_off, in->validity, dst, vb.p);
-    else if (method == 1) GPL_LAUNCH(ctx, k_geodesic_length<1>, grid, 128, 0, in->type, n, xy, in->geom_off, in->part_off, in->ring_off, in->validity, dst, vb.p);
-    else GPL_LAUNCH(ctx, k_geodesic_length<2>, grid, 128, 0, in->type, n, xy, in->geom_off, in->part_off, in->ring_off, in->validity, dst, vb.p);
-    if (out_validity) {
-        if (mem == GPL_DEVICE) {
-            GPL_TRY(pack_bits(ctx, vb.p, out_validity, n));
-        } else {
-            GPL_TRY(bm.get(ctx, (size_t)(n + 7) / 8));
-            GPL_TRY(pack_bits(ctx, vb.p, bm.p, n));
-            GPL_TRY(deliver(ctx, out_validity, bm.p, (size_t)(n + 7) / 8, GPL_HOST));
-        }
-    }
-    return deliver(ctx, out, dst, sizeof(double) * n, mem);
+    const int grid = warp_grid(n, 4);
+    if (method == 0) GPL_LAUNCH(ctx, k_geodesic_length<0>, grid, 128, 0, in->type, n, xy, in->geom_off, in->part_off, in->ring_off, in->validity, res.p, valid.p);
+    else if (method == 1) GPL_LAUNCH(ctx, k_geodesic_length<1>, grid, 128, 0, in->type, n, xy, in->geom_off, in->part_off, in->ring_off, in->validity, res.p, valid.p);
+    else GPL_LAUNCH(ctx, k_geodesic_length<2>, grid, 128, 0, in->type, n, xy, in->geom_off, in->part_off, in->ring_off, in->validity, res.p, valid.p);
+    GPL_TRY(valid.deliver(ctx));
+    return res.deliver(ctx);
 }

@@ -15,6 +15,7 @@
 
 #include "common.cuh"
 #include "geodesic.cuh"
+#include "output.cuh"
 
 namespace gpl {
 
@@ -227,9 +228,6 @@ __global__ void k_row_starts(int type, int64_t n, const int64_t *__restrict__ ge
     }
 }
 
-int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n);
-int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
-
 /* Polygon / MultiPolygon rows: the edge pass and the row pass over row chunks of at most kMaxEdgesPerPass edges (one chunk
  * unless the column is larger; a single row with more edges is a chunk of its own) */
 static int geodesic_area_polygons(gpl_ctx *ctx, const gpl_array *in, int sign, double *area, double *perim, uint8_t *vb) {
@@ -291,43 +289,24 @@ extern "C" int gpl_geodesic_area(gpl_ctx *ctx, const gpl_array *in, int sign, do
     GPL_REQUIRE(ctx && in, GPL_ERR_INVALID_ARG, "gpl_geodesic_area: NULL argument");
     GPL_REQUIRE(area || perimeter, GPL_ERR_INVALID_ARG, "gpl_geodesic_area: area and perimeter are both NULL");
     GPL_REQUIRE(sign == 0 || sign == 1, GPL_ERR_INVALID_ARG, "gpl_geodesic_area: sign must be 0 (unsigned) or 1 (signed), got %d", sign);
-    GPL_REQUIRE(mem == GPL_HOST || mem == GPL_DEVICE, GPL_ERR_INVALID_ARG, "gpl_geodesic_area: mem must be GPL_HOST or GPL_DEVICE");
-    GPL_REQUIRE(in->type >= GPL_POINT && in->type <= GPL_MULTIPOLYGON && in->type != GPL_LINEARRING, GPL_ERR_INVALID_TYPE,
+    GPL_TRY(check_mem(mem, "gpl_geodesic_area"));
+    GPL_REQUIRE(known_type(in->type), GPL_ERR_INVALID_TYPE,
                 "gpl_geodesic_area: unsupported geometry type %s", type_name(in->type));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = in->n_geoms;
     if (n == 0) return GPL_OK;
-    Scratch<double> ta, tp;
-    Scratch<uint8_t> vb;
-    double *da = area, *dp = perimeter;
-    if (mem == GPL_HOST) {
-        if (area) {
-            GPL_TRY(ta.get(ctx, (size_t)n));
-            da = ta.p;
-        }
-        if (perimeter) {
-            GPL_TRY(tp.get(ctx, (size_t)n));
-            dp = tp.p;
-        }
-    }
-    GPL_TRY(vb.get(ctx, (size_t)n));
-    if (in->type == GPL_POLYGON || in->type == GPL_MULTIPOLYGON) {
-        GPL_TRY(geodesic_area_polygons(ctx, in, sign, da, dp, vb.p));
+    RowOut<double> ra, rp;
+    ValidOut valid;
+    GPL_TRY(ra.get(ctx, area, n, mem));
+    GPL_TRY(rp.get(ctx, perimeter, n, mem));
+    GPL_TRY(valid.get(ctx, out_validity, n, mem, true));
+    if (is_area(in->type)) {
+        GPL_TRY(geodesic_area_polygons(ctx, in, sign, ra.p, rp.p, valid.p));
     } else {
         GPL_LAUNCH(ctx, k_geodesic_zero_rows, warp_grid(n, 4), 128, 0, in->type, n, reinterpret_cast<const double2 *>(in->xy), in->geom_off,
-                   in->ring_off, in->validity, da, dp, vb.p);
+                   in->ring_off, in->validity, ra.p, rp.p, valid.p);
     }
-    if (out_validity) {
-        if (mem == GPL_DEVICE) {
-            GPL_TRY(pack_bits(ctx, vb.p, out_validity, n));
-        } else {
-            Scratch<uint8_t> bm;
-            GPL_TRY(bm.get(ctx, (size_t)(n + 7) / 8));
-            GPL_TRY(pack_bits(ctx, vb.p, bm.p, n));
-            GPL_TRY(deliver(ctx, out_validity, bm.p, (size_t)(n + 7) / 8, GPL_HOST));
-        }
-    }
-    if (area) GPL_TRY(deliver(ctx, area, da, sizeof(double) * n, mem));
-    if (perimeter) GPL_TRY(deliver(ctx, perimeter, dp, sizeof(double) * n, mem));
-    return GPL_OK;
+    GPL_TRY(valid.deliver(ctx));
+    GPL_TRY(ra.deliver(ctx));
+    return rp.deliver(ctx);
 }

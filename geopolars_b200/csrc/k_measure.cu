@@ -13,6 +13,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "output.cuh"
 
 namespace gpl {
 
@@ -352,53 +353,16 @@ __global__ void __launch_bounds__(256) k_length(int type, int64_t n_geoms, const
     }
 }
 
-// bytes (one per row) -> Arrow LSB bitmap
-__global__ void k_pack_bits(const uint8_t *__restrict__ bytes, uint8_t *__restrict__ bitmap, int64_t n) {
-    int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;  // output byte
-    int64_t nb = (n + 7) / 8;
-    if (i >= nb) return;
-    uint8_t v = 0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        int64_t j = i * 8 + k;
-        if (j < n && bytes[j]) v |= (uint8_t)(1u << k);
-    }
-    bitmap[i] = v;
-}
-int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n) {
-    if (n == 0) return GPL_OK;
-    int64_t nb = (n + 7) / 8;
-    GPL_LAUNCH(ctx, k_pack_bits, (int)ceil_div(nb, 256), 256, 0, bytes_dev, bitmap_dev, n);
-    return GPL_OK;
-}
-
-static int warp_grid(int64_t n_geoms) {
-    int64_t want = ceil_div(n_geoms, 8);  // 8 warps per 256-thread CTA
-    return (int)std::max<int64_t>(1, std::min<int64_t>(want, kSMs * 8));
-}
-
-// copy a device result to the caller's buffer (host: stream-ordered D2H + sync)
-int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem) {
-    if (bytes == 0) return GPL_OK;
-    if (mem == GPL_HOST) {
-        GPL_CUDA(cudaMemcpyAsync(dst, src_dev, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    } else if (dst != src_dev) {
-        GPL_CUDA(cudaMemcpyAsync(dst, src_dev, bytes, cudaMemcpyDeviceToDevice, ctx->stream));
-    }
-    return GPL_OK;
-}
-
 int centroid_raw(gpl_ctx *ctx, const gpl_array *in, double2 *out_dev, uint8_t *valid_bytes_dev) {
     if (in->n_geoms == 0) return GPL_OK;
-    GPL_LAUNCH(ctx, k_centroid, warp_grid(in->n_geoms), 256, 0, in->type, in->n_geoms,
+    GPL_LAUNCH(ctx, k_centroid, warp_grid(in->n_geoms, 8, 8), 256, 0, in->type, in->n_geoms,
                reinterpret_cast<const double2 *>(in->xy), in->geom_off, in->part_off, in->ring_off, in->validity, out_dev,
                valid_bytes_dev);
     return GPL_OK;
 }
 int envelope_raw(gpl_ctx *ctx, const gpl_array *in, double *out4_dev, uint8_t *valid_bytes_dev) {
     if (in->n_geoms == 0) return GPL_OK;
-    GPL_LAUNCH(ctx, k_envelope, warp_grid(in->n_geoms), 256, 0, in->type, in->n_geoms,
+    GPL_LAUNCH(ctx, k_envelope, warp_grid(in->n_geoms, 8, 8), 256, 0, in->type, in->n_geoms,
                reinterpret_cast<const double2 *>(in->xy), in->geom_off, in->part_off, in->ring_off, in->validity, out4_dev,
                valid_bytes_dev);
     return GPL_OK;
@@ -466,50 +430,42 @@ extern "C" int gpl_envelope_query(gpl_ctx *ctx, const gpl_array *in, double minx
                                   uint8_t *out_bitmap, int mem) {
     GPL_REQUIRE(ctx && in && out_bitmap, GPL_ERR_INVALID_ARG, "gpl_envelope_query: NULL argument");
     GPL_REQUIRE(mode == 0 || mode == 1, GPL_ERR_INVALID_ARG, "gpl_envelope_query: mode must be 0 (contained) or 1 (intersecting)");
+    GPL_TRY(check_mem(mem, "gpl_envelope_query"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = in->n_geoms;
     if (n == 0) return GPL_OK;
     Scratch<double> b4;
-    Scratch<uint8_t> vb, hit, bm;
+    Scratch<uint8_t> vb, hit;
     GPL_TRY(b4.get(ctx, (size_t)n * 4));
     GPL_TRY(vb.get(ctx, (size_t)n));
     GPL_TRY(hit.get(ctx, (size_t)n));
     GPL_TRY(envelope_raw(ctx, in, b4.p, vb.p));
     GPL_LAUNCH(ctx, k_envelope_query, (int)ceil_div(n, 256), 256, 0, b4.p, vb.p, n, minx, miny, maxx, maxy, mode, hit.p);
-    if (mem == GPL_DEVICE) return pack_bits(ctx, hit.p, out_bitmap, n);
-    GPL_TRY(bm.get(ctx, (size_t)(n + 7) / 8));
-    GPL_TRY(pack_bits(ctx, hit.p, bm.p, n));
-    return deliver(ctx, out_bitmap, bm.p, (size_t)(n + 7) / 8, GPL_HOST);
+    return finish_bitmap(ctx, hit.p, n, out_bitmap, mem);
 }
 
 extern "C" int gpl_area(gpl_ctx *ctx, const gpl_array *in, double *out, int mem) {
     GPL_REQUIRE(ctx && in && out, GPL_ERR_INVALID_ARG, "gpl_area: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_area"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     if (in->n_geoms == 0) return GPL_OK;
-    Scratch<double> tmp;
-    double *dst = out;
-    if (mem == GPL_HOST) {
-        GPL_TRY(tmp.get(ctx, (size_t)in->n_geoms));
-        dst = tmp.p;
-    }
-    GPL_LAUNCH(ctx, k_area, warp_grid(in->n_geoms), 256, 0, in->type, in->n_geoms, reinterpret_cast<const double2 *>(in->xy),
-               in->geom_off, in->part_off, in->ring_off, dst);
-    return deliver(ctx, out, dst, sizeof(double) * in->n_geoms, mem);
+    RowOut<double> res;
+    GPL_TRY(res.get(ctx, out, in->n_geoms, mem));
+    GPL_LAUNCH(ctx, k_area, warp_grid(in->n_geoms, 8, 8), 256, 0, in->type, in->n_geoms, reinterpret_cast<const double2 *>(in->xy),
+               in->geom_off, in->part_off, in->ring_off, res.p);
+    return res.deliver(ctx);
 }
 
 extern "C" int gpl_euclidean_length(gpl_ctx *ctx, const gpl_array *in, double *out, int mem) {
     GPL_REQUIRE(ctx && in && out, GPL_ERR_INVALID_ARG, "gpl_euclidean_length: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_euclidean_length"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     if (in->n_geoms == 0) return GPL_OK;
-    Scratch<double> tmp;
-    double *dst = out;
-    if (mem == GPL_HOST) {
-        GPL_TRY(tmp.get(ctx, (size_t)in->n_geoms));
-        dst = tmp.p;
-    }
-    GPL_LAUNCH(ctx, k_length, warp_grid(in->n_geoms), 256, 0, in->type, in->n_geoms,
-               reinterpret_cast<const double2 *>(in->xy), in->geom_off, in->part_off, in->ring_off, dst);
-    return deliver(ctx, out, dst, sizeof(double) * in->n_geoms, mem);
+    RowOut<double> res;
+    GPL_TRY(res.get(ctx, out, in->n_geoms, mem));
+    GPL_LAUNCH(ctx, k_length, warp_grid(in->n_geoms, 8, 8), 256, 0, in->type, in->n_geoms,
+               reinterpret_cast<const double2 *>(in->xy), in->geom_off, in->part_off, in->ring_off, res.p);
+    return res.deliver(ctx);
 }
 
 extern "C" int gpl_centroid(gpl_ctx *ctx, const gpl_array *in, gpl_array **out) {
@@ -532,6 +488,7 @@ extern "C" int gpl_centroid(gpl_ctx *ctx, const gpl_array *in, gpl_array **out) 
 
 extern "C" int gpl_envelope(gpl_ctx *ctx, const gpl_array *in, gpl_array **out, double *out4, int mem) {
     GPL_REQUIRE(ctx && in && (out || out4), GPL_ERR_INVALID_ARG, "gpl_envelope: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_envelope"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     int64_t n = in->n_geoms;
     Scratch<double> b4;

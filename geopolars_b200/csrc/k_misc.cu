@@ -4,12 +4,10 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "output.cuh"
 #include "scan.cuh"
 
 namespace gpl {
-
-int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n);
-int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
 
 __global__ void k_geom_type(int type, int64_t n, const uint8_t *__restrict__ validity, int8_t *__restrict__ out) {
     int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -95,36 +93,25 @@ __global__ void __launch_bounds__(256) k_exterior_copy(int64_t n, const double2 
     }
 }
 
-static int bool_result(gpl_ctx *ctx, const uint8_t *bytes, int64_t n, uint8_t *out_bitmap, int mem) {
-    size_t nb = (size_t)(n + 7) / 8;
-    if (mem == GPL_DEVICE) return pack_bits(ctx, bytes, out_bitmap, n);
-    Scratch<uint8_t> bm;
-    GPL_TRY(bm.get(ctx, nb));
-    GPL_TRY(pack_bits(ctx, bytes, bm.p, n));
-    return deliver(ctx, out_bitmap, bm.p, nb, GPL_HOST);
-}
-
 }  // namespace gpl
 
 using namespace gpl;
 
 extern "C" int gpl_geom_type(gpl_ctx *ctx, const gpl_array *in, int8_t *out, int mem) {
     GPL_REQUIRE(ctx && in && out, GPL_ERR_INVALID_ARG, "gpl_geom_type: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_geom_type"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     int64_t n = in->n_geoms;
     if (n == 0) return GPL_OK;
-    Scratch<int8_t> tmp;
-    int8_t *dst = out;
-    if (mem == GPL_HOST) {
-        GPL_TRY(tmp.get(ctx, (size_t)n));
-        dst = tmp.p;
-    }
-    GPL_LAUNCH(ctx, k_geom_type, (int)ceil_div(n, 256), 256, 0, in->type, n, in->validity, dst);
-    return deliver(ctx, out, dst, (size_t)n, mem);
+    RowOut<int8_t> res;
+    GPL_TRY(res.get(ctx, out, n, mem));
+    GPL_LAUNCH(ctx, k_geom_type, (int)ceil_div(n, 256), 256, 0, in->type, n, in->validity, res.p);
+    return res.deliver(ctx);
 }
 
 extern "C" int gpl_is_empty(gpl_ctx *ctx, const gpl_array *in, uint8_t *out_bitmap, int mem) {
     GPL_REQUIRE(ctx && in && out_bitmap, GPL_ERR_INVALID_ARG, "gpl_is_empty: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_is_empty"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     int64_t n = in->n_geoms;
     if (n == 0) return GPL_OK;
@@ -132,11 +119,12 @@ extern "C" int gpl_is_empty(gpl_ctx *ctx, const gpl_array *in, uint8_t *out_bitm
     GPL_TRY(bytes.get(ctx, (size_t)n));
     GPL_LAUNCH(ctx, k_is_empty, (int)ceil_div(n, 256), 256, 0, in->type, n, reinterpret_cast<const double2 *>(in->xy), in->geom_off,
                in->part_off, in->ring_off, bytes.p);
-    return bool_result(ctx, bytes.p, n, out_bitmap, mem);
+    return finish_bitmap(ctx, bytes.p, n, out_bitmap, mem);
 }
 
 extern "C" int gpl_is_ring(gpl_ctx *ctx, const gpl_array *in, uint8_t *out_bitmap, int mem) {
     GPL_REQUIRE(ctx && in && out_bitmap, GPL_ERR_INVALID_ARG, "gpl_is_ring: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_is_ring"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     int64_t n = in->n_geoms;
     if (n == 0) return GPL_OK;
@@ -144,23 +132,20 @@ extern "C" int gpl_is_ring(gpl_ctx *ctx, const gpl_array *in, uint8_t *out_bitma
     GPL_TRY(bytes.get(ctx, (size_t)n));
     GPL_LAUNCH(ctx, k_is_ring, (int)ceil_div(n, 256), 256, 0, in->type, n, reinterpret_cast<const double2 *>(in->xy), in->geom_off,
                bytes.p);
-    return bool_result(ctx, bytes.p, n, out_bitmap, mem);
+    return finish_bitmap(ctx, bytes.p, n, out_bitmap, mem);
 }
 
 static int component(gpl_ctx *ctx, const gpl_array *in, int comp, double *out, int mem) {
     GPL_REQUIRE(ctx && in && out, GPL_ERR_INVALID_ARG, "gpl_x/gpl_y: NULL argument");
     GPL_REQUIRE(in->type == GPL_POINT, GPL_ERR_INVALID_TYPE, "Expected Point (found geometry type %d)", in->type);
+    GPL_TRY(check_mem(mem, "gpl_x/gpl_y"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     int64_t n = in->n_geoms;
     if (n == 0) return GPL_OK;
-    Scratch<double> tmp;
-    double *dst = out;
-    if (mem == GPL_HOST) {
-        GPL_TRY(tmp.get(ctx, (size_t)n));
-        dst = tmp.p;
-    }
-    GPL_LAUNCH(ctx, k_component, (int)ceil_div(n, 256), 256, 0, reinterpret_cast<const double2 *>(in->xy), n, comp, dst);
-    return deliver(ctx, out, dst, sizeof(double) * n, mem);
+    RowOut<double> res;
+    GPL_TRY(res.get(ctx, out, n, mem));
+    GPL_LAUNCH(ctx, k_component, (int)ceil_div(n, 256), 256, 0, reinterpret_cast<const double2 *>(in->xy), n, comp, res.p);
+    return res.deliver(ctx);
 }
 extern "C" int gpl_x(gpl_ctx *ctx, const gpl_array *in, double *out, int mem) { return component(ctx, in, 0, out, mem); }
 extern "C" int gpl_y(gpl_ctx *ctx, const gpl_array *in, double *out, int mem) { return component(ctx, in, 1, out, mem); }
@@ -182,8 +167,7 @@ extern "C" int gpl_exterior(gpl_ctx *ctx, const gpl_array *in, gpl_array **out) 
     Scratch<double> xy;
     GPL_TRY(xy.get(ctx, (size_t)h_total * 2));
     if (n > 0 && h_total > 0) {
-        int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 8), (int64_t)kSMs * 8));
-        GPL_LAUNCH(ctx, k_exterior_copy, grid, 256, 0, n, reinterpret_cast<const double2 *>(in->xy), in->geom_off, in->ring_off, off.p,
+        GPL_LAUNCH(ctx, k_exterior_copy, warp_grid(n, 8, 8), 256, 0, n, reinterpret_cast<const double2 *>(in->xy), in->geom_off, in->ring_off, off.p,
                    reinterpret_cast<double2 *>(xy.p));
     }
     gpl_array *o = array_new(ctx, GPL_LINESTRING);

@@ -34,6 +34,7 @@
 #include "common.cuh"
 #include "join_grid.cuh"
 #include "join_host.cuh"
+#include "output.cuh"
 #include "pair_dist.cuh"
 #include "point_dist.cuh"
 #include "scan.cuh"
@@ -432,9 +433,6 @@ __global__ void __launch_bounds__(256) k_nearest_overflow(NearestView v, const d
         atomicAdd(ctr + 1, points);
     }
 }
-
-int envelope_raw(gpl_ctx *ctx, const gpl_array *in, double *out4_dev, uint8_t *valid_bytes_dev);
-int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
 
 static int nn_grid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, kNnWarps * 32), (int64_t)kSMs * 8)); }
 
@@ -1086,6 +1084,7 @@ extern "C" int gpl_nearest_index_stats(gpl_ctx *ctx, const gpl_nearest_index *id
 extern "C" int gpl_nearest_join(gpl_ctx *ctx, const gpl_nearest_index *idx, const double *points_xy, int64_t n_points, double max_distance,
                                 int32_t *nearest_id, double *distance, int32_t *n_tied, int mem) {
     GPL_REQUIRE(ctx && idx && nearest_id && (points_xy || n_points <= 0), GPL_ERR_INVALID_ARG, "gpl_nearest_join: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_nearest_join"));
     GPL_REQUIRE(n_points >= 0, GPL_ERR_INVALID_ARG, "gpl_nearest_join: negative point count");
     GPL_TRY(check_query(n_points, max_distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
@@ -1104,6 +1103,7 @@ extern "C" int gpl_nearest_join(gpl_ctx *ctx, const gpl_nearest_index *idx, cons
 extern "C" int gpl_nearest_join_array(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *points, double max_distance,
                                       int32_t *nearest_id, double *distance, int32_t *n_tied, int mem) {
     GPL_REQUIRE(ctx && idx && points && nearest_id, GPL_ERR_INVALID_ARG, "gpl_nearest_join_array: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_nearest_join_array"));
     GPL_REQUIRE(points->type == GPL_POINT, GPL_ERR_INVALID_TYPE, "nearest join: the left side must be Point (found %s)",
                 type_name(points->type));
     GPL_TRY(check_query(points->n_geoms, max_distance));
@@ -1118,6 +1118,7 @@ extern "C" int gpl_nearest_join_pairs_array(gpl_ctx *ctx, const gpl_nearest_inde
                                             gpl_pairs **out, double *distance, int mem) {
     GPL_REQUIRE(ctx && idx && points && out, GPL_ERR_INVALID_ARG, "gpl_nearest_join_pairs_array: NULL argument");
     *out = nullptr;
+    GPL_TRY(check_mem(mem, "gpl_nearest_join_pairs_array"));
     GPL_REQUIRE(points->type == GPL_POINT, GPL_ERR_INVALID_TYPE, "nearest join: the left side must be Point (found %s)",
                 type_name(points->type));
     GPL_TRY(check_query(points->n_geoms, max_distance));
@@ -1143,6 +1144,7 @@ extern "C" int gpl_nearest_join_pairs_array(gpl_ctx *ctx, const gpl_nearest_inde
 extern "C" int gpl_nearest_join_geom(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double max_distance,
                                      int32_t *nearest_id, double *distance, int32_t *n_tied, int mem) {
     GPL_REQUIRE(ctx && idx && lhs && nearest_id, GPL_ERR_INVALID_ARG, "gpl_nearest_join_geom: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_nearest_join_geom"));
     GPL_TRY(check_geom_left(lhs, max_distance));
     if (lhs->type == GPL_POINT) return gpl_nearest_join_array(ctx, idx, lhs, max_distance, nearest_id, distance, n_tied, mem);
     GPL_CUDA(cudaSetDevice(ctx->device));
@@ -1157,6 +1159,7 @@ extern "C" int gpl_nearest_join_geom_pairs(gpl_ctx *ctx, const gpl_nearest_index
                                            gpl_pairs **out, double *distance, int mem) {
     GPL_REQUIRE(ctx && idx && lhs && out, GPL_ERR_INVALID_ARG, "gpl_nearest_join_geom_pairs: NULL argument");
     *out = nullptr;
+    GPL_TRY(check_mem(mem, "gpl_nearest_join_geom_pairs"));
     GPL_TRY(check_geom_left(lhs, max_distance));
     if (lhs->type == GPL_POINT) return gpl_nearest_join_pairs_array(ctx, idx, lhs, max_distance, out, distance, mem);
     GPL_CUDA(cudaSetDevice(ctx->device));
@@ -1180,20 +1183,16 @@ extern "C" int gpl_nearest_join_geom_pairs(gpl_ctx *ctx, const gpl_nearest_index
 
 extern "C" int gpl_dwithin_count(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int32_t *count, int mem) {
     GPL_REQUIRE(ctx && idx && lhs && (count || lhs->n_geoms == 0), GPL_ERR_INVALID_ARG, "gpl_dwithin_count: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_dwithin_count"));
     GPL_TRY(check_dwithin(lhs, distance));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = lhs->n_geoms;
     RowClasses lc;
-    Scratch<int32_t> dc;
     if (n && lhs->type != GPL_POINT) GPL_TRY(classify_rows(ctx, lhs, lc));
-    int32_t *out = count;
-    if (mem != GPL_DEVICE) {
-        GPL_TRY(dc.get(ctx, (size_t)n));
-        out = dc.p;
-    }
-    GPL_TRY(dwithin_run(ctx, idx, lhs, lc.cls.p, lc.box4.p, distance, out, nullptr, nullptr, nullptr));
-    if (mem != GPL_DEVICE) GPL_TRY(deliver(ctx, count, dc.p, sizeof(int32_t) * (size_t)n, mem));
-    return GPL_OK;
+    RowOut<int32_t> res;
+    GPL_TRY(res.get(ctx, count, n, mem));
+    GPL_TRY(dwithin_run(ctx, idx, lhs, lc.cls.p, lc.box4.p, distance, res.p, nullptr, nullptr, nullptr));
+    return res.deliver(ctx);
 }
 
 extern "C" int gpl_dwithin_join_pairs(gpl_ctx *ctx, const gpl_nearest_index *idx, const gpl_array *lhs, double distance, int with_distance,

@@ -22,6 +22,7 @@
 
 #include "common.cuh"
 #include "join_grid.cuh"
+#include "output.cuh"
 #include "overlay.cuh"
 #include "pair_dist.cuh"
 
@@ -235,32 +236,24 @@ using namespace gpl;
 
 extern "C" int gpl_intersection_area(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, double *out, uint8_t *out_validity, int mem) {
     GPL_REQUIRE(ctx && a && b && out, GPL_ERR_INVALID_ARG, "gpl_intersection_area: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_intersection_area"));
     GPL_REQUIRE(is_area(a->type) && is_area(b->type), GPL_ERR_INVALID_TYPE, "Expected (Multi)Polygon x (Multi)Polygon (found %s x %s)",
                 type_name(a->type), type_name(b->type));
-    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "intersection_area: lengths differ (%lld vs %lld)",
-                (long long)a->n_geoms, (long long)b->n_geoms);
+    GPL_TRY(require_same_length(a, b, "intersection_area"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = a->n_geoms;
     if (n == 0) return GPL_OK;
     RingPrep pa, pb;
     GPL_TRY(ring_prep(ctx, a, pa));
     GPL_TRY(ring_prep(ctx, b, pb));
-    Scratch<double> tmp;
-    Scratch<uint8_t> vbytes;
-    double *dst = out;
-    if (mem == GPL_HOST) {
-        GPL_TRY(tmp.get(ctx, (size_t)n));
-        dst = tmp.p;
-    }
-    uint8_t *vb = nullptr;
-    if (out_validity) {
-        GPL_TRY(vbytes.get(ctx, (size_t)n));
-        vb = vbytes.p;
-    }
+    RowOut<double> res;
+    ValidOut valid;
+    GPL_TRY(res.get(ctx, out, n, mem));
+    GPL_TRY(valid.get(ctx, out_validity, n, mem, false));
     GPL_LAUNCH(ctx, k_overlap_area, warp_grid(n, kOverlapThreads / 32), kOverlapThreads, 0, n, pa.view, pa.members, a->validity, pa.sigma.p, pa.box.p, pb.view, pb.members,
-               b->validity, pb.sigma.p, pb.box.p, nullptr, nullptr, dst, vb);
-    if (out_validity) GPL_TRY(finish_bitmap(ctx, vb, n, out_validity, mem));
-    return deliver(ctx, out, dst, sizeof(double) * n, mem);
+               b->validity, pb.sigma.p, pb.box.p, nullptr, nullptr, res.p, valid.p);
+    GPL_TRY(valid.deliver(ctx));
+    return res.deliver(ctx);
 }
 
 extern "C" int gpl_overlay_area_join(gpl_ctx *ctx, const gpl_array *lhs, const gpl_array *rhs, gpl_pairs **out) {

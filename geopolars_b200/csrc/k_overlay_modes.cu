@@ -10,6 +10,7 @@
 #include "boolean.cuh"
 #include "common.cuh"
 #include "join_host.cuh"
+#include "output.cuh"
 #include "overlay.cuh"
 #include "pair_dist.cuh"
 #include "scan.cuh"
@@ -68,44 +69,16 @@ int gather_polygons(gpl_ctx *ctx, const gpl_array *const srcs[3], const int8_t *
     PolySrcs ps{};
     for (int s = 0; s < 3; ++s)
         if (srcs[s]) ps.s[s] = PolySrc{polygon_view(srcs[s]), srcs[s]->type == GPL_MULTIPOLYGON ? srcs[s]->geom_off : nullptr, srcs[s]->validity};
-    Scratch<int64_t> cm, cr, cc, geom_off, rbase, cbase, part_off, ring_off, tot;
-    Scratch<double> oxy;
-    Scratch<uint8_t> rv, bm;
-    GPL_TRY(cm.get(ctx, (size_t)m));
-    GPL_TRY(cr.get(ctx, (size_t)m));
-    GPL_TRY(cc.get(ctx, (size_t)m));
+    RaggedOut res;
+    Scratch<uint8_t> rv;
+    GPL_TRY(res.init(ctx, m, 3));
     GPL_TRY(rv.get(ctx, (size_t)m));
-    GPL_TRY(geom_off.get(ctx, (size_t)m + 1));
-    GPL_TRY(rbase.get(ctx, (size_t)m + 1));
-    GPL_TRY(cbase.get(ctx, (size_t)m + 1));
-    GPL_TRY(tot.get(ctx, 3));
-    if (m > 0) GPL_LAUNCH(ctx, k_gather_count, flat_grid(m), 256, 0, m, ps, src, row, cm.p, cr.p, cc.p, rv.p);
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cm.p, m, geom_off.p, tot.p)));
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cr.p, m, rbase.p, tot.p + 1)));
-    GPL_TRY((exclusive_scan<int64_t, int64_t>(ctx, cc.p, m, cbase.p, tot.p + 2)));
-    int64_t h_tot[3] = {0, 0, 0};
-    GPL_CUDA(cudaMemcpyAsync(h_tot, tot.p, sizeof(h_tot), cudaMemcpyDeviceToHost, ctx->stream));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));
-    GPL_TRY(part_off.get(ctx, (size_t)h_tot[0] + 1));
-    GPL_TRY(ring_off.get(ctx, (size_t)h_tot[1] + 1));
-    GPL_TRY(oxy.get(ctx, (size_t)h_tot[2] * 2));
+    if (m > 0) GPL_LAUNCH(ctx, k_gather_count, flat_grid(m), 256, 0, m, ps, src, row, res.count[0].p, res.count[1].p, res.count[2].p, rv.p);
+    GPL_TRY(res.scan_and_allocate());
     if (m > 0)
-        GPL_LAUNCH(ctx, k_gather_write, warp_grid(m, 8), 256, 0, m, ps, src, row, geom_off.p, rbase.p, cbase.p, part_off.p, ring_off.p,
-                   reinterpret_cast<double2 *>(oxy.p));
-    GPL_CUDA(cudaMemcpyAsync(part_off.p + h_tot[0], rbase.p + m, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    GPL_CUDA(cudaMemcpyAsync(ring_off.p + h_tot[1], cbase.p + m, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    GPL_TRY(bm.get(ctx, (size_t)(m + 7) / 8));
-    if (m > 0) GPL_TRY(pack_bits(ctx, rv.p, bm.p, m));
-    GPL_CUDA(cudaStreamSynchronize(ctx->stream));  // the scratch above returns to the cache when this scope ends
-    gpl_array *res = array_new(ctx, GPL_MULTIPOLYGON);
-    res->n_geoms = m, res->n_parts = h_tot[0], res->n_rings = h_tot[1], res->n_coords = h_tot[2];
-    res->geom_off = geom_off.take(), res->own_geom = true;
-    res->part_off = part_off.take(), res->own_part = true;
-    res->ring_off = ring_off.take(), res->own_ring = true;
-    res->xy = oxy.take(), res->own_xy = true;
-    res->validity = bm.take(), res->own_valid = true;
-    *out = res;
-    return GPL_OK;
+        GPL_LAUNCH(ctx, k_gather_write, warp_grid(m, 8), 256, 0, m, ps, src, row, res.base[0].p, res.base[1].p, res.base[2].p, res.off[0].p,
+                   res.off[1].p, reinterpret_cast<double2 *>(res.xy.p));
+    return res.finish(rv.p, GPL_MULTIPOLYGON, out);
 }
 
 // a remainder is emitted when it has a member

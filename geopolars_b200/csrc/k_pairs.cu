@@ -30,6 +30,7 @@
 #include "common.cuh"
 #include "join_grid.cuh"
 #include "join_host.cuh"
+#include "output.cuh"
 #include "pair_dist.cuh"
 #include "point_dist.cuh"
 #include "scan.cuh"
@@ -519,7 +520,7 @@ __global__ void k_point_point_dist(int64_t n, const double2 *__restrict__ a, con
 
 static int side_class_host(int t) { return (t == GPL_POINT || t == GPL_MULTIPOINT) ? 0 : (t == GPL_LINESTRING || t == GPL_MULTILINESTRING) ? 1 : 2; }
 
-// finish_bitmap, polygon_view: pair_dist.cuh
+// polygon_view: pair_dist.cuh
 
 }  // namespace gpl
 
@@ -527,11 +528,9 @@ using namespace gpl;
 
 extern "C" int gpl_intersects(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, uint8_t *out_bitmap, int mem) {
     GPL_REQUIRE(ctx && a && b && out_bitmap, GPL_ERR_INVALID_ARG, "gpl_intersects: NULL argument");
-    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "intersects: lengths differ (%lld vs %lld)",
-                (long long)a->n_geoms, (long long)b->n_geoms);
-    GPL_REQUIRE(a->type >= GPL_POINT && a->type <= GPL_MULTIPOLYGON && a->type != GPL_LINEARRING && b->type >= GPL_POINT &&
-                    b->type <= GPL_MULTIPOLYGON && b->type != GPL_LINEARRING,
-                GPL_ERR_INVALID_TYPE, "intersects: unsupported geometry pair %s x %s", type_name(a->type), type_name(b->type));
+    GPL_TRY(check_mem(mem, "gpl_intersects"));
+    GPL_TRY(require_same_length(a, b, "intersects"));
+    GPL_REQUIRE(known_type(a->type) && known_type(b->type), GPL_ERR_INVALID_TYPE, "intersects: unsupported geometry pair %s x %s", type_name(a->type), type_name(b->type));
     GPL_CUDA(cudaSetDevice(ctx->device));
     int64_t n = a->n_geoms;
     if (n == 0) return GPL_OK;
@@ -553,11 +552,10 @@ extern "C" int gpl_intersects(gpl_ctx *ctx, const gpl_array *a, const gpl_array 
 
 extern "C" int gpl_contains(gpl_ctx *ctx, const gpl_array *polygons, const gpl_array *points, uint8_t *out_bitmap, int mem) {
     GPL_REQUIRE(ctx && polygons && points && out_bitmap, GPL_ERR_INVALID_ARG, "gpl_contains: NULL argument");
-    GPL_REQUIRE(polygons->n_geoms == points->n_geoms, GPL_ERR_LENGTH_MISMATCH, "contains: lengths differ (%lld vs %lld)",
-                (long long)polygons->n_geoms, (long long)points->n_geoms);
-    const bool area = polygons->type == GPL_POLYGON || polygons->type == GPL_MULTIPOLYGON;
-    const bool lines = polygons->type == GPL_LINESTRING || polygons->type == GPL_MULTILINESTRING;
-    GPL_REQUIRE((area || lines) && points->type == GPL_POINT, GPL_ERR_INVALID_TYPE,
+    GPL_TRY(check_mem(mem, "gpl_contains"));
+    GPL_TRY(require_same_length(polygons, points, "contains"));
+    const bool lines = is_line(polygons->type);
+    GPL_REQUIRE((is_area(polygons->type) || lines) && points->type == GPL_POINT, GPL_ERR_INVALID_TYPE,
                 "Expected (Multi)Polygon or (Multi)LineString x Point (found %s x %s)", type_name(polygons->type),
                 type_name(points->type));
     GPL_CUDA(cudaSetDevice(ctx->device));
@@ -579,29 +577,17 @@ extern "C" int gpl_contains(gpl_ctx *ctx, const gpl_array *polygons, const gpl_a
 
 extern "C" int gpl_distance(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, double *out, uint8_t *out_validity, int mem) {
     GPL_REQUIRE(ctx && a && b && out, GPL_ERR_INVALID_ARG, "gpl_distance: NULL argument");
-    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "distance: lengths differ (%lld vs %lld)",
-                (long long)a->n_geoms, (long long)b->n_geoms);
+    GPL_TRY(check_mem(mem, "gpl_distance"));
+    GPL_TRY(require_same_length(a, b, "distance"));
     const int ta = a->type, tb = b->type;
-    auto known = [](int t) {
-        return t == GPL_POINT || t == GPL_LINESTRING || t == GPL_POLYGON || t == GPL_MULTIPOINT || t == GPL_MULTILINESTRING || t == GPL_MULTIPOLYGON;
-    };
-    GPL_REQUIRE(known(ta) && known(tb), GPL_ERR_INVALID_TYPE, "distance: unsupported geometry pair %s x %s", type_name(ta), type_name(tb));
-    auto is_multi = [](int t) { return t == GPL_MULTIPOINT || t == GPL_MULTILINESTRING || t == GPL_MULTIPOLYGON; };
+    GPL_REQUIRE(known_type(ta) && known_type(tb), GPL_ERR_INVALID_TYPE, "distance: unsupported geometry pair %s x %s", type_name(ta), type_name(tb));
     GPL_CUDA(cudaSetDevice(ctx->device));
     int64_t n = a->n_geoms;
     if (n == 0) return GPL_OK;
-    Scratch<double> tmp;
-    Scratch<uint8_t> vbytes;
-    double *dst = out;
-    if (mem == GPL_HOST) {
-        GPL_TRY(tmp.get(ctx, (size_t)n));
-        dst = tmp.p;
-    }
-    uint8_t *vb = nullptr;
-    if (out_validity) {
-        GPL_TRY(vbytes.get(ctx, (size_t)n));
-        vb = vbytes.p;
-    }
+    RowOut<double> res;
+    ValidOut valid;
+    GPL_TRY(res.get(ctx, out, n, mem));
+    GPL_TRY(valid.get(ctx, out_validity, n, mem, false));
     const double2 *axy = reinterpret_cast<const double2 *>(a->xy), *bxy = reinterpret_cast<const double2 *>(b->xy);
     if (is_multi(ta) || is_multi(tb)) {  // minimum over the members (geo's impl for iterable geometries)
         auto view = [](const gpl_array *g, const double2 *xy) {
@@ -613,32 +599,32 @@ extern "C" int gpl_distance(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b
             }
         };
         GPL_LAUNCH(ctx, k_distance_multi, warp_grid(n, 8), 256, 0, n, view(a, axy), is_multi(ta) ? a->geom_off : nullptr, a->validity,
-                   view(b, bxy), is_multi(tb) ? b->geom_off : nullptr, b->validity, dst, vb);
+                   view(b, bxy), is_multi(tb) ? b->geom_off : nullptr, b->validity, res.p, valid.p);
     } else if (ta == GPL_LINESTRING && tb == GPL_LINESTRING) {
         Scratch<uint8_t> flag;
         GPL_TRY(flag.get(ctx, (size_t)n));
         GPL_LAUNCH(ctx, k_ls_ls_fast<1>, warp_grid(n, kPairWarps), kPairWarps * 32, 0, n, axy, a->geom_off, a->validity, bxy, b->geom_off,
-                   b->validity, nullptr, dst, vb, flag.p);
+                   b->validity, nullptr, res.p, valid.p, flag.p);
         GPL_LAUNCH(ctx, k_ls_ls_exact<1>, warp_grid(ceil_div(n, 32), kPairWarps), kPairWarps * 32, 0, n, axy, a->geom_off, bxy, b->geom_off,
-                   flag.p, nullptr, dst, vb);
+                   flag.p, nullptr, res.p, valid.p);
     } else if (ta == GPL_POINT && tb == GPL_POINT) {
-        GPL_LAUNCH(ctx, k_point_point_dist, (int)ceil_div(n, 256), 256, 0, n, axy, a->validity, bxy, b->validity, dst, vb);
+        GPL_LAUNCH(ctx, k_point_point_dist, (int)ceil_div(n, 256), 256, 0, n, axy, a->validity, bxy, b->validity, res.p, valid.p);
     } else if (ta == GPL_POINT && tb == GPL_LINESTRING) {
-        GPL_LAUNCH(ctx, k_point_ls_dist, warp_grid(n, 8), 256, 0, n, axy, a->validity, bxy, b->geom_off, b->validity, dst, vb);
+        GPL_LAUNCH(ctx, k_point_ls_dist, warp_grid(n, 8), 256, 0, n, axy, a->validity, bxy, b->geom_off, b->validity, res.p, valid.p);
     } else if (ta == GPL_LINESTRING && tb == GPL_POINT) {
-        GPL_LAUNCH(ctx, k_point_ls_dist, warp_grid(n, 8), 256, 0, n, bxy, b->validity, axy, a->geom_off, a->validity, dst, vb);
+        GPL_LAUNCH(ctx, k_point_ls_dist, warp_grid(n, 8), 256, 0, n, bxy, b->validity, axy, a->geom_off, a->validity, res.p, valid.p);
     } else if (ta == GPL_POINT && tb == GPL_POLYGON) {
         GPL_LAUNCH(ctx, k_poly_point<1>, warp_grid(n, 8), 256, 0, b->type, n, bxy, b->geom_off, b->part_off, b->ring_off, b->validity,
-                   axy, a->validity, nullptr, dst, vb);
+                   axy, a->validity, nullptr, res.p, valid.p);
     } else if (tb != GPL_POINT) {  // LineString x Polygon, Polygon x LineString, Polygon x Polygon
         Side sa{ta, axy, a->geom_off, a->part_off, a->ring_off}, sb{tb, bxy, b->geom_off, b->part_off, b->ring_off};
-        GPL_LAUNCH(ctx, k_distance_generic, warp_grid(n, 8), 256, 0, n, sa, a->validity, sb, b->validity, dst, vb);
+        GPL_LAUNCH(ctx, k_distance_generic, warp_grid(n, 8), 256, 0, n, sa, a->validity, sb, b->validity, res.p, valid.p);
     } else {
         GPL_LAUNCH(ctx, k_poly_point<1>, warp_grid(n, 8), 256, 0, a->type, n, axy, a->geom_off, a->part_off, a->ring_off, a->validity,
-                   bxy, b->validity, nullptr, dst, vb);
+                   bxy, b->validity, nullptr, res.p, valid.p);
     }
-    if (out_validity) GPL_TRY(finish_bitmap(ctx, vb, n, out_validity, mem));
-    return deliver(ctx, out, dst, sizeof(double) * n, mem);
+    GPL_TRY(valid.deliver(ctx));
+    return res.deliver(ctx);
 }
 
 // ================================================================================================================
@@ -657,8 +643,6 @@ extern "C" int gpl_distance(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b
 // general one.
 // JoinGrid, jg_cell and the grid build (join_grid_build): join_grid.cuh; struct gpl_pairs: common.cuh
 namespace gpl {
-
-int envelope_raw(gpl_ctx *ctx, const gpl_array *in, double *out4_dev, uint8_t *valid_bytes_dev);
 
 template <int PASS>
 __global__ void k_join_candidates(const double *__restrict__ l4, const uint8_t *__restrict__ lhas, int64_t nl, const double *__restrict__ r4,
@@ -814,6 +798,7 @@ extern "C" int64_t gpl_pairs_count(const gpl_pairs *p) { return p ? p->n : 0; }
 extern "C" int gpl_pairs_copy_distance(gpl_ctx *ctx, const gpl_pairs *p, double *distance, int mem) {
     GPL_REQUIRE(ctx && p && (p->n == 0 || distance), GPL_ERR_INVALID_ARG, "gpl_pairs_copy_distance: NULL argument");
     GPL_REQUIRE(p->with_dist, GPL_ERR_INVALID_ARG, "gpl_pairs_copy_distance: this pair list carries no distances");
+    GPL_TRY(check_mem(mem, "gpl_pairs_copy_distance"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     if (p->n == 0) return GPL_OK;
     const cudaMemcpyKind kind = mem == GPL_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
@@ -823,6 +808,7 @@ extern "C" int gpl_pairs_copy_distance(gpl_ctx *ctx, const gpl_pairs *p, double 
 }
 extern "C" int gpl_pairs_copy(gpl_ctx *ctx, const gpl_pairs *p, uint64_t *lhs, uint64_t *rhs, int mem) {
     GPL_REQUIRE(ctx && p && (p->n == 0 || (lhs && rhs)), GPL_ERR_INVALID_ARG, "gpl_pairs_copy: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_pairs_copy"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     if (p->n == 0) return GPL_OK;
     const cudaMemcpyKind kind = mem == GPL_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
@@ -835,8 +821,8 @@ extern "C" int gpl_pairs_copy(gpl_ctx *ctx, const gpl_pairs *p, uint64_t *lhs, u
 // row-wise (Multi)Polygon.contains(Polygon)
 extern "C" int gpl_contains_polygon(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, uint8_t *out_bitmap, int mem) {
     GPL_REQUIRE(ctx && a && b && out_bitmap, GPL_ERR_INVALID_ARG, "gpl_contains_polygon: NULL argument");
-    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "contains: lengths differ (%lld vs %lld)", (long long)a->n_geoms,
-                (long long)b->n_geoms);
+    GPL_TRY(check_mem(mem, "gpl_contains_polygon"));
+    GPL_TRY(require_same_length(a, b, "contains"));
     GPL_REQUIRE((a->type == GPL_POLYGON || a->type == GPL_MULTIPOLYGON) && b->type == GPL_POLYGON, GPL_ERR_INVALID_TYPE,
                 "Expected (Multi)Polygon x Polygon (found %s x %s)", type_name(a->type), type_name(b->type));
     GPL_CUDA(cudaSetDevice(ctx->device));

@@ -48,6 +48,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "output.cuh"
 #include "scan.cuh"
 
 namespace cg = cooperative_groups;
@@ -2415,6 +2416,7 @@ extern "C" int gpl_pip_index_build(gpl_ctx *ctx, const gpl_array *polys, gpl_pip
 extern "C" int gpl_contains_join(gpl_ctx *ctx, const gpl_pip_index *idx, const double *points_xy, int64_t n_points,
                                  int32_t *first_id, int32_t *count, int mem) {
     GPL_REQUIRE(ctx && idx && first_id && (points_xy || n_points == 0), GPL_ERR_INVALID_ARG, "gpl_contains_join: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_contains_join"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     if (n_points == 0) return GPL_OK;
     if (mem == GPL_DEVICE) return pip_query(ctx, idx, points_xy, nullptr, n_points, first_id, count, ctx->stream);
@@ -2436,6 +2438,7 @@ extern "C" int gpl_contains_join_counts(gpl_ctx *ctx, const gpl_pip_index *idx, 
                                         int32_t *first_id, uint64_t *counts, int mem) {
     GPL_REQUIRE(ctx && idx && first_id && counts && (points_xy || n_points == 0), GPL_ERR_INVALID_ARG,
                 "gpl_contains_join_counts: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_contains_join_counts"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     if (n_points == 0) return GPL_OK;
     if (mem == GPL_DEVICE)
@@ -2459,6 +2462,7 @@ extern "C" int gpl_contains_join_counts(gpl_ctx *ctx, const gpl_pip_index *idx, 
 extern "C" int gpl_contains_join_array(gpl_ctx *ctx, const gpl_pip_index *idx, const gpl_array *points, int32_t *first_id,
                                        int32_t *count, int mem) {
     GPL_REQUIRE(ctx && idx && points && first_id, GPL_ERR_INVALID_ARG, "gpl_contains_join_array: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_contains_join_array"));
     GPL_REQUIRE(points->type == GPL_POINT, GPL_ERR_INVALID_TYPE, "Expected Point (found geometry type %d)", points->type);
     GPL_CUDA(cudaSetDevice(ctx->device));
     int64_t n = points->n_geoms;
@@ -2502,6 +2506,7 @@ static int pip_pairs(gpl_ctx *ctx, const gpl_pip_index *idx, const double *pts, 
 extern "C" int gpl_contains_join_pairs(gpl_ctx *ctx, const gpl_pip_index *idx, const double *points_xy, int64_t n_points,
                                        uint64_t *lhs, uint64_t *rhs, int64_t *n_pairs, int mem) {
     GPL_REQUIRE(ctx && idx && n_pairs, GPL_ERR_INVALID_ARG, "gpl_contains_join_pairs: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_contains_join_pairs"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     if (n_points == 0) {
         *n_pairs = 0;
@@ -2628,6 +2633,7 @@ extern "C" int gpl_contains_join_host(gpl_ctx *ctx, const gpl_pip_index *idx, co
 extern "C" int gpl_join_histogram(gpl_ctx *ctx, const int32_t *first_id, int64_t n_points, uint64_t *counts, int64_t n_polygons,
                                   int mem) {
     GPL_REQUIRE(ctx && counts && (first_id || n_points == 0), GPL_ERR_INVALID_ARG, "gpl_join_histogram: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_join_histogram"));
     GPL_REQUIRE(mem == GPL_DEVICE, GPL_ERR_UNSUPPORTED, "gpl_join_histogram: device buffers only");
     GPL_CUDA(cudaSetDevice(ctx->device));
     if (n_points == 0) return GPL_OK;

@@ -21,6 +21,7 @@
 #include "common.cuh"
 #include "join_grid.cuh"
 #include "join_host.cuh"
+#include "output.cuh"
 #include "overlay.cuh"
 #include "pair_dist.cuh"
 #include "scan.cuh"
@@ -382,13 +383,10 @@ __global__ void __launch_bounds__(kRelateThreads, 3) k_relate(int64_t n, ROp a, 
 static int cls_of(int t) {
     return (t == GPL_POINT || t == GPL_MULTIPOINT) ? 0 : (t == GPL_LINESTRING || t == GPL_MULTILINESTRING) ? 1 : 2;
 }
-static bool known_type(int t) {
-    return t == GPL_POINT || t == GPL_LINESTRING || t == GPL_POLYGON || t == GPL_MULTIPOINT || t == GPL_MULTILINESTRING || t == GPL_MULTIPOLYGON;
-}
 // the column as an ROp; a (Multi)Polygon column gets its ring σ / boxes in prep
 static int make_op(gpl_ctx *ctx, const gpl_array *g, RingPrep &prep, ROp &o) {
     const double2 *xy = reinterpret_cast<const double2 *>(g->xy);
-    const bool multi = g->type == GPL_MULTIPOINT || g->type == GPL_MULTILINESTRING || g->type == GPL_MULTIPOLYGON;
+    const bool multi = is_multi(g->type);
     o = ROp{cls_of(g->type), xy, multi ? g->geom_off : nullptr, nullptr, nullptr, nullptr, nullptr, g->validity};
     if (o.cls == 1) o.ro = g->type == GPL_LINESTRING ? g->geom_off : g->ring_off;
     if (o.cls == 2) {
@@ -466,8 +464,8 @@ using namespace gpl;
 
 extern "C" int gpl_relate(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, int8_t *matrix, uint8_t *out_validity, int mem) {
     GPL_REQUIRE(ctx && a && b && matrix, GPL_ERR_INVALID_ARG, "gpl_relate: NULL argument");
-    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "relate: lengths differ (%lld vs %lld)", (long long)a->n_geoms,
-                (long long)b->n_geoms);
+    GPL_TRY(check_mem(mem, "gpl_relate"));
+    GPL_TRY(require_same_length(a, b, "relate"));
     GPL_TRY(check_pair(a, b, "relate"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = a->n_geoms;
@@ -478,20 +476,20 @@ extern "C" int gpl_relate(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, 
     GPL_TRY(make_op(ctx, b, pb, ob));
     RelSpec full;
     memset(&full, 0, sizeof(full));
-    Scratch<int8_t> mat;
-    Scratch<uint8_t> ok;
-    GPL_TRY(mat.get(ctx, (size_t)n * 9));
-    GPL_TRY(ok.get(ctx, (size_t)n));
-    GPL_LAUNCH(ctx, k_relate, warp_grid(n, kRelateThreads / 32), kRelateThreads, 0, n, oa, ob, nullptr, nullptr, full, mat.p, ok.p, nullptr);
-    if (out_validity) GPL_TRY(finish_bitmap(ctx, ok.p, n, out_validity, mem));
-    return deliver(ctx, matrix, mat.p, (size_t)n * 9, mem);
+    RowOut<int8_t> mat;
+    ValidOut valid;
+    GPL_TRY(mat.get(ctx, matrix, n * 9, mem));
+    GPL_TRY(valid.get(ctx, out_validity, n, mem, true));
+    GPL_LAUNCH(ctx, k_relate, warp_grid(n, kRelateThreads / 32), kRelateThreads, 0, n, oa, ob, nullptr, nullptr, full, mat.p, valid.p, nullptr);
+    GPL_TRY(valid.deliver(ctx));
+    return mat.deliver(ctx);
 }
 
 extern "C" int gpl_relate_predicate(gpl_ctx *ctx, const gpl_array *a, const gpl_array *b, int predicate, const char *pattern, uint8_t *out_bitmap,
                                     int mem) {
     GPL_REQUIRE(ctx && a && b && out_bitmap, GPL_ERR_INVALID_ARG, "gpl_relate_predicate: NULL argument");
-    GPL_REQUIRE(a->n_geoms == b->n_geoms, GPL_ERR_LENGTH_MISMATCH, "relate_predicate: lengths differ (%lld vs %lld)", (long long)a->n_geoms,
-                (long long)b->n_geoms);
+    GPL_TRY(check_mem(mem, "gpl_relate_predicate"));
+    GPL_TRY(require_same_length(a, b, "relate_predicate"));
     GPL_TRY(check_pair(a, b, "relate_predicate"));
     RelSpec spec;
     GPL_REQUIRE(make_spec(predicate, pattern, cls_of(a->type), cls_of(b->type), spec), GPL_ERR_INVALID_ARG,

@@ -24,6 +24,7 @@
 
 #include "common.cuh"
 #include "join_grid.cuh"
+#include "output.cuh"
 #include "pair_dist.cuh"
 #include "scan.cuh"
 #include "sym_point.cuh"
@@ -558,27 +559,25 @@ using namespace gpl;
 
 extern "C" int gpl_is_valid(gpl_ctx *ctx, const gpl_array *in, int8_t *reason, uint8_t *out_validity, int mem) {
     GPL_REQUIRE(ctx && in && reason, GPL_ERR_INVALID_ARG, "gpl_is_valid: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_is_valid"));
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = in->n_geoms;
     if (n == 0) return GPL_OK;
-    Scratch<int8_t> code, tmp;
-    Scratch<uint8_t> live;
+    Scratch<int8_t> code;
     Scratch<uint32_t> flags;
+    ValidOut live;
     GPL_TRY(code.get(ctx, (size_t)n));
-    GPL_TRY(live.get(ctx, (size_t)n));
+    GPL_TRY(live.get(ctx, out_validity, n, mem, true));
     GPL_LAUNCH(ctx, k_valid_rows, warp_grid(n, 8), 256, 0, in->type, n, reinterpret_cast<const double2 *>(in->xy), in->geom_off, in->part_off,
                in->ring_off, in->validity, code.p, live.p);
-    if (in->type == GPL_POLYGON || in->type == GPL_MULTIPOLYGON) {
+    if (is_area(in->type)) {
         GPL_TRY(flags.get(ctx, (size_t)n));
         GPL_CUDA(cudaMemsetAsync(flags.p, 0, sizeof(uint32_t) * (size_t)n, ctx->stream));
         GPL_TRY(polygon_rules(ctx, in, code.p, live.p, flags.p));
     }
-    int8_t *dst = reason;
-    if (mem == GPL_HOST) {
-        GPL_TRY(tmp.get(ctx, (size_t)n));
-        dst = tmp.p;
-    }
-    GPL_LAUNCH(ctx, k_valid_finish, (int)ceil_div(n, 256), 256, 0, n, code.p, flags.p, dst);
-    if (out_validity) GPL_TRY(finish_bitmap(ctx, live.p, n, out_validity, mem));
-    return deliver(ctx, reason, dst, (size_t)n, mem);
+    RowOut<int8_t> res;
+    GPL_TRY(res.get(ctx, reason, n, mem));
+    GPL_LAUNCH(ctx, k_valid_finish, (int)ceil_div(n, 256), 256, 0, n, code.p, flags.p, res.p);
+    GPL_TRY(live.deliver(ctx));
+    return res.deliver(ctx);
 }

@@ -22,6 +22,7 @@
 #include <limits.h>
 
 #include "common.cuh"
+#include "output.cuh"
 #include "scan.cuh"
 
 namespace gpl {
@@ -400,9 +401,6 @@ __global__ void k_valid_bytes_from_bitmap(int64_t n, const uint8_t *__restrict__
     if (i < n) bytes[i] = bit_get(bm, i) ? 1 : 0;
 }
 
-int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n);
-int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
-
 static int stream_grid(int64_t rows, bool warp) {
     const int64_t want = warp ? ceil_div(rows, 8) : ceil_div(rows, 256);
     return (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)kSMs * 16));
@@ -499,8 +497,8 @@ using namespace gpl;
 extern "C" int gpl_wkb_decode(gpl_ctx *ctx, const uint8_t *bytes, const void *offsets, int offset_width, const uint8_t *validity,
                               int64_t n, int mem, gpl_array **out) {
     GPL_REQUIRE(ctx && out && n >= 0 && (n == 0 || (bytes && offsets)), GPL_ERR_INVALID_ARG, "gpl_wkb_decode: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_wkb_decode"));
     GPL_REQUIRE(offset_width == 32 || offset_width == 64, GPL_ERR_INVALID_ARG, "gpl_wkb_decode: offset_width must be 32 or 64");
-    GPL_REQUIRE(mem == GPL_HOST || mem == GPL_DEVICE, GPL_ERR_INVALID_ARG, "gpl_wkb_decode: bad memory kind");
     GPL_CUDA(cudaSetDevice(ctx->device));
     const size_t ow = (size_t)offset_width / 8;
     // first / last offset: the payload range (a sliced Arrow array need not start at 0)
@@ -548,8 +546,9 @@ extern "C" int gpl_wkb_decode(gpl_ctx *ctx, const uint8_t *bytes, const void *of
 extern "C" int gpl_wkb_encode(gpl_ctx *ctx, const gpl_array *a, void *offsets, int offset_width, uint8_t *bytes, int64_t *n_bytes,
                               int mem) {
     GPL_REQUIRE(ctx && a && offsets && n_bytes, GPL_ERR_INVALID_ARG, "gpl_wkb_encode: NULL argument");
+    GPL_TRY(check_mem(mem, "gpl_wkb_encode"));
     GPL_REQUIRE(offset_width == 32 || offset_width == 64, GPL_ERR_INVALID_ARG, "gpl_wkb_encode: offset_width must be 32 or 64");
-    GPL_REQUIRE(a->type >= GPL_POINT && a->type <= GPL_MULTIPOLYGON && a->type != GPL_LINEARRING, GPL_ERR_INVALID_TYPE,
+    GPL_REQUIRE(known_type(a->type), GPL_ERR_INVALID_TYPE,
                 "cannot encode geometry type %d as WKB", a->type);
     GPL_CUDA(cudaSetDevice(ctx->device));
     const int64_t n = a->n_geoms;

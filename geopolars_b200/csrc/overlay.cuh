@@ -17,8 +17,6 @@ struct RingPrep {
 };
 int ring_prep(gpl_ctx *ctx, const gpl_array *g, RingPrep &out);
 
-static inline bool is_area(int t) { return t == GPL_POLYGON || t == GPL_MULTIPOLYGON; }
-
 // every coordinate of the rings of members [m0, m1) of the POLYGON view s is finite (warp-uniform)
 __device__ __forceinline__ bool members_finite(const Side &s, int64_t m0, int64_t m1, int lane) {
     bool ok = true;

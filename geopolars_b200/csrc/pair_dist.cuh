@@ -467,20 +467,7 @@ __device__ __forceinline__ double member_distance(const Side &a, int64_t ia, con
     return sqrt(m);
 }
 
-// ---- host helpers of the row-wise binary ops (k_pairs.cu, k_overlay.cu) -------------------------------------------
-int pack_bits(gpl_ctx *ctx, const uint8_t *bytes_dev, uint8_t *bitmap_dev, int64_t n);
-int deliver(gpl_ctx *ctx, void *dst, const void *src_dev, size_t bytes, int mem);
-
-// bool result: bytes on device -> Arrow bitmap in the caller's memory
-static int finish_bitmap(gpl_ctx *ctx, const uint8_t *bytes_dev, int64_t n, uint8_t *out_bitmap, int mem) {
-    size_t nb = (size_t)(n + 7) / 8;
-    if (mem == GPL_DEVICE) return pack_bits(ctx, bytes_dev, out_bitmap, n);
-    Scratch<uint8_t> bm;
-    GPL_TRY(bm.get(ctx, nb));
-    GPL_TRY(pack_bits(ctx, bytes_dev, bm.p, n));
-    return deliver(ctx, out_bitmap, bm.p, nb, GPL_HOST);
-}
-
+// ---- host side ------------------------------------------------------------------------------------------------------
 // POLYGON view of a Polygon or MultiPolygon array: `go` gives the rings of each polygon member (a MultiPolygon row's
 // members are [geom_off[r], geom_off[r + 1]) of this view, a Polygon row is member r)
 static Side polygon_view(const gpl_array *g) {

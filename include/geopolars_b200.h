@@ -20,7 +20,7 @@
  *     gpl_array handles released with gpl_array_free().
  *   - `mem` arguments say where a caller buffer lives: GPL_HOST (copied with cudaMemcpyAsync on the
  *     context stream; pinned memory from gpl_host_alloc() makes that truly asynchronous) or
- *     GPL_DEVICE (used in place).
+ *     GPL_DEVICE (used in place).  Any other value is rejected with GPL_ERR_INVALID_ARG.
  *   - null rows propagate to null outputs (the reference panics on them, util.rs:32): a strict
  *     superset of the reference behaviour.
  *   - all work is enqueued on the context stream; functions that return data to GPL_HOST buffers
